@@ -15,6 +15,12 @@ HRL_ABI_VERSION = 2
 ALGO_ID = {'MC': 0, 'TD': 1, 'UPGO': 2, 'VTRACE': 3}
 LOSS_KEYS = ('p', 'v', 'r', 'ent', 'total', 'dcnt')
 NUM_LOSS = 6
+# learner diagnostics sums, in the order of the HRL_DIAG_* indices of include/hrl_b200.h: the loss pass's first
+# (HRL_NUM_LOSS_DIAG of them), then the optimiser's
+DIAG_KEYS = ('n_pol', 'rho', 'rho_clip', 'logr', 'logr2', 'adv', 'adv2', 'n_val', 'tv', 'tv2', 'ev', 'ev2', 'tr', 'tr2', 'er', 'er2',
+             'gnorm', 'gnorm2', 'gclip', 'steps')
+NUM_LOSS_DIAG = 16
+NUM_DIAG = 20
 
 _f32p = C.POINTER(C.c_float)
 _i64p = C.POINTER(C.c_int64)
@@ -109,12 +115,16 @@ class HrlGatherArgs(C.Structure):
 SYMBOLS = {
     'hrl_loss_workspace_bytes': (C.c_size_t, [C.c_int32] * 5),
     'hrl_loss_fwd_bwd': (C.c_int, [C.POINTER(HrlLossArgs), C.c_void_p]),
+    'hrl_loss_diag_workspace_bytes': (C.c_size_t, [C.c_int32] * 5),
+    'hrl_loss_fwd_bwd_diag': (C.c_int, [C.POINTER(HrlLossArgs), C.c_void_p, C.c_void_p]),
     'hrl_compute_target': (C.c_int, [C.c_int32] * 6 + [C.c_void_p] * 3 + [C.c_float, C.c_float] +
                            [C.c_void_p] * 5 + [C.c_void_p]),
     'hrl_sumsq_num_partials': (C.c_int32, []),
     'hrl_grad_sumsq': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     'hrl_clip_adam_step': (C.c_int, [C.c_void_p] * 4 + [C.c_int64] + [C.c_void_p] * 3 +
                            [C.c_double] * 5 + [C.c_void_p, C.c_void_p]),
+    'hrl_clip_adam_step_diag': (C.c_int, [C.c_void_p] * 4 + [C.c_int64] + [C.c_void_p] * 3 +
+                                [C.c_double] * 5 + [C.c_void_p, C.c_void_p, C.c_void_p]),
     'hrl_peer_allreduce_sumsq': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int64,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'hrl_bn_workspace_floats': (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),

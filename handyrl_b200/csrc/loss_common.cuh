@@ -15,7 +15,15 @@ struct LossParams {
     int scan;             // recurrences as a parallel suffix scan (long windows) instead of a serial loop per column
     int cluster;          // CTAs per window (bulk kernel): 1, or 2 = thread-block cluster splitting the time axis
     long long *trace;  // optional per-phase clock64 stamps of one CTA (HRL_LOSS_TRACE, debugging only)
+    float *diag;       // HRL_NUM_DIAG diagnostics sums (kernels built with DIAG only)
 };
+
+// workspace: [2048-byte header (ticket) | 8 floats per CTA, up to eight CTAs per window | diagnostics: kDiagStride floats per CTA]
+constexpr int kDiagStride = HRL_NUM_LOSS_DIAG;
+__host__ __device__ inline size_t loss_workspace_base_bytes(int B) { return 2048 + 8 * (size_t)(B > 0 ? B : 0) * 8 * sizeof(float); }
+__host__ __device__ inline size_t loss_diag_workspace_bytes(int B) {
+    return loss_workspace_base_bytes(B) + 8 * (size_t)(B > 0 ? B : 0) * kDiagStride * sizeof(float);
+}
 
 // shared-memory carve-up, in floats
 struct SmemLayout {
@@ -292,9 +300,11 @@ __device__ __forceinline__ void baselines(const LossParams &prm, const SmemLayou
 
 // phases 2b/2c: from per-row statistics (logp, rho, ent in smem) and the baselines of phase 2a to per-cell gradient
 // factors and the six loss partial sums of this thread.  Caller must __syncthreads() before (statistics and
-// baselines visible) and after.
+// baselines visible) and after.  DIAG: also the HRL_NUM_LOSS_DIAG diagnostics partial sums of this thread in dpart
+// (separate accumulators: the order of every loss sum is that of the plain kernels).
+template <bool DIAG>
 __device__ __forceinline__ void targets_and_losses(const LossParams &prm, const SmemLayout &L, float *smem, const CtaCtx &c,
-                                                   float part[6]) {
+                                                   float part[6], float *dpart) {
     const HrlLossArgs &a = prm.a;
     const int P = c.P, Pa = c.Pa, Tt = c.Tt;
     const int vt = a.value_target, pt = a.policy_target;
@@ -384,6 +394,10 @@ __device__ __forceinline__ void targets_and_losses(const LossParams &prm, const 
     if (prm.trace && blockIdx.x == gridDim.x / 2 && c.tid == 0) prm.trace[17] = clock64();
     // ---- 2c: targets, advantages, per-cell loss terms and gradient factors, one job per (cell, player)
     float Lp = 0.f, Lv = 0.f, Lr = 0.f, Lent = 0.f, Lreg = 0.f, dcnt = 0.f;
+    if (DIAG) {
+#pragma unroll
+        for (int k = 0; k < HRL_NUM_LOSS_DIAG; k++) dpart[k] = 0.f;
+    }
     for (int i = c.tid; i < c.ncols; i += c.nthr) {
         const int cell = fdiv(i, P, c.shP), p = i - cell * P;
         const int e = (c.nE == 1) ? 0 : fdiv(cell, Tt, c.shTt), t = cell - e * Tt;
@@ -440,6 +454,35 @@ __device__ __forceinline__ void targets_and_losses(const LossParams &prm, const 
         Lent += own * h;
         Lreg += own * (h * (1.0f - smem[L.prog + cell] * (1.0f - a.entropy_regularization_decay)));   // train.py:212
         dcnt += own * tm;
+        if (DIAG && own != 0.0f) {
+            // the log ratio exactly as row_epilogue forms it before the exp and the clip (train.py:231-238)
+            const float em = smem[L.emask + cell], mu = smem[L.prob + row];
+            const float lr = smem[L.logp + row] - logf(fminf(fmaxf(mu, 1e-16f), 1.0f)) * em;
+            if (tm != 0.0f) {
+                dpart[HRL_DIAG_N_POL] += tm;
+                dpart[HRL_DIAG_RHO] += tm * expf(lr);
+                dpart[HRL_DIAG_RHO_CLIP] += lr > 0.0f ? tm : 0.0f;
+                dpart[HRL_DIAG_LOGR] += tm * lr;
+                dpart[HRL_DIAG_LOGR2] += tm * lr * lr;
+                dpart[HRL_DIAG_ADV] += tm * tot_adv;
+                dpart[HRL_DIAG_ADV2] += tm * tot_adv * tot_adv;
+            }
+            if (prm.has_v) {
+                const float e = tg[0] - smem[L.vraw + row] * om;
+                dpart[HRL_DIAG_N_VAL] += om;
+                dpart[HRL_DIAG_TV] += om * tg[0];
+                dpart[HRL_DIAG_TV2] += om * tg[0] * tg[0];
+                dpart[HRL_DIAG_EV] += om * e;
+                dpart[HRL_DIAG_EV2] += om * e * e;
+            }
+            if (prm.has_r) {
+                const float e = tg[1] - smem[L.rout + i];
+                dpart[HRL_DIAG_TR] += om * tg[1];
+                dpart[HRL_DIAG_TR2] += om * tg[1] * tg[1];
+                dpart[HRL_DIAG_ER] += om * e;
+                dpart[HRL_DIAG_ER2] += om * e * e;
+            }
+        }
         if (own != 0.0f && (a.tap_target_value || a.tap_target_return || a.tap_advantage)) {
             const size_t gcol = ((size_t)(c.b0 + e) * c.T0 + c.bi + t) * P + p;
             if (a.tap_target_value) a.tap_target_value[gcol] = tg[0];
@@ -519,6 +562,66 @@ __device__ __forceinline__ void finalize_losses(const LossParams &prm, const Sme
         out[HRL_LOSS_DCNT] = (float)s[5];
         *counter = 0u;  // leave the workspace ready for the next launch
     }
+}
+
+// ---- diagnostics (DIAG kernels only): their own block reduction, publish and fixed-order fp64 fold
+__device__ __forceinline__ float *diag_partials(const LossParams &prm) {
+    return reinterpret_cast<float *>(reinterpret_cast<char *>(prm.a.workspace) + loss_workspace_base_bytes(prm.a.B));
+}
+
+// All threads: block-reduce dpart (8 sums per round through the reduction scratch) and store this CTA's partials.  Each
+// storing thread fences before the barrier, so the partials are visible device-wide before the publishing warp takes its
+// ticket.  Ends with a barrier: the scratch is free for reduce_partials.
+__device__ __forceinline__ void reduce_diag(const LossParams &prm, const SmemLayout &L, float *smem, const CtaCtx &c,
+                                           const float *dpart) {
+    const int warp = c.tid >> 5, wl = c.tid & 31, nwarp = (c.nthr + 31) >> 5;
+    float *out = diag_partials(prm) + (size_t)blockIdx.x * kDiagStride;
+#pragma unroll
+    for (int r0 = 0; r0 < HRL_NUM_LOSS_DIAG; r0 += 8) {
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            const float v = warp_sum(dpart[r0 + i]);
+            if (wl == 0) smem[L.red + i * 32 + warp] = v;
+        }
+        __syncthreads();
+        if (c.tid < 8) {
+            float s = 0.f;
+            for (int w2 = 0; w2 < nwarp; w2++) s += smem[L.red + c.tid * 32 + w2];
+            __stcg(out + r0 + c.tid, s);
+            __threadfence();
+        }
+        __syncthreads();
+    }
+}
+
+// Last CTA only (after finalize_losses): fold every CTA's diagnostics partials in a fixed order in fp64, write prm.diag.
+__device__ __forceinline__ void finalize_diag(const LossParams &prm, const SmemLayout &L, float *smem, const CtaCtx &c) {
+    const int warp = c.tid >> 5, wl = c.tid & 31, nwarp = (c.nthr + 31) >> 5;
+    const float *partials = diag_partials(prm);
+    double acc[HRL_NUM_LOSS_DIAG];
+#pragma unroll
+    for (int i = 0; i < HRL_NUM_LOSS_DIAG; i++) acc[i] = 0.0;
+    for (int blk = c.tid; blk < (int)gridDim.x; blk += c.nthr) {
+#pragma unroll
+        for (int i = 0; i < HRL_NUM_LOSS_DIAG; i++) acc[i] += (double)__ldcg(partials + (size_t)blk * kDiagStride + i);
+    }
+    double *dred = reinterpret_cast<double *>(smem + L.red);   // 6 x 32 doubles: four sums per round
+#pragma unroll
+    for (int r0 = 0; r0 < HRL_NUM_LOSS_DIAG; r0 += 4) {
+        __syncthreads();
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const double v = warp_sum_d(acc[r0 + i]);
+            if (wl == 0) dred[i * 32 + warp] = v;
+        }
+        __syncthreads();
+        if (c.tid < 4) {
+            double s = 0.0;
+            for (int w2 = 0; w2 < nwarp; w2++) s += dred[c.tid * 32 + w2];
+            prm.diag[r0 + c.tid] = (float)s;
+        }
+    }
+    if (c.tid < HRL_NUM_DIAG - HRL_NUM_LOSS_DIAG) prm.diag[HRL_NUM_LOSS_DIAG + c.tid] = 0.0f;   // the optimiser's entries
 }
 
 // per-row gradient factors gathered from the per-cell terms (sum over players when Pa == 1)

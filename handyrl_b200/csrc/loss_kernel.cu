@@ -143,7 +143,8 @@ __device__ __forceinline__ void row_epilogue(const LossParams &prm, const SmemLa
 
 // ======================================================================== rows kernel
 // IOS: logits and action masks staged in shared memory by cp.async (rows read/written on chip only).
-template <int LPR, int NPL, bool VEC, bool IOS>
+// DIAG (every kernel): the learner diagnostics sums are accumulated in phase 2c and folded with the losses.
+template <int LPR, int NPL, bool VEC, bool IOS, bool DIAG>
 __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
     extern __shared__ __align__(128) float smem[];
     __shared__ bool s_last;
@@ -257,9 +258,10 @@ __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
     HRL_STAMP(3);
 
     // ---------------- phase 2: targets, recurrences, per-cell terms; one warp publishes the scalars
-    float part[6];
-    targets_and_losses(prm, L, smem, c, part);
+    float part[6], dpart[DIAG ? HRL_NUM_LOSS_DIAG : 1];
+    targets_and_losses<DIAG>(prm, L, smem, c, part, dpart);
     HRL_STAMP(4);
+    if (DIAG) reduce_diag(prm, L, smem, c, dpart);
     reduce_partials(L, smem, c, part);
     if ((tid >> 5) == (nthr >> 5) - 1) publish_partials(prm, L, smem, c, &s_last);
     HRL_STAMP(5);
@@ -333,7 +335,10 @@ __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
     }
     zero_burn_in(prm, c);
     __syncthreads();
-    if (s_last) finalize_losses(prm, L, smem, c);
+    if (s_last) {
+        finalize_losses(prm, L, smem, c);
+        if (DIAG) finalize_diag(prm, L, smem, c);
+    }
     HRL_STAMP(6);
 }
 
@@ -342,6 +347,7 @@ __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
 // are coalesced without any staging copy, every element-wise step (masking, exp, gradient) is one short
 // dependent chain per thread, and the row-wise steps (max, sums, scalar tail) are short loops over A <= 32
 // values held in shared memory.  This is the latency-optimal mapping when a window is only a few KB.
+template <bool DIAG>
 __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
     extern __shared__ __align__(128) float smem[];
     __shared__ bool s_last;
@@ -410,9 +416,10 @@ __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
     __syncthreads();
     HRL_STAMP(3);
 
-    float part[6];
-    targets_and_losses(prm, L, smem, c, part);
+    float part[6], dpart[DIAG ? HRL_NUM_LOSS_DIAG : 1];
+    targets_and_losses<DIAG>(prm, L, smem, c, part, dpart);
     HRL_STAMP(4);
+    if (DIAG) reduce_diag(prm, L, smem, c, dpart);
     reduce_partials(L, smem, c, part);
     if ((tid >> 5) == (nthr >> 5) - 1) publish_partials(prm, L, smem, c, &s_last);
     HRL_STAMP(5);
@@ -443,7 +450,10 @@ __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
     HRL_STAMP(19);
     zero_burn_in(prm, c);
     __syncthreads();
-    if (s_last) finalize_losses(prm, L, smem, c);
+    if (s_last) {
+        finalize_losses(prm, L, smem, c);
+        if (DIAG) finalize_diag(prm, L, smem, c);
+    }
     HRL_STAMP(6);
 }
 
@@ -451,7 +461,7 @@ __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
 // Same job as the element kernel with fewer barrier-separated stages: RL = 2^k >= A lanes own one row, so the row
 // maximum, the exponential sums and the gathered logit are warp shuffles inside the lane group (one fused stage
 // instead of four), and the gradient stage recomputes the row factors per lane instead of a separate row pass.
-template <int RL>
+template <int RL, bool DIAG>
 __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) {
     extern __shared__ __align__(128) float smem[];
     __shared__ bool s_last;
@@ -502,9 +512,10 @@ __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) 
     __syncthreads();
     HRL_STAMP(3);
 
-    float part[6];
-    targets_and_losses(prm, L, smem, c, part);
+    float part[6], dpart[DIAG ? HRL_NUM_LOSS_DIAG : 1];
+    targets_and_losses<DIAG>(prm, L, smem, c, part, dpart);
     HRL_STAMP(4);
+    if (DIAG) reduce_diag(prm, L, smem, c, dpart);
     reduce_partials(L, smem, c, part);
     if ((tid >> 5) == (nthr >> 5) - 1) publish_partials(prm, L, smem, c, &s_last);
     HRL_STAMP(5);
@@ -531,7 +542,10 @@ __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) 
     HRL_STAMP(19);
     zero_burn_in(prm, c);
     __syncthreads();
-    if (s_last) finalize_losses(prm, L, smem, c);
+    if (s_last) {
+        finalize_losses(prm, L, smem, c);
+        if (DIAG) finalize_diag(prm, L, smem, c);
+    }
     HRL_STAMP(6);
 }
 
@@ -545,6 +559,7 @@ __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) 
 //   * after the (redundant, cheap) recurrences each warp turns its rows into gradients in place and sends every
 //     row home with a bulk store.
 // Shared memory is zbuf + ~14 KB, so two CTAs (32 row-reducing warps) share an SM.
+template <bool DIAG>
 __global__ void __launch_bounds__(544, 2) loss_bulk_kernel(const LossParams prm) {
     extern __shared__ __align__(128) float smem[];
     __shared__ bool s_last;
@@ -696,9 +711,10 @@ __global__ void __launch_bounds__(544, 2) loss_bulk_kernel(const LossParams prm)
     __syncthreads();
     HRL_STAMP(3);
 
-    float part[6];
-    targets_and_losses(prm, L, smem, c, part);
+    float part[6], dpart[DIAG ? HRL_NUM_LOSS_DIAG : 1];
+    targets_and_losses<DIAG>(prm, L, smem, c, part, dpart);
     HRL_STAMP(4);
+    if (DIAG) reduce_diag(prm, L, smem, c, dpart);
     reduce_partials(L, smem, c, part);
     if (warp == NC - 1) publish_partials(prm, L, smem, c, &s_last);
     HRL_STAMP(5);
@@ -771,7 +787,10 @@ __global__ void __launch_bounds__(544, 2) loss_bulk_kernel(const LossParams prm)
     if (lane == 0) bulk_store_wait_all();
     if (crank == 0) zero_burn_in(prm, c);
     __syncthreads();
-    if (s_last) finalize_losses(prm, L, smem, c);
+    if (s_last) {
+        finalize_losses(prm, L, smem, c);
+        if (DIAG) finalize_diag(prm, L, smem, c);
+    }
     HRL_STAMP(6);
 }
 
@@ -785,8 +804,9 @@ static int launch_kernel(K kern, const LossParams &prm, int grid, int threads, s
     return HRL_OK;
 }
 
+template <bool DIAG>
 static int launch_bulk(const LossParams &prm, int grid, int threads, size_t smem_bytes, cudaStream_t stream) {
-    HRL_CUDA_CHECK(cudaFuncSetAttribute(loss_bulk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    HRL_CUDA_CHECK(cudaFuncSetAttribute(loss_bulk_kernel<DIAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(threads);
@@ -799,7 +819,7 @@ static int launch_bulk(const LossParams &prm, int grid, int threads, size_t smem
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    HRL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, loss_bulk_kernel, prm));
+    HRL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, loss_bulk_kernel<DIAG>, prm));
     return HRL_OK;
 }
 
@@ -809,17 +829,19 @@ static int pow2_ceil(int x) {
     return p;
 }
 
-}  // namespace hrl
-
-extern "C" size_t hrl_loss_workspace_bytes(int32_t B, int32_t, int32_t, int32_t, int32_t) {
-    return 2048 + 8 * (size_t)(B > 0 ? B : 0) * 8 * sizeof(float);   // header (ticket) + up to eight CTAs (a cluster) per window
-}
-
-extern "C" int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream_) {
-    using namespace hrl;
+// The dispatch of hrl_loss_fwd_bwd; DIAG picks the kernels with the diagnostics sums compiled in (same choice of variant,
+// launch shape and shared memory).
+template <bool DIAG>
+static int loss_fwd_bwd(const HrlLossArgs *args, float *diag, void *stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     HRL_REQUIRE(args != nullptr, HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: args is NULL");
     const HrlLossArgs &a = *args;
+    if (DIAG) {
+        HRL_REQUIRE(diag != nullptr, HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd_diag: diag is NULL");
+        HRL_REQUIRE(a.workspace != nullptr && a.workspace_bytes >= loss_diag_workspace_bytes(a.B), HRL_ERR_WORKSPACE,
+                    "hrl_loss_fwd_bwd_diag: workspace of %zu bytes is too small (need %zu, hrl_loss_diag_workspace_bytes)",
+                    a.workspace_bytes, loss_diag_workspace_bytes(a.B));
+    }
     HRL_REQUIRE(a.B > 0 && a.T > 0 && a.P > 0 && a.A > 0, HRL_ERR_BAD_ARG,
                 "hrl_loss_fwd_bwd: non-positive dimension (B=%d T=%d P=%d A=%d)", a.B, a.T, a.P, a.A);
     HRL_REQUIRE(a.Pa == 1 || a.Pa == a.P, HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: Pa must be 1 or P (Pa=%d P=%d)", a.Pa, a.P);
@@ -841,6 +863,7 @@ extern "C" int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream_) {
     prm.has_v = a.value_raw != nullptr;
     prm.has_r = a.return_raw != nullptr;
     prm.cluster = 1;
+    prm.diag = diag;
     const HrlLossTuning &tune = a.tuning;
     HRL_REQUIRE(tune.variant >= 0 && tune.variant <= 5 && tune.recurrence >= 0 && tune.recurrence <= 2 && tune.cluster >= 0 &&
                     tune.cluster <= 8 && tune.consumers >= 0 && tune.threads >= 0 && tune.threads <= 1024 && tune.threads % 32 == 0,
@@ -899,7 +922,7 @@ extern "C" int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream_) {
             const int grid = a.B * best_cs;
             HRL_REQUIRE(a.workspace != nullptr && a.workspace_bytes >= 2048 + (size_t)grid * 8 * sizeof(float), HRL_ERR_WORKSPACE,
                         "hrl_loss_fwd_bwd: workspace of %zu bytes is too small", a.workspace_bytes);
-            return launch_bulk(prm, grid, NC * 32, best_bytes, stream);
+            return launch_bulk<DIAG>(prm, grid, NC * 32, best_bytes, stream);
         }
         HRL_REQUIRE(mode != 2, HRL_ERR_UNSUPPORTED, "hrl_loss_fwd_bwd: bulk kernel forced but the window does not fit");
     }
@@ -930,12 +953,12 @@ extern "C" int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream_) {
                         "hrl_loss_fwd_bwd: workspace of %zu bytes is too small", a.workspace_bytes);
             const size_t bytes = (size_t)L.total * 4;
             switch (RL) {
-                case 1: return launch_kernel(loss_group_kernel<1>, prm, grid0, threads, bytes, stream);
-                case 2: return launch_kernel(loss_group_kernel<2>, prm, grid0, threads, bytes, stream);
-                case 4: return launch_kernel(loss_group_kernel<4>, prm, grid0, threads, bytes, stream);
-                case 8: return launch_kernel(loss_group_kernel<8>, prm, grid0, threads, bytes, stream);
-                case 16: return launch_kernel(loss_group_kernel<16>, prm, grid0, threads, bytes, stream);
-                default: return launch_kernel(loss_group_kernel<32>, prm, grid0, threads, bytes, stream);
+                case 1: return launch_kernel(loss_group_kernel<1, DIAG>, prm, grid0, threads, bytes, stream);
+                case 2: return launch_kernel(loss_group_kernel<2, DIAG>, prm, grid0, threads, bytes, stream);
+                case 4: return launch_kernel(loss_group_kernel<4, DIAG>, prm, grid0, threads, bytes, stream);
+                case 8: return launch_kernel(loss_group_kernel<8, DIAG>, prm, grid0, threads, bytes, stream);
+                case 16: return launch_kernel(loss_group_kernel<16, DIAG>, prm, grid0, threads, bytes, stream);
+                default: return launch_kernel(loss_group_kernel<32, DIAG>, prm, grid0, threads, bytes, stream);
             }
         }
     }
@@ -963,7 +986,7 @@ extern "C" int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream_) {
             const int grid = (a.B + EPB - 1) / EPB;
             HRL_REQUIRE(a.workspace != nullptr && a.workspace_bytes >= 2048 + (size_t)grid * 8 * sizeof(float), HRL_ERR_WORKSPACE,
                         "hrl_loss_fwd_bwd: workspace of %zu bytes is too small", a.workspace_bytes);
-            return launch_kernel(loss_elem_kernel, prm, grid, threads, (size_t)L.total * 4, stream);
+            return launch_kernel(loss_elem_kernel<DIAG>, prm, grid, threads, (size_t)L.total * 4, stream);
         }
     }
 
@@ -1010,7 +1033,7 @@ extern "C" int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream_) {
                 2048 + (size_t)grid * 8 * sizeof(float));
 
 #define HRL_CASE(l, n, v, s) \
-    if (LPR == l && NPL == n && vec == v && ios == s) return launch_kernel(loss_rows_kernel<l, n, v, s>, prm, grid, threads, smem_bytes, stream);
+    if (LPR == l && NPL == n && vec == v && ios == s) return launch_kernel(loss_rows_kernel<l, n, v, s, DIAG>, prm, grid, threads, smem_bytes, stream);
 #define HRL_CASE2(l, n) HRL_CASE(l, n, false, false) HRL_CASE(l, n, false, true)
     HRL_CASE2(1, 1) HRL_CASE2(1, 2) HRL_CASE2(1, 4) HRL_CASE2(1, 8) HRL_CASE2(1, 16)
     HRL_CASE2(2, 16) HRL_CASE2(4, 16) HRL_CASE2(8, 16) HRL_CASE2(16, 16) HRL_CASE2(32, 16)
@@ -1020,4 +1043,20 @@ extern "C" int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream_) {
 #undef HRL_CASE
     set_error("hrl_loss_fwd_bwd: no kernel for LPR=%d NPL=%d", LPR, NPL);
     return HRL_ERR_UNSUPPORTED;
+}
+
+}  // namespace hrl
+
+extern "C" size_t hrl_loss_workspace_bytes(int32_t B, int32_t, int32_t, int32_t, int32_t) {
+    return hrl::loss_workspace_base_bytes(B);   // header (ticket) + up to eight CTAs (a cluster) per window
+}
+
+extern "C" size_t hrl_loss_diag_workspace_bytes(int32_t B, int32_t, int32_t, int32_t, int32_t) {
+    return hrl::loss_diag_workspace_bytes(B);   // + the diagnostics partials of up to eight CTAs per window
+}
+
+extern "C" int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream) { return hrl::loss_fwd_bwd<false>(args, nullptr, stream); }
+
+extern "C" int hrl_loss_fwd_bwd_diag(const HrlLossArgs *args, float *diag, void *stream) {
+    return hrl::loss_fwd_bwd<true>(args, diag, stream);
 }

@@ -35,11 +35,13 @@ __global__ void __launch_bounds__(kOptThreads) grad_sumsq_kernel(const float *__
     }
 }
 
+// DIAG: block 0 also adds g, g^2, [g > max_norm], 1 to diag[0..3] (learner diagnostics, include/hrl_b200.h)
+template <bool DIAG>
 __global__ void __launch_bounds__(kOptThreads) clip_adam_kernel(
     float *__restrict__ param, const float *__restrict__ grad, float *__restrict__ exp_avg,
     float *__restrict__ exp_avg_sq, int64_t n, const float *__restrict__ partials, const float *__restrict__ lr_p,
     int64_t *step_p, double max_norm_d, double beta1_d, double beta2_d, double eps_d, double wd_d,
-    float *grad_norm_out) {
+    float *grad_norm_out, double *diag) {
     const float max_norm = (float)max_norm_d, beta2 = (float)beta2_d, eps = (float)eps_d, wd = (float)wd_d;
     // every block folds the partial sums in the same order -> identical clip coefficient everywhere
     __shared__ double red[kOptThreads / 32];
@@ -56,6 +58,12 @@ __global__ void __launch_bounds__(kOptThreads) clip_adam_kernel(
         float coef = max_norm / (total_norm + 1e-6f);  // torch clip_grad_norm_
         s_coef = fminf(coef, 1.0f);
         if (blockIdx.x == 0 && grad_norm_out) *grad_norm_out = total_norm;
+        if (DIAG && blockIdx.x == 0) {
+            diag[0] += (double)total_norm;
+            diag[1] += (double)total_norm * (double)total_norm;
+            diag[2] += total_norm > max_norm ? 1.0 : 0.0;
+            diag[3] += 1.0;
+        }
     }
     __syncthreads();
     const float coef = s_coef;
@@ -200,19 +208,37 @@ extern "C" int hrl_grad_sumsq(const float *grad, int64_t n, float *partials, voi
     return HRL_OK;
 }
 
-extern "C" int hrl_clip_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
-                                  const float *partials, const float *lr, int64_t *step, double max_norm, double beta1,
-                                  double beta2, double eps, double weight_decay, float *grad_norm_out, void *stream) {
-    using namespace hrl;
+namespace hrl {
+template <bool DIAG>
+static int clip_adam_step(const char *name, float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
+                          const float *partials, const float *lr, int64_t *step, double max_norm, double beta1, double beta2,
+                          double eps, double weight_decay, float *grad_norm_out, double *diag, void *stream) {
     HRL_REQUIRE(param && grad && exp_avg && exp_avg_sq && partials && lr && step && n > 0, HRL_ERR_BAD_ARG,
-                "hrl_clip_adam_step: NULL pointer or n <= 0");
+                "%s: NULL pointer or n <= 0", name);
+    HRL_REQUIRE(!DIAG || diag, HRL_ERR_BAD_ARG, "%s: diag_accum is NULL", name);
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     int grid = (int)((n + kOptThreads - 1) / kOptThreads);
     if (grid > kPartials) grid = kPartials;
-    clip_adam_kernel<<<grid, kOptThreads, 0, s>>>(param, grad, exp_avg, exp_avg_sq, n, partials, lr, step, max_norm,
-                                                  beta1, beta2, eps, weight_decay, grad_norm_out);
+    clip_adam_kernel<DIAG><<<grid, kOptThreads, 0, s>>>(param, grad, exp_avg, exp_avg_sq, n, partials, lr, step, max_norm,
+                                                        beta1, beta2, eps, weight_decay, grad_norm_out, diag);
     HRL_CUDA_CHECK(cudaGetLastError());
     bump_step_kernel<<<1, 1, 0, s>>>(step);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
+}
+}  // namespace hrl
+
+extern "C" int hrl_clip_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
+                                  const float *partials, const float *lr, int64_t *step, double max_norm, double beta1,
+                                  double beta2, double eps, double weight_decay, float *grad_norm_out, void *stream) {
+    return hrl::clip_adam_step<false>("hrl_clip_adam_step", param, grad, exp_avg, exp_avg_sq, n, partials, lr, step, max_norm,
+                                      beta1, beta2, eps, weight_decay, grad_norm_out, nullptr, stream);
+}
+
+extern "C" int hrl_clip_adam_step_diag(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
+                                       const float *partials, const float *lr, int64_t *step, double max_norm, double beta1,
+                                       double beta2, double eps, double weight_decay, float *grad_norm_out, double *diag_accum,
+                                       void *stream) {
+    return hrl::clip_adam_step<true>("hrl_clip_adam_step_diag", param, grad, exp_avg, exp_avg_sq, n, partials, lr, step,
+                                     max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, diag_accum, stream);
 }

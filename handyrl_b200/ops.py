@@ -9,7 +9,7 @@ import ctypes as C
 import torch
 
 from . import _capi
-from ._capi import ALGO_ID, LOSS_KEYS, NUM_LOSS, HrlLossArgs, check, lib
+from ._capi import ALGO_ID, DIAG_KEYS, LOSS_KEYS, NUM_DIAG, NUM_LOSS, HrlLossArgs, check, lib
 
 # kernels of THIS library launched through the wrappers below (bench.py reports them as `gpu_launches`; a CUDA graph
 # replays the launches counted while it was captured)
@@ -53,7 +53,7 @@ def algo_id(name):
 class LossBuffers:
     """Pre-allocated outputs of one fused loss launch (re-used across steps / graph replays)."""
 
-    def __init__(self, B, T, P, Pa, A, has_value, has_return, device, taps=False, policy_dtype=torch.float32):
+    def __init__(self, B, T, P, Pa, A, has_value, has_return, device, taps=False, policy_dtype=torch.float32, diagnostics=False):
         f = dict(dtype=torch.float32, device=device)
         self.dims = (B, T, P, Pa, A)
         self.dpolicy = torch.empty((B, T, Pa, A), dtype=policy_dtype, device=device)      # bf16 logits get bf16 gradients
@@ -68,9 +68,20 @@ class LossBuffers:
                 'rho': torch.zeros((B, T, Pa, 1), **f), 'entropy': torch.zeros((B, T, Pa), **f),
             }
         self.workspace = torch.zeros(lib().hrl_loss_workspace_bytes(B, T, P, Pa, A), dtype=torch.uint8, device=device)
+        self.diagnostics = self.diag_workspace = None
+        if diagnostics:
+            self.enable_diagnostics()
+
+    def enable_diagnostics(self):
+        """Allocate the outputs of the diagnostics form of the pass: `diagnostics` (NUM_DIAG sums in DIAG_KEYS order) and its
+        own, larger workspace."""
+        if self.diagnostics is None:
+            device = self.losses.device
+            self.diagnostics = torch.zeros(NUM_DIAG, dtype=torch.float32, device=device)
+            self.diag_workspace = torch.zeros(lib().hrl_loss_diag_workspace_bytes(*self.dims), dtype=torch.uint8, device=device)
 
 
-def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None):
+def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None, diagnostics=False):
     """Fused mask epilogue + compute_loss + closed-form backward (reference train.py:176-267).
 
     outputs: raw net outputs {'policy': (B,T,Pa,A), 'value': (B,T,Pa,1)?, 'return': (B,T,Pa,1)?}
@@ -80,6 +91,8 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None):
     tuning:  None (the library chooses), or a dict for tests / profiling with any of
              variant ('rows-direct'|'rows-staged'|'bulk'|'element'|'group'), recurrence ('serial'|'scan'),
              cluster, consumers, threads, unstaged, trace (an int64 CUDA tensor of >= 32 elements)
+    diagnostics: also accumulate the learner diagnostics sums (hrl_loss_fwd_bwd_diag) into .diagnostics, in DIAG_KEYS order;
+             losses and gradients are bit-identical to the plain pass
     returns  LossBuffers with .losses = [p, v, r, ent, total, dcnt] and the gradients.
     """
     policy = outputs['policy']
@@ -96,6 +109,8 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None):
     if buffers is None:
         buffers = LossBuffers(B, T, P, Pa, A, value is not None, ret_head is not None, policy.device, taps=taps, policy_dtype=policy.dtype)
     assert buffers.dims == (B, T, P, Pa, A) and buffers.dpolicy.dtype == policy.dtype
+    if diagnostics:
+        buffers.enable_diagnostics()
 
     # static buffers (CUDA-graph replays): the argument block of the previous call is still valid
     key = (policy.data_ptr(), 0 if value is None else value.data_ptr(), 0 if ret_head is None else ret_head.data_ptr(),
@@ -104,10 +119,10 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None):
            buffers.taps is not None, None if tuning is None else tuple(sorted((k, v if not torch.is_tensor(v) else v.data_ptr())
                                                                                  for k, v in tuning.items()))) + \
         tuple(batch[k].data_ptr() for k in _BATCH_KEYS)
-    cached = getattr(buffers, '_cached', None)
+    slot = '_cached_diag' if diagnostics else '_cached'      # one argument block per form
+    cached = getattr(buffers, slot, None)
     if cached is not None and cached[0] == key:
-        check(lib().hrl_loss_fwd_bwd(C.byref(cached[1]), _stream_ptr()))
-        _count()
+        _launch(cached[1], buffers, diagnostics)
         return buffers
 
     a = HrlLossArgs()
@@ -139,8 +154,9 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None):
         a.tap_target_value, a.tap_target_return, a.tap_advantage = _ptr(t['target_value']), _ptr(t['target_return']), _ptr(t['advantage'])
         a.tap_logp, a.tap_rho, a.tap_entropy = _ptr(t['logp']), _ptr(t['rho']), _ptr(t['entropy'])
     a.io_bf16 = int(io_bf16)
-    a.workspace = _ptr(buffers.workspace)
-    a.workspace_bytes = buffers.workspace.numel()
+    ws = buffers.diag_workspace if diagnostics else buffers.workspace
+    a.workspace = _ptr(ws)
+    a.workspace_bytes = ws.numel()
     if tuning:
         t = dict(tuning)
         a.tuning.variant = _capi.LOSS_VARIANTS[t.pop('variant', 'auto')]
@@ -153,15 +169,72 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None):
             setattr(a.tuning, k, int(t.pop(k, 0)))
         if t:
             raise ValueError('unknown loss tuning keys: %s' % sorted(t))
-    check(lib().hrl_loss_fwd_bwd(C.byref(a), _stream_ptr()))
-    _count()
+    _launch(a, buffers, diagnostics)
     buffers._keep = keep  # the launch is asynchronous: keep temporaries alive
     if all(k is None or k is o for k, o in zip(keep[3:], (batch['action_mask'], batch['action'], batch['selected_prob'],
                                                           batch['reward'], batch['return'], batch['turn_mask'],
                                                           batch['observation_mask'], batch['episode_mask'],
                                                           batch['progress'], batch['outcome']))):
-        buffers._cached = (key, a)   # only when no temporary copies were made
+        setattr(buffers, slot, (key, a))   # only when no temporary copies were made
     return buffers
+
+
+def _launch(a, buffers, diagnostics):
+    if diagnostics:
+        check(lib().hrl_loss_fwd_bwd_diag(C.byref(a), _ptr(buffers.diagnostics), _stream_ptr()))
+    else:
+        check(lib().hrl_loss_fwd_bwd(C.byref(a), _stream_ptr()))
+    _count()
+
+
+def summarize_diagnostics(sums):
+    """Diagnostics sums (a sequence in DIAG_KEYS order, or a dict keyed by DIAG_KEYS; missing entries count as 0) -> means:
+      rho     mean unclipped importance ratio pi(a)/mu(a)        clip    fraction of samples with rho > 1 (clipped at 1)
+      kl      -mean log ratio, the sample estimate of KL(mu||pi)  logr_sd spread of the log ratio
+      adv     mean advantage                                      adv_sd  its standard deviation
+      ev_v    explained variance of the value target, 1 - Var(target - value) / Var(target); ev_r: the return head's
+      gnorm   mean pre-clip global gradient norm                  gclip   fraction of steps whose norm exceeded max_norm
+    A field whose count (or target variance) is zero is left out: nothing is ever divided by zero."""
+    if isinstance(sums, dict):
+        s = {k: float(sums.get(k, 0.0)) for k in DIAG_KEYS}
+    else:
+        vals = [float(x) for x in (sums.tolist() if hasattr(sums, 'tolist') else sums)]
+        s = dict(zip(DIAG_KEYS, vals + [0.0] * (NUM_DIAG - len(vals))))
+
+    def sd(total, total2, n):
+        return max(total2 / n - (total / n) ** 2, 0.0) ** 0.5
+
+    out = {}
+    n = s['n_pol']
+    if n > 0:
+        out['rho'] = s['rho'] / n
+        out['clip'] = s['rho_clip'] / n
+        out['kl'] = -s['logr'] / n
+        out['logr_sd'] = sd(s['logr'], s['logr2'], n)
+        out['adv'] = s['adv'] / n
+        out['adv_sd'] = sd(s['adv'], s['adv2'], n)
+    n = s['n_val']
+    if n > 0:
+        for key, t, t2, e, e2 in (('ev_v', 'tv', 'tv2', 'ev', 'ev2'), ('ev_r', 'tr', 'tr2', 'er', 'er2')):
+            var_t = s[t2] / n - (s[t] / n) ** 2      # (0 without the head)
+            if var_t > 0:
+                out[key] = 1.0 - max(s[e2] / n - (s[e] / n) ** 2, 0.0) / var_t
+    n = s['steps']
+    if n > 0:
+        out['gnorm'] = s['gnorm'] / n
+        out['gnorm_sd'] = sd(s['gnorm'], s['gnorm2'], n)
+        out['gclip'] = s['gclip'] / n
+    return out
+
+
+_DIAG_FORMAT = (('rho', '%.3f'), ('clip', '%.3f'), ('kl', '%.4g'), ('logr_sd', '%.4g'), ('adv', '%.4g'), ('adv_sd', '%.4g'),
+                ('ev_v', '%.3f'), ('ev_r', '%.3f'), ('gnorm', '%.4g'), ('gnorm_sd', '%.4g'), ('gclip', '%.3f'))
+
+
+def format_diagnostics(summary):
+    """The Trainer's per-epoch line: 'diagnostics = rho:1.024 clip:0.318 kl:0.041 ...' -- `key:value` pairs in a fixed
+    order, fields absent from `summary` left out."""
+    return 'diagnostics = %s' % ' '.join(k + ':' + (f % summary[k]) for k, f in _DIAG_FORMAT if k in summary)
 
 
 def compute_target(algorithm, values, returns, rewards, lmb, gamma, rhos, cs, masks):
@@ -234,6 +307,9 @@ class FlatAdam:
         self.step_count = torch.zeros(1, dtype=torch.int64, device=device)
         self.grad_norm = torch.zeros(1, dtype=torch.float32, device=device)
         self.betas, self.eps, self.weight_decay, self.max_norm = betas, eps, weight_decay, max_norm
+        # diagnostics: a float64 CUDA tensor of 4 (the gnorm, gnorm2, gclip, steps entries of a DIAG_KEYS accumulator) that
+        # every step adds its pre-clip norm statistics to, in the step's own launch; None = off
+        self.diag = None
 
     @property
     def extra_slots(self):
@@ -248,19 +324,23 @@ class FlatAdam:
     def step_reduced(self, reduced):
         """clip + Adam on an already all-reduced bucket whose sum-of-squares partials are in self.partials
         (hrl_peer_allreduce_sumsq)."""
-        check(lib().hrl_clip_adam_step(_ptr(self.flat_param), _ptr(reduced), _ptr(self.exp_avg), _ptr(self.exp_avg_sq),
-                                       self.n_pad, _ptr(self.partials), _ptr(self.lr), _ptr(self.step_count), self.max_norm,
-                                       self.betas[0], self.betas[1], self.eps, self.weight_decay, _ptr(self.grad_norm),
-                                       _stream_ptr()))
+        self._clip_adam(reduced, _stream_ptr())
         _count(2)
+
+    def _clip_adam(self, grad, s):
+        fixed = (_ptr(self.flat_param), _ptr(grad), _ptr(self.exp_avg), _ptr(self.exp_avg_sq), self.n_pad, _ptr(self.partials),
+                 _ptr(self.lr), _ptr(self.step_count), self.max_norm, self.betas[0], self.betas[1], self.eps, self.weight_decay,
+                 _ptr(self.grad_norm))
+        if self.diag is not None:
+            assert self.diag.is_cuda and self.diag.dtype == torch.float64 and self.diag.numel() == 4 and self.diag.is_contiguous()
+            check(lib().hrl_clip_adam_step_diag(*fixed, _ptr(self.diag), s))
+        else:
+            check(lib().hrl_clip_adam_step(*fixed, s))
 
     def step(self):
         s = _stream_ptr()
         check(lib().hrl_grad_sumsq(_ptr(self.flat_grad), self.n_pad, _ptr(self.partials), s))
-        check(lib().hrl_clip_adam_step(_ptr(self.flat_param), _ptr(self.flat_grad), _ptr(self.exp_avg),
-                                       _ptr(self.exp_avg_sq), self.n_pad, _ptr(self.partials), _ptr(self.lr),
-                                       _ptr(self.step_count), self.max_norm, self.betas[0], self.betas[1], self.eps,
-                                       self.weight_decay, _ptr(self.grad_norm), s))
+        self._clip_adam(self.flat_grad, s)
         _count(3)
         from . import fastnet
         fastnet.new_step()          # cached adjoint weights of the convolutions are stale now

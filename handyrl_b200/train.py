@@ -28,7 +28,7 @@ import torch
 
 from . import ops, fastnet
 from .batch import tree_map, tree_leaves, make_batch, gather_windows, sample_window
-from ._capi import LOSS_KEYS, NUM_LOSS
+from ._capi import DIAG_KEYS, LOSS_KEYS, NUM_DIAG, NUM_LOSS, NUM_LOSS_DIAG
 
 
 # --------------------------------------------------------------------------- forward
@@ -303,10 +303,16 @@ class PendingModel:
 
     def resolve(self):
         self.done.synchronize()
-        sums = dict(zip(LOSS_KEYS, self.host_losses.tolist()))
+        host = self.host_losses.tolist()
+        sums = dict(zip(LOSS_KEYS, host[:NUM_LOSS]))
         dcnt = sums['dcnt']
+        self.diagnostics = None
+        if len(host) > NUM_LOSS:        # the learner's diagnostics sums ride behind the loss sums
+            self.diagnostics = ops.summarize_diagnostics(host[NUM_LOSS:])
         if dcnt > 0:
             print('loss = %s' % ' '.join([k + ':' + '%.3f' % (sums[k] / dcnt) for k in self.heads]))
+            if self.diagnostics is not None:
+                print(ops.format_diagnostics(self.diagnostics))
         tpl = self.template
         state = self.stepper.state.state_dict_from(self.host_state, tpl.state_dict().keys())
         for k, b in self.stepper.state.loose:
@@ -334,13 +340,23 @@ class LearnerStep:
     fused loss fwd+bwd kernel -> net backward -> (all-reduce SUM) -> clip + Adam].
     The six loss sums land in `last_losses` / `loss_accum` on the device; nothing in here
     synchronises the host.
+
+    diagnostics (default: train_args['diagnostics'], off): the loss pass also takes the learner diagnostics sums
+    (ops.DIAG_KEYS), which ride the gradient bucket behind the loss sums, and the optimiser adds its pre-clip norm
+    statistics; both accumulate in `diag_accum` (float64, on the device) until end_epoch / pop_diagnostics.  Losses,
+    gradients and weights are the same with and without.
     """
 
     def __init__(self, model, args, example_batch, lr, device=None, process_group=None, use_graph=True,
                  max_norm=4.0, weight_decay=1e-5, time_loss_kernel=False, channels_last=True, cudnn_benchmark=True,
-                 small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None):
+                 small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None):
         self.device = torch.device(device if device is not None else 'cuda')
         self.args = args
+        if diagnostics is None:
+            diagnostics = bool(args.get('diagnostics', False))
+        self.diagnostics = diagnostics
+        n_sums = NUM_LOSS + (NUM_DIAG if diagnostics else 0)                # accumulator: loss sums [+ diagnostics sums]
+        n_tail = NUM_LOSS + (NUM_LOSS_DIAG if diagnostics else 0)           # bucket tail: [+ the loss pass's diagnostics]
         # the learner owns its precision contract (1e-5 of the reference's fp32 arithmetic): PyTorch's default lets
         # cuDNN convolutions run on TF32 tensor cores (10-bit mantissa).  train_args['allow_tf32'] = True opts out.
         if allow_tf32 is None:
@@ -377,12 +393,12 @@ class LearnerStep:
             peer_allreduce = self.world > 1 and os.environ.get('HRL_PEER_ALLREDUCE', '1') != '0'
         self.peer = ops.PeerAllReduce(self.pg, self.device) if (peer_allreduce and self.world > 1) else None
         self.state = StateStore(self.model, self.device)
-        self.opt = ops.FlatAdam(params, lr=lr, weight_decay=weight_decay, max_norm=max_norm, extra=NUM_LOSS,
+        self.opt = ops.FlatAdam(params, lr=lr, weight_decay=weight_decay, max_norm=max_norm, extra=n_tail,
                                 grad_alloc=self.peer.alloc if self.peer is not None else None,
                                 param_storage=self.state.flat_param)
         self.state.index_params(self.model)
         self.state_snap = torch.empty_like(self.state.bytes)
-        self.acc_snap = torch.zeros(NUM_LOSS, dtype=torch.float64, device=self.device)
+        self.acc_snap = torch.zeros(n_sums, dtype=torch.float64, device=self.device)
         self.copy_stream = torch.cuda.Stream(device=self.device)
         self._handoff_slots = None
         self._handoff_i = 0
@@ -408,7 +424,12 @@ class LearnerStep:
             self.engine = tower.FusedBoardNet(self.model, B * T * Pa, self.device)
         self.loss_buf = None
         self.last_losses = torch.zeros(NUM_LOSS, device=self.device)
-        self.loss_accum = torch.zeros(NUM_LOSS, dtype=torch.float64, device=self.device)
+        self.accum = torch.zeros(n_sums, dtype=torch.float64, device=self.device)
+        self.loss_accum = self.accum[:NUM_LOSS]
+        self.diag_accum = None
+        if diagnostics:
+            self.diag_accum = self.accum[NUM_LOSS:]
+            self.opt.diag = self.diag_accum[NUM_LOSS_DIAG:]        # the optimiser's entries: accumulated by its own kernel
         self.host_slots = torch.zeros((8, NUM_LOSS)).pin_memory()
         self._slot = 0
         self.graph = self.graph_fwd = self.graph_bwd = None
@@ -449,7 +470,7 @@ class LearnerStep:
     def _part_loss(self):
         outs = self._outs
         ops.loss_fwd_bwd({k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, self.dev, self.args,
-                         buffers=self.loss_buf)
+                         buffers=self.loss_buf, diagnostics=self.diagnostics)
 
     def _part_backward(self):
         outs, buf = self._outs, self.loss_buf
@@ -467,16 +488,22 @@ class LearnerStep:
             with ops.deferred_weight_gradients():       # shared (recurrent) convolution weights: one product per weight, at the end
                 torch.autograd.backward(heads, grads)
         self.opt.extra_slots[:NUM_LOSS].copy_(buf.losses)     # the loss sums ride the gradient bucket
+        if self.diagnostics:
+            self.opt.extra_slots[NUM_LOSS:NUM_LOSS + NUM_LOSS_DIAG].copy_(buf.diagnostics[:NUM_LOSS_DIAG])
         if self.peer is not None:
             reduced = self.peer(self.opt.n_pad, self.opt.partials)      # all-reduce + norm partials, one kernel
             self.opt.step_reduced(reduced)
-            self.last_losses.copy_(reduced[self.opt.n_pad:self.opt.n_pad + NUM_LOSS])
+            tail = reduced[self.opt.n_pad:]
+            self.last_losses.copy_(tail[:NUM_LOSS])
         else:
             if self.world > 1:
                 torch.distributed.all_reduce(self.opt.flat_grad, op=torch.distributed.ReduceOp.SUM, group=self.pg)
             self.opt.step()
-            self.last_losses.copy_(self.opt.extra_slots[:NUM_LOSS])
+            tail = self.opt.extra_slots
+            self.last_losses.copy_(tail[:NUM_LOSS])
         self.loss_accum.add_(self.last_losses)
+        if self.diagnostics:
+            self.diag_accum[:NUM_LOSS_DIAG].add_(tail[NUM_LOSS:NUM_LOSS + NUM_LOSS_DIAG])
 
     def _device_step(self):
         self._part_forward()
@@ -516,7 +543,7 @@ class LearnerStep:
     def _snapshot(self):
         bufs = {k: v.clone() for k, v in self.model.state_dict().items()}
         return (bufs, self.opt.exp_avg.clone(), self.opt.exp_avg_sq.clone(), self.opt.step_count.clone(),
-                self.loss_accum.clone())
+                self.accum.clone())
 
     def _restore(self, state):
         bufs, m, v, sc, acc = state
@@ -526,7 +553,7 @@ class LearnerStep:
             self.opt.exp_avg.copy_(m)
             self.opt.exp_avg_sq.copy_(v)
             self.opt.step_count.copy_(sc)
-            self.loss_accum.copy_(acc)
+            self.accum.copy_(acc)
 
     def new_packed(self):
         return PackedBatch(self.layout)
@@ -625,6 +652,16 @@ class LearnerStep:
         self.loss_accum.zero_()
         return dict(zip(LOSS_KEYS, vals))
 
+    def pop_diagnostics(self):
+        """Diagnostics sums (ops.DIAG_KEYS -> float) accumulated since the last call or epoch boundary (one host sync);
+        ops.summarize_diagnostics turns them into means."""
+        if self.diag_accum is None:
+            raise RuntimeError('LearnerStep was built without diagnostics (train_args["diagnostics"] / diagnostics=True)')
+        self.stream.synchronize()
+        vals = self.diag_accum.cpu().tolist()
+        self.diag_accum.zero_()
+        return dict(zip(DIAG_KEYS, vals))
+
     def close(self):
         """Release the captured graphs (they pin NCCL kernels: destroy them before the process group)."""
         self.stream.synchronize()
@@ -649,8 +686,8 @@ class LearnerStep:
         """Device half of the epoch boundary, on the current stream: move the epoch's loss sums aside and apply the
         learning-rate schedule from the (all-reduced, hence global) data count.  Every rank of a sharded learner
         enqueues this at the same step, so all ranks keep identical learning rates without a broadcast."""
-        self.acc_snap.copy_(self.loss_accum)
-        self.loss_accum.zero_()
+        self.acc_snap.copy_(self.accum)
+        self.accum.zero_()
         dcnt = self.acc_snap[5:6].float()
         fresh = self.ema * 0.8 + dcnt * (0.2 / (1e-2 + batch_cnt))
         self.ema.copy_(torch.where(dcnt > 0, fresh, self.ema))
@@ -664,7 +701,7 @@ class LearnerStep:
         next epoch's steps already run.  Returns a PendingModel."""
         if self._handoff_slots is None:
             self._handoff_slots = [(torch.empty(self.state.bytes.numel(), dtype=torch.uint8).pin_memory(),
-                                    torch.zeros(NUM_LOSS, dtype=torch.float64).pin_memory()) for _ in range(2)]
+                                    torch.zeros(self.acc_snap.numel(), dtype=torch.float64).pin_memory()) for _ in range(2)]
         host_state, host_losses = self._handoff_slots[self._handoff_i % 2]
         self._handoff_i += 1
         with torch.cuda.stream(self.stream):

@@ -9,6 +9,8 @@
  *                            handyrl/train.py:189-215 (compose_losses)
  *                            handyrl/losses.py:16-80  (monte_carlo / temporal_difference / upgo / vtrace)
  *                            + the autograd pass of train.py:369 restricted to those ops
+ *   hrl_loss_fwd_bwd_diag <- the same pass + learner diagnostics sums (importance ratios, advantages, value fit);
+ *                            no reference counterpart
  *   hrl_compute_target    <- handyrl/losses.py:63-80  (compute_target, stand-alone)
  *   hrl_peer_allreduce_sumsq <- the gradient exchange nn.DataParallel does implicitly (train.py:339-340), as a
  *                            fused peer-memory kernel
@@ -138,6 +140,35 @@ size_t hrl_loss_workspace_bytes(int32_t B, int32_t T, int32_t P, int32_t Pa, int
 int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream);
 
 /*
+ * Learner diagnostics (opt-in): additive sums, so that shards add up and the sums can ride the gradient all-reduce.
+ * The loss pass sums over trained cells (t >= burn_in), column i = (b, t, p), tm = turn_mask, om = observation_mask,
+ * q = the column's policy row (0 when Pa == 1, else p):
+ *   n_pol     sum tm                                 (== HRL_LOSS_DCNT)
+ *   rho       sum tm * rho, rho = exp(l) UNclipped,  l = log pi(a) * em - log(clamp(mu, 1e-16, 1)) * em   (em = episode_mask)
+ *   rho_clip  sum tm * [rho > 1]                     (samples the V-Trace / UPGO clip at 1 acts on)
+ *   logr      sum tm * l         logr2  sum tm * l^2 (-logr / n_pol estimates KL(mu || pi))
+ *   adv       sum tm * Adv       adv2   sum tm * Adv^2   (Adv = the clipped-rho total advantage, train.py:265)
+ *   n_val     sum om             (value head only; the value / return sums stay 0 without their head)
+ *   tv, tv2   sum om * tgt_v, sum om * tgt_v^2         ev, ev2   sum om * (tgt_v - v), sum om * (tgt_v - v)^2, v = value_raw * om
+ *   tr, tr2, er, er2   the same for the return head
+ * The optimiser step sums g, g^2, [g > max_norm] and 1 per step, g = the pre-clip global gradient norm.
+ */
+enum { HRL_DIAG_N_POL = 0, HRL_DIAG_RHO = 1, HRL_DIAG_RHO_CLIP = 2, HRL_DIAG_LOGR = 3, HRL_DIAG_LOGR2 = 4, HRL_DIAG_ADV = 5,
+       HRL_DIAG_ADV2 = 6, HRL_DIAG_N_VAL = 7, HRL_DIAG_TV = 8, HRL_DIAG_TV2 = 9, HRL_DIAG_EV = 10, HRL_DIAG_EV2 = 11,
+       HRL_DIAG_TR = 12, HRL_DIAG_TR2 = 13, HRL_DIAG_ER = 14, HRL_DIAG_ER2 = 15,
+       HRL_NUM_LOSS_DIAG = 16,                                   /* the sums of the loss pass come first */
+       HRL_DIAG_GNORM = 16, HRL_DIAG_GNORM2 = 17, HRL_DIAG_GCLIP = 18, HRL_DIAG_STEPS = 19,
+       HRL_NUM_DIAG = 20 };
+
+/* Workspace of hrl_loss_fwd_bwd_diag (>= hrl_loss_workspace_bytes; same zero-header rule). */
+size_t hrl_loss_diag_workspace_bytes(int32_t B, int32_t T, int32_t P, int32_t Pa, int32_t A);
+
+/* hrl_loss_fwd_bwd with the diagnostics sums accumulated in the same pass: the same kernels with the extra block sums
+ * compiled in, folded by the last CTA in a fixed order in fp64.  Losses and gradients are bit-identical to
+ * hrl_loss_fwd_bwd.  diag: HRL_NUM_DIAG device floats, overwritten (the optimiser entries with 0). */
+int hrl_loss_fwd_bwd_diag(const HrlLossArgs *args, float *diag, void *stream);
+
+/*
  * Stand-alone compute_target (losses.py:63-80) on (B,T,P) columns.
  *   values   (B,T,P) or NULL  -> targets = advantages = returns (losses.py:64-66)
  *   returns  (B,Tr,P) with Tr == T or Tr == 1 (the (B,1,P,1) outcome of train.py:254)
@@ -169,6 +200,12 @@ int hrl_clip_adam_step(float *param, const float *grad, float *exp_avg, float *e
                        int64_t n, const float *partials, const float *lr, int64_t *step,
                        double max_norm, double beta1, double beta2, double eps, double weight_decay,
                        float *grad_norm_out /* may be NULL */, void *stream);
+/* The same step, also adding g, g^2, [g > max_norm] and 1 (g = the pre-clip norm) to diag_accum[0..3] (device doubles,
+ * the HRL_DIAG_GNORM .. HRL_DIAG_STEPS entries of a diagnostics accumulator) -- in the same launch. */
+int hrl_clip_adam_step_diag(float *param, const float *grad, float *exp_avg, float *exp_avg_sq,
+                            int64_t n, const float *partials, const float *lr, int64_t *step,
+                            double max_norm, double beta1, double beta2, double eps, double weight_decay,
+                            float *grad_norm_out /* may be NULL */, double *diag_accum, void *stream);
 
 /*
  * Multi-GPU form of the same step: one-shot all-reduce (SUM) of the flat gradient bucket over NVLink peer
