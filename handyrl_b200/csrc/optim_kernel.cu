@@ -180,6 +180,33 @@ __global__ void __launch_bounds__(kOptThreads) peer_allreduce_sumsq_kernel(
 // reads the same value regardless of scheduling
 __global__ void bump_step_kernel(int64_t *step_p) { *step_p += 1; }
 
+// moving average of the learner's state after the optimiser step: a <- fmaf(w, x - a, a),
+// w = 1 - decay once seeded, else max(1 - decay, 1 / t) with t = *step_p.  w == 1 (the first step)
+// stores x itself: fmaf(1, x - a, a) would round x - a.  Purely elementwise, so every element sees
+// the same arithmetic whatever the grid.
+__device__ __forceinline__ float ema_update(float a, float x, float w) { return w == 1.f ? x : fmaf(w, x - a, a); }
+
+__global__ void __launch_bounds__(kOptThreads) weight_ema_kernel(float *__restrict__ avg, const float *__restrict__ state, int64_t n,
+                                                                 const int64_t *__restrict__ step_p, float decay, int seeded) {
+    const float keep = 1.f - decay;
+    const int64_t t = *step_p;
+    const float w = seeded ? keep : fmaxf(keep, 1.f / (float)(t > 1 ? t : 1));
+    const int64_t n4 = n >> 2;
+    float4 *a4 = reinterpret_cast<float4 *>(avg);
+    const float4 *x4 = reinterpret_cast<const float4 *>(state);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
+        float4 a = a4[i];
+        const float4 x = x4[i];
+        a.x = ema_update(a.x, x.x, w);
+        a.y = ema_update(a.y, x.y, w);
+        a.z = ema_update(a.z, x.z, w);
+        a.w = ema_update(a.w, x.w, w);
+        a4[i] = a;
+    }
+    if (blockIdx.x == 0)
+        for (int64_t i = (n4 << 2) + threadIdx.x; i < n; i += blockDim.x) avg[i] = ema_update(avg[i], state[i], w);
+}
+
 }  // namespace hrl
 
 extern "C" int32_t hrl_sumsq_num_partials(void) { return hrl::kPartials; }
@@ -241,4 +268,21 @@ extern "C" int hrl_clip_adam_step_diag(float *param, const float *grad, float *e
                                        void *stream) {
     return hrl::clip_adam_step<true>("hrl_clip_adam_step_diag", param, grad, exp_avg, exp_avg_sq, n, partials, lr, step,
                                      max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, diag_accum, stream);
+}
+
+extern "C" int hrl_weight_ema(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
+                              void *stream) {
+    using namespace hrl;
+    HRL_REQUIRE(avg && state && step && n > 0, HRL_ERR_BAD_ARG, "hrl_weight_ema: NULL pointer or n <= 0");
+    HRL_REQUIRE(((reinterpret_cast<uintptr_t>(avg) | reinterpret_cast<uintptr_t>(state)) & 15) == 0, HRL_ERR_BAD_ARG,
+                "hrl_weight_ema: avg and state must be 16-byte aligned");
+    HRL_REQUIRE(decay > 0.f && decay < 1.f, HRL_ERR_BAD_ARG, "hrl_weight_ema: decay must lie in (0, 1), got %g", (double)decay);
+    const int64_t n4 = n >> 2;
+    int64_t grid = (n4 + kOptThreads - 1) / kOptThreads;
+    if (grid < 1) grid = 1;                     // n < 4: block 0 does the tail alone
+    if (grid > 4 * kNumSM) grid = 4 * kNumSM;
+    weight_ema_kernel<<<(int)grid, kOptThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(avg, state, n, step, decay,
+                                                                                             seeded ? 1 : 0);
+    HRL_CUDA_CHECK(cudaGetLastError());
+    return HRL_OK;
 }

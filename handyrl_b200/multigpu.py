@@ -137,7 +137,7 @@ def _helper_main(rank, world, port, args, model_blob, lr, conn):
         assert cmds.get()[0] == 'start'                # the backlog has arrived in `episodes`
         batch = Batcher(args, episodes)._make()
         batch = tree_map(lambda t: t[:t.shape[0] // world].contiguous(), batch)
-        stepper = LearnerStep(model, args, batch, lr, device=device, process_group=pg)
+        stepper = LearnerStep(model, args, batch, lr, device=device, process_group=pg, weight_ema=0)   # rank 0 averages
         stepper.warm_up()
         gb = GpuBatcher(args, episodes, device, seed=args.get('seed', 0) * 7919 + 17 + rank)
         gb.run()

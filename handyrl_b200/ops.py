@@ -346,6 +346,21 @@ class FlatAdam:
         fastnet.new_step()          # cached adjoint weights of the convolutions are stale now
 
 
+def weight_ema_update(avg, state_f32, step_count, decay, seeded):
+    """avg <- fmaf(w, state_f32 - avg, avg) in place, w = max(1 - decay, 1 / t) (1 - decay when `seeded`), t = the int64 device
+    counter `step_count` as it stands when the launch runs (hrl_weight_ema, csrc/optim_kernel.cu).  One launch, graph-capturable."""
+    for t, name in ((avg, 'avg'), (state_f32, 'state_f32')):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+            raise _capi.HrlError('handyrl_b200: %s must be a contiguous float32 CUDA tensor' % name)
+    if avg.numel() != state_f32.numel():
+        raise _capi.HrlError('handyrl_b200: avg (%d) and state_f32 (%d) differ in size' % (avg.numel(), state_f32.numel()))
+    if not (step_count.is_cuda and step_count.dtype == torch.int64 and step_count.numel() == 1):
+        raise _capi.HrlError('handyrl_b200: step_count must be a one-element int64 CUDA tensor')
+    check(lib().hrl_weight_ema(_ptr(avg), _ptr(state_f32), avg.numel(), _ptr(step_count), float(decay), int(bool(seeded)),
+                               _stream_ptr()))
+    _count()
+
+
 def gemm_tf32x3(a, b, bias=None, a_kmajor=True, b_kmajor=True, splits=1, out=None):
     """C = A_op @ B_op^T (+ bias) on the tensor cores with fp32-class accuracy (hrl_gemm_tf32x3, csrc/gemm_kernel.cu).
 

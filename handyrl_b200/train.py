@@ -15,6 +15,7 @@ Same public names as handyrl/train.py for the path
 """
 import collections
 import copy
+import numbers
 import os
 import pickle
 import queue
@@ -290,16 +291,63 @@ class StateStore:
                 out[k] = views[tag][off:off + n].clone().view(shape)
         return out
 
+    def averaged_bytes(self, host_avg, host_bytes):
+        """A host image of `bytes` holding the moving average: the fp32 words [0, i_off) are already in `host_avg` (a host
+        buffer of the size of `bytes`), the int64 buffers are taken from the live image `host_bytes`."""
+        host_avg[self.i_off:self.nbytes].copy_(host_bytes[self.i_off:self.nbytes])
+        return host_avg
+
+
+def weight_ema_decay(value):
+    """train_args['weight_ema'] -> the decay of the weights' moving average, or None when averaging is off (key absent, 0 or
+    None).  Anything else outside (0, 1) raises ValueError."""
+    if value is None or (isinstance(value, numbers.Real) and value == 0):
+        return None
+    if not isinstance(value, numbers.Real) or not 0.0 < float(value) < 1.0:
+        raise ValueError("train_args['weight_ema'] must be a decay in (0, 1) (e.g. 0.999), or 0 / None for no averaging; got %r"
+                         % (value,))
+    return float(value)
+
+
+class AveragedCheckpoints:
+    """Files of the moving average of the weights, next to the Learner's checkpoints (reference train.py:441-454):
+    models/<epoch>.ema.pth and models/latest.ema.pth, in the Learner's relative `models` directory, written with torch.save.
+    <epoch> is the number the Learner gives the model handed back with it: restart_epoch + the models handed back so far."""
+
+    def __init__(self, restart_epoch=0, directory='models'):
+        self.directory = directory
+        self.restart_epoch = int(restart_epoch or 0)
+        self.epoch = self.restart_epoch
+
+    def path(self, epoch):
+        return os.path.join(self.directory, '%s.ema.pth' % epoch)
+
+    def seed_path(self):
+        """The average a restarted run resumes from (models/<restart_epoch>.ema.pth), or None."""
+        if self.restart_epoch > 0 and os.path.exists(self.path(self.restart_epoch)):
+            return self.path(self.restart_epoch)
+        return None
+
+    def save(self, state_dict):
+        """Write the average of the next epoch; returns its path."""
+        self.epoch += 1
+        os.makedirs(self.directory, exist_ok=True)
+        torch.save(state_dict, self.path(self.epoch))
+        torch.save(state_dict, self.path('latest'))
+        return self.path(self.epoch)
+
 
 class PendingModel:
     """The model of a finished epoch, still on its way to the host.  `resolve()` (called by Trainer.update() on the
     Learner's thread) waits for the side-stream copy only, prints the epoch's loss line, rebuilds the CPU model in
     eval mode and caches its pickled bytes on it (the Learner pickles the model for every worker request,
-    train.py:605-615)."""
+    train.py:605-615).  With a moving average of the weights (`host_avg`), it also leaves the averaged state_dict, keyed
+    like the model's, in `ema_state`."""
 
-    def __init__(self, stepper, done_event, host_state, host_losses, heads, template):
+    def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host_avg=None):
         self.stepper, self.done, self.host_state, self.host_losses = stepper, done_event, host_state, host_losses
-        self.heads, self.template = heads, template
+        self.heads, self.template, self.host_avg = heads, template, host_avg
+        self.ema_state = None
 
     def resolve(self):
         self.done.synchronize()
@@ -314,9 +362,14 @@ class PendingModel:
             if self.diagnostics is not None:
                 print(ops.format_diagnostics(self.diagnostics))
         tpl = self.template
-        state = self.stepper.state.state_dict_from(self.host_state, tpl.state_dict().keys())
-        for k, b in self.stepper.state.loose:
+        store = self.stepper.state
+        keys = list(tpl.state_dict().keys())
+        state = store.state_dict_from(self.host_state, keys)
+        for k, b in store.loose:
             state[k] = b.detach().cpu()
+        if self.host_avg is not None:           # loose buffers: the live model's
+            avg = store.state_dict_from(store.averaged_bytes(self.host_avg, self.host_state), keys)
+            self.ema_state = collections.OrderedDict((k, avg[k] if k in avg else state[k].clone()) for k in keys)
         tpl.load_state_dict(state)
         tpl.eval()
         blob = pickle.dumps(tpl)
@@ -345,11 +398,19 @@ class LearnerStep:
     (ops.DIAG_KEYS), which ride the gradient bucket behind the loss sums, and the optimiser adds its pre-clip norm
     statistics; both accumulate in `diag_accum` (float64, on the device) until end_epoch / pop_diagnostics.  Losses,
     gradients and weights are the same with and without.
+
+    weight_ema (default: train_args['weight_ema'], off): a decay d in (0, 1).  Every step ends with one more launch that
+    updates a moving average of the fp32 state (parameters and BatchNorm buffers, StateStore bytes [0, i_off)) on the
+    device: a <- a + w (x - a), w = max(1 - d, 1 / t) at optimiser step t, or 1 - d once seeded (seed_weight_ema).
+    end_epoch hands it over with the model (PendingModel.ema_state); ema_state_dict() reads it now.  Training itself is
+    the same with and without.
     """
 
     def __init__(self, model, args, example_batch, lr, device=None, process_group=None, use_graph=True,
                  max_norm=4.0, weight_decay=1e-5, time_loss_kernel=False, channels_last=True, cudnn_benchmark=True,
-                 small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None):
+                 small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None,
+                 weight_ema=None):
+        self.weight_ema = weight_ema_decay(args.get('weight_ema') if weight_ema is None else weight_ema)
         self.device = torch.device(device if device is not None else 'cuda')
         self.args = args
         if diagnostics is None:
@@ -398,6 +459,12 @@ class LearnerStep:
                                 param_storage=self.state.flat_param)
         self.state.index_params(self.model)
         self.state_snap = torch.empty_like(self.state.bytes)
+        self.avg_bytes = self.avg = self.avg_snap = None       # moving average of the fp32 state: a copy of bytes [0, i_off)
+        self.avg_seeded = False
+        if self.weight_ema is not None:
+            self.avg_bytes = self.state.bytes[:self.state.i_off].clone()
+            self.avg = self.avg_bytes.view(torch.float32)
+            self.avg_snap = torch.empty_like(self.avg_bytes)
         self.acc_snap = torch.zeros(n_sums, dtype=torch.float64, device=self.device)
         self.copy_stream = torch.cuda.Stream(device=self.device)
         self._handoff_slots = None
@@ -504,6 +571,9 @@ class LearnerStep:
         self.loss_accum.add_(self.last_losses)
         if self.diagnostics:
             self.diag_accum[:NUM_LOSS_DIAG].add_(tail[NUM_LOSS:NUM_LOSS + NUM_LOSS_DIAG])
+        if self.avg is not None:        # after the optimiser: step_count already counts this step
+            ops.weight_ema_update(self.avg, self.state.bytes[:self.state.i_off].view(torch.float32), self.opt.step_count,
+                                  self.weight_ema, self.avg_seeded)
 
     def _device_step(self):
         self._part_forward()
@@ -543,10 +613,10 @@ class LearnerStep:
     def _snapshot(self):
         bufs = {k: v.clone() for k, v in self.model.state_dict().items()}
         return (bufs, self.opt.exp_avg.clone(), self.opt.exp_avg_sq.clone(), self.opt.step_count.clone(),
-                self.accum.clone())
+                self.accum.clone(), self.avg.clone() if self.avg is not None else None)
 
     def _restore(self, state):
-        bufs, m, v, sc, acc = state
+        bufs, m, v, sc, acc, avg = state
         with torch.no_grad():
             for k, t in self.model.state_dict().items():
                 t.copy_(bufs[k])
@@ -554,6 +624,8 @@ class LearnerStep:
             self.opt.exp_avg_sq.copy_(v)
             self.opt.step_count.copy_(sc)
             self.accum.copy_(acc)
+            if avg is not None:
+                self.avg.copy_(avg)
 
     def new_packed(self):
         return PackedBatch(self.layout)
@@ -675,12 +747,50 @@ class LearnerStep:
     def cpu_state_dict(self):
         """Blocking copy of the model's state_dict to the host (tests, checkpoints)."""
         self.stream.synchronize()
-        host = self.state.bytes.cpu()
+        return self._state_dict_of(self.state.bytes.cpu())
+
+    def _state_dict_of(self, host):
         keys = [k for k in self.model.state_dict().keys() if not k.endswith('_sel_cache')]
         out = self.state.state_dict_from(host, keys)
         for k, b in self.state.loose:
             out[k] = b.detach().cpu().clone()
         return {k: out[k] for k in keys}
+
+    def _require_average(self):
+        if self.avg is None:
+            raise RuntimeError('LearnerStep was built without a weight average (train_args["weight_ema"] / weight_ema=decay)')
+
+    def ema_state_dict(self):
+        """Blocking copy of the moving average of the weights to the host, keyed like cpu_state_dict(); the int64 buffers
+        and the buffers StateStore keeps outside its allocation are the live model's."""
+        self._require_average()
+        self.stream.synchronize()
+        host = self.state.bytes.cpu()
+        host[:self.state.i_off] = self.avg_bytes.cpu()
+        return self._state_dict_of(host)
+
+    def seed_weight_ema(self, state_dict):
+        """Start the average from a saved one (a CPU state_dict keyed like the model's, e.g. a <epoch>.ema.pth file): its fp32
+        entries replace the average, and every later step weighs the live weights with 1 - decay.  Call it before the first
+        step (or warm_up), which fixes the captured launch."""
+        self._require_average()
+        if getattr(self, '_captured', False):
+            raise RuntimeError('seed_weight_ema must come before the first step / warm_up()')
+        store = self.state
+        views = {'p': self.avg[:store.n_pad], 'f': self.avg[store.f_off // 4:]}
+        fp32 = [k for k, (tag, _, _) in store.where.items() if tag in views]
+        missing = [k for k in fp32 if k not in state_dict]
+        if missing:
+            raise KeyError('seed_weight_ema: the state_dict lacks %s' % ', '.join(missing))
+        with torch.no_grad():
+            for k in fp32:
+                tag, off, shape = store.where[k]
+                src = torch.as_tensor(state_dict[k])
+                if tuple(src.shape) != shape:
+                    raise ValueError('seed_weight_ema: %s has shape %s, the model %s' % (k, tuple(src.shape), shape))
+                n = src.numel()
+                views[tag][off:off + n].copy_(src.reshape(-1).to(torch.float32))
+        self.avg_seeded = True
 
     def epoch_schedule(self, batch_cnt, steps, default_lr):
         """Device half of the epoch boundary, on the current stream: move the epoch's loss sums aside and apply the
@@ -698,27 +808,34 @@ class LearnerStep:
         sums and the whole model state device-to-device, apply the learning-rate schedule ON THE DEVICE
         (data_cnt_ema <- 0.8 ema + 0.2 dcnt/(0.01+batch_cnt); lr <- 3e-8 ema/(1+steps 1e-5), train.py:382-384 -- dcnt is
         the all-reduced global count) and let a side stream carry the snapshot to pinned host memory while the
-        next epoch's steps already run.  Returns a PendingModel."""
+        next epoch's steps already run.  Returns a PendingModel (with the moving average of the weights, when there is one,
+        snapshot and copied the same way)."""
         if self._handoff_slots is None:
             self._handoff_slots = [(torch.empty(self.state.bytes.numel(), dtype=torch.uint8).pin_memory(),
-                                    torch.zeros(self.acc_snap.numel(), dtype=torch.float64).pin_memory()) for _ in range(2)]
-        host_state, host_losses = self._handoff_slots[self._handoff_i % 2]
+                                    torch.zeros(self.acc_snap.numel(), dtype=torch.float64).pin_memory(),
+                                    torch.empty(self.state.bytes.numel(), dtype=torch.uint8).pin_memory()
+                                    if self.avg is not None else None) for _ in range(2)]
+        host_state, host_losses, host_avg = self._handoff_slots[self._handoff_i % 2]
         self._handoff_i += 1
         with torch.cuda.stream(self.stream):
             self.epoch_schedule(batch_cnt, steps, default_lr)
             if getattr(self, '_last_done', None) is not None:
                 self.stream.wait_event(self._last_done)          # the previous snapshot has left the device buffer
             self.state_snap.copy_(self.state.bytes)
+            if self.avg is not None:
+                self.avg_snap.copy_(self.avg_bytes)
             ready = torch.cuda.Event()
             ready.record(self.stream)
         with torch.cuda.stream(self.copy_stream):
             self.copy_stream.wait_event(ready)
             host_state.copy_(self.state_snap, non_blocking=True)
             host_losses.copy_(self.acc_snap, non_blocking=True)
+            if self.avg is not None:
+                host_avg[:self.state.i_off].copy_(self.avg_snap, non_blocking=True)
             done = torch.cuda.Event()
             done.record(self.copy_stream)
         self._last_done = done
-        return PendingModel(self, done, host_state, host_losses, heads, template)
+        return PendingModel(self, done, host_state, host_losses, heads, template, host_avg=host_avg)
 
 
 # --------------------------------------------------------------------------- batcher + trainer
@@ -1026,9 +1143,16 @@ class Trainer:
     Multi-GPU (the reference wraps its model in nn.DataParallel when it sees several GPUs, train.py:325, 339-340):
     with train_args['num_gpus'] > 1 (default: every visible GPU, as the reference) this process is rank 0 and spawns
     one helper process per further GPU (multigpu.py); every rank holds the whole replay, samples batch_size/num_gpus
-    windows per step and the gradient bucket is all-reduced (SUM) inside the captured step."""
+    windows per step and the gradient bucket is all-reduced (SUM) inside the captured step.
+
+    train_args['weight_ema'] = d in (0, 1): the learner also keeps a moving average of the weights (LearnerStep), and
+    update() writes it to models/<epoch>.ema.pth and models/latest.ema.pth (AveragedCheckpoints) beside the Learner's
+    checkpoints; a run restarted at restart_epoch resumes from models/<restart_epoch>.ema.pth when that file exists.  The
+    returned model is the live one either way."""
 
     def __init__(self, args, model):
+        self.weight_ema = weight_ema_decay(args.get('weight_ema'))
+        self.ema_files = AveragedCheckpoints(args.get('restart_epoch', 0)) if self.weight_ema is not None else None
         self.episodes = EpisodeDeque()
         self.args = args
         self.model = model
@@ -1067,6 +1191,8 @@ class Trainer:
             model, sums = item.resolve()
             if sums['dcnt'] > 0:           # train.py:357: an epoch needs at least one sample with a turn in it
                 break
+        if self.ema_files is not None and item.ema_state is not None:
+            self.ema_files.save(item.ema_state)
         # host mirrors of the schedule the device applied (train.py:382-384), for inspection / logging
         self.data_cnt_ema = self.data_cnt_ema * 0.8 + sums['dcnt'] / (1e-2 + item.batch_cnt) * 0.2
         self.lr = self.default_lr * self.data_cnt_ema / (1 + steps * 1e-5)
@@ -1084,6 +1210,9 @@ class Trainer:
             self.fleet = multigpu.Fleet(self.world, self.args, self.cpu_template, list(self.episodes), self.lr)
             pg = self.fleet.process_group
         self.stepper = LearnerStep(self.model, self.args, batch, self.lr, process_group=pg)
+        seed = self.ema_files.seed_path() if self.ema_files is not None else None
+        if seed is not None:
+            self.stepper.seed_weight_ema(torch.load(seed, map_location='cpu'))
         self.stepper.warm_up()
         self.batcher.pool = [self.stepper.new_packed() for _ in range(4)]
         if self.gpu_replay:

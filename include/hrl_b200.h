@@ -17,6 +17,8 @@
  *   hrl_grad_sumsq /
  *   hrl_clip_adam_step    <- handyrl/train.py:370-371 (clip_grad_norm_(params, 4.0) + Adam.step,
  *                            Adam(lr, weight_decay=1e-5) of train.py:331)
+ *   hrl_weight_ema        <- a per-step moving average of the weights; no reference counterpart (scripts/aux_swa.py
+ *                            averages epoch checkpoints)
  *   hrl_gather_pad        <- handyrl/train.py:33-124  (make_batch: window slice + pad + collate)
  *   hrl_gemm_tf32x3       <- the Linear/Conv contractions of the user's net inside train.py:142-146 (+ autograd, :369)
  *
@@ -206,6 +208,18 @@ int hrl_clip_adam_step_diag(float *param, const float *grad, float *exp_avg, flo
                             int64_t n, const float *partials, const float *lr, int64_t *step,
                             double max_norm, double beta1, double beta2, double eps, double weight_decay,
                             float *grad_norm_out /* may be NULL */, double *diag_accum, void *stream);
+
+/*
+ * Moving average of the learner's weights (opt-in, no reference counterpart; reference scripts/aux_swa.py averages
+ * epoch checkpoints instead).  Enqueued after the optimiser step, on the n fp32 words of the learner's state -- the
+ * parameters (zero pad included) and the fp32 buffers (BatchNorm running statistics):
+ *     avg[i] <- fmaf(w, state[i] - avg[i], avg[i]),   w = max(1 - decay, 1 / t)   (fp32),   t = *step
+ * where *step is the optimiser's step counter after this step's increment (hrl_clip_adam_step), read on the device so
+ * that a captured CUDA graph replays correctly.  The first step (t = 1, w = 1) stores state[i] exactly and early steps
+ * form an equal running mean; seeded != 0 (an average resumed from a saved one) uses w = 1 - decay from its first step.  Elementwise and
+ * deterministic; avg and state 16-byte aligned, any n > 0, decay in (0, 1).
+ */
+int hrl_weight_ema(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded, void *stream);
 
 /*
  * Multi-GPU form of the same step: one-shot all-reduce (SUM) of the flat gradient bucket over NVLink peer
