@@ -106,8 +106,9 @@ def _init_group(rank, world, port):
     return dist.group.WORLD
 
 
-def _helper_main(rank, world, port, args, model_blob, lr, conn):
-    """Body of a helper rank (own process, own GPU)."""
+def _helper_main(rank, world, port, args, model_blob, lr, conn, optim_state=None):
+    """Body of a helper rank (own process, own GPU).  `optim_state`: the optimiser state rank 0 resumes from (an
+    OptimizerStateFormat dict, replicated on every rank), or None."""
     try:
         from .train import Batcher, EpisodeDeque, GpuBatcher, LearnerStep
         from .batch import tree_map
@@ -137,7 +138,10 @@ def _helper_main(rank, world, port, args, model_blob, lr, conn):
         assert cmds.get()[0] == 'start'                # the backlog has arrived in `episodes`
         batch = Batcher(args, episodes)._make()
         batch = tree_map(lambda t: t[:t.shape[0] // world].contiguous(), batch)
-        stepper = LearnerStep(model, args, batch, lr, device=device, process_group=pg, weight_ema=0)   # rank 0 averages
+        # rank 0 averages and writes the optimiser state
+        stepper = LearnerStep(model, args, batch, lr, device=device, process_group=pg, weight_ema=0, save_optimizer=False)
+        if optim_state is not None:
+            stepper.load_optimizer_state(optim_state)
         stepper.warm_up()
         gb = GpuBatcher(args, episodes, device, seed=args.get('seed', 0) * 7919 + 17 + rank)
         gb.run()
@@ -175,9 +179,10 @@ def _helper_main(rank, world, port, args, model_blob, lr, conn):
 
 
 class Fleet:
-    """Rank 0's handle on the helper ranks."""
+    """Rank 0's handle on the helper ranks.  `optim_state` (an OptimizerStateFormat dict, or None) is the optimiser state
+    every helper loads before its first step."""
 
-    def __init__(self, world, args, template, backlog, lr):
+    def __init__(self, world, args, template, backlog, lr, optim_state=None):
         import torch.multiprocessing as mp
         self.world = world
         self.args = args
@@ -188,7 +193,7 @@ class Fleet:
         self.conns, self.procs = [], []
         for r in range(1, world):
             parent, child = ctx.Pipe()
-            p = ctx.Process(target=_helper_main, args=(r, world, port, plain_args, blob, lr, child), daemon=True)
+            p = ctx.Process(target=_helper_main, args=(r, world, port, plain_args, blob, lr, child, optim_state), daemon=True)
             p.start()
             self.conns.append(parent)
             self.procs.append(p)

@@ -310,31 +310,134 @@ def weight_ema_decay(value):
 
 
 class AveragedCheckpoints:
-    """Files of the moving average of the weights, next to the Learner's checkpoints (reference train.py:441-454):
-    models/<epoch>.ema.pth and models/latest.ema.pth, in the Learner's relative `models` directory, written with torch.save.
-    <epoch> is the number the Learner gives the model handed back with it: restart_epoch + the models handed back so far."""
+    """Files written next to the Learner's checkpoints (reference train.py:441-454): models/<epoch>.<suffix>.pth and
+    models/latest.<suffix>.pth, in the Learner's relative `models` directory, written with torch.save.  <epoch> is the number
+    the Learner gives the model handed back with them: restart_epoch + the models handed back so far.  One object numbers
+    every kind of file (the moving average of the weights, 'ema'; the optimiser state, 'optim'), so the files of one epoch
+    share <epoch>.  `suffix` is the kind path(), seed_path() and save() use when not told otherwise."""
 
-    def __init__(self, restart_epoch=0, directory='models'):
+    def __init__(self, restart_epoch=0, directory='models', suffix='ema'):
         self.directory = directory
+        self.suffix = suffix
         self.restart_epoch = int(restart_epoch or 0)
         self.epoch = self.restart_epoch
 
-    def path(self, epoch):
-        return os.path.join(self.directory, '%s.ema.pth' % epoch)
+    def path(self, epoch, suffix=None):
+        return os.path.join(self.directory, '%s.%s.pth' % (epoch, suffix or self.suffix))
 
-    def seed_path(self):
-        """The average a restarted run resumes from (models/<restart_epoch>.ema.pth), or None."""
-        if self.restart_epoch > 0 and os.path.exists(self.path(self.restart_epoch)):
-            return self.path(self.restart_epoch)
+    def seed_path(self, suffix=None):
+        """The file of this kind a restarted run resumes from (models/<restart_epoch>.<suffix>.pth), or None."""
+        if self.restart_epoch > 0 and os.path.exists(self.path(self.restart_epoch, suffix)):
+            return self.path(self.restart_epoch, suffix)
         return None
 
     def save(self, state_dict):
-        """Write the average of the next epoch; returns its path."""
+        """Write the file of the default kind for the next epoch; returns its path."""
+        return self.save_epoch({self.suffix: state_dict})[self.suffix]
+
+    def save_epoch(self, files):
+        """Write the files of the next epoch, {suffix: object to torch.save}; returns {suffix: path}."""
         self.epoch += 1
-        os.makedirs(self.directory, exist_ok=True)
-        torch.save(state_dict, self.path(self.epoch))
-        torch.save(state_dict, self.path('latest'))
-        return self.path(self.epoch)
+        if files:
+            os.makedirs(self.directory, exist_ok=True)
+        for suffix, obj in files.items():
+            torch.save(obj, self.path(self.epoch, suffix))
+            torch.save(obj, self.path('latest', suffix))
+        return {suffix: self.path(self.epoch, suffix) for suffix in files}
+
+
+class OptimizerStateFormat:
+    """The learner's optimiser state as a plain dict that loads without this package:
+
+        {'optimizer': what torch.optim.Adam(net.parameters(), lr, betas, eps, weight_decay).state_dict() holds after a step:
+                      'state': {i: {'step', 'exp_avg', 'exp_avg_sq'}} shaped like parameter i, 'param_groups': [one group],
+         'param_names': [names in net.named_parameters() order],
+         'schedule': {'steps': int, 'data_cnt_ema': float, 'lr': float},
+         'max_norm': float}
+
+    Parameter i is the i-th of net.parameters(), words [off_i, off_i + numel_i) of FlatAdam's flat buckets; the words from n
+    up to n_pad are padding, not part of the format, and zero after a load.  'step' is the number of optimiser steps taken
+    (FlatAdam.step_count), a float32 tensor as torch keeps it.  'schedule' holds what the next step uses: the learning rate
+    and the data-count average it came from (the device's float32 values), and the step count it was scheduled at."""
+
+    def __init__(self, named_params, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-5, max_norm=4.0):
+        self.names, self.shapes, self.offsets = [], [], []
+        off = 0
+        for k, p in named_params:
+            self.names.append(k)
+            self.shapes.append(tuple(p.shape))
+            self.offsets.append(off)
+            off += p.numel()
+        self.n = off
+        self.n_pad = (off + 3) // 4 * 4
+        self.betas = (float(betas[0]), float(betas[1]))
+        self.eps, self.weight_decay, self.max_norm = float(eps), float(weight_decay), float(max_norm)
+
+    def _spans(self):
+        for name, shape, off in zip(self.names, self.shapes, self.offsets):
+            n = 1
+            for d in shape:
+                n *= d
+            yield name, shape, off, n
+
+    def to_dict(self, exp_avg, exp_avg_sq, step, lr, data_cnt_ema, steps):
+        """The dict of flat CPU moments (at least n words each), the step count and the schedule; fresh storage per tensor."""
+        dummies = [torch.zeros(1, requires_grad=True) for _ in self.names]       # the param group exactly as torch writes it
+        groups = torch.optim.Adam(dummies, lr=float(lr), betas=self.betas, eps=self.eps,
+                                  weight_decay=self.weight_decay).state_dict()['param_groups']
+        state = {}
+        for i, (_, shape, off, n) in enumerate(self._spans()):
+            state[i] = {'step': torch.tensor(float(step), dtype=torch.float32),
+                        'exp_avg': exp_avg[off:off + n].clone().view(shape),
+                        'exp_avg_sq': exp_avg_sq[off:off + n].clone().view(shape)}
+        return {'optimizer': {'state': state, 'param_groups': groups},
+                'param_names': list(self.names),
+                'schedule': {'steps': int(steps), 'data_cnt_ema': float(data_cnt_ema), 'lr': float(lr)},
+                'max_norm': self.max_norm}
+
+    def unpack(self, d):
+        """Check a dict of this format against the net and the optimiser's settings and return its flat form
+        (exp_avg, exp_avg_sq: float32 CPU tensors of n_pad words with zero padding; step; lr; data_cnt_ema; steps).
+        Raises KeyError (an entry or a parameter name missing or extra) or ValueError (a shape, betas, eps, weight_decay or
+        max_norm that differs)."""
+        for key in ('optimizer', 'param_names', 'schedule', 'max_norm'):
+            if key not in d:
+                raise KeyError('optimiser state: no %r entry' % key)
+        names = list(d['param_names'])
+        missing = [k for k in self.names if k not in names]
+        extra = [k for k in names if k not in self.names]
+        if missing or extra or len(names) != len(self.names):
+            raise KeyError('optimiser state: parameter names differ from the net\'s (missing: %s; extra or repeated: %s)'
+                           % (', '.join(missing) or '-', ', '.join(extra) or '-'))
+        groups = d['optimizer']['param_groups']
+        if len(groups) != 1:
+            raise ValueError('optimiser state: %d parameter groups, the learner has one' % len(groups))
+        group = groups[0]
+        got = {'betas': tuple(float(b) for b in group['betas']), 'eps': float(group['eps']),
+               'weight_decay': float(group['weight_decay']), 'max_norm': float(d['max_norm'])}
+        want = {'betas': self.betas, 'eps': self.eps, 'weight_decay': self.weight_decay, 'max_norm': self.max_norm}
+        for key in want:
+            if got[key] != want[key]:
+                raise ValueError('optimiser state: %s is %r, the learner\'s %r' % (key, got[key], want[key]))
+        state = d['optimizer']['state']
+        index = {k: i for i, k in enumerate(names)}
+        m, v = torch.zeros(self.n_pad), torch.zeros(self.n_pad)
+        steps_seen = set()
+        for name, shape, off, n in self._spans():
+            s = state.get(index[name])
+            if s is None:
+                raise KeyError('optimiser state: no state for parameter %d (%s)' % (index[name], name))
+            for key, flat in (('exp_avg', m), ('exp_avg_sq', v)):
+                src = torch.as_tensor(s[key])
+                if tuple(src.shape) != shape:
+                    raise ValueError('optimiser state: %s of %s has shape %s, the parameter %s'
+                                     % (key, name, tuple(src.shape), shape))
+                flat[off:off + n] = src.reshape(-1).to(torch.float32)
+            steps_seen.add(float(s['step']))
+        if len(steps_seen) != 1:
+            raise ValueError('optimiser state: the parameters have different step counts %s' % sorted(steps_seen))
+        sched = d['schedule']
+        return m, v, int(round(steps_seen.pop())), float(group['lr']), float(sched['data_cnt_ema']), int(sched['steps'])
 
 
 class PendingModel:
@@ -342,12 +445,16 @@ class PendingModel:
     Learner's thread) waits for the side-stream copy only, prints the epoch's loss line, rebuilds the CPU model in
     eval mode and caches its pickled bytes on it (the Learner pickles the model for every worker request,
     train.py:605-615).  With a moving average of the weights (`host_avg`), it also leaves the averaged state_dict, keyed
-    like the model's, in `ema_state`."""
+    like the model's, in `ema_state`; with the optimiser state (`host_optim`, LearnerStep.end_epoch's layout), it leaves
+    that state in the OptimizerStateFormat dict in `optim_state`, scheduled at step count `steps`."""
 
-    def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host_avg=None):
+    def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host_avg=None, host_optim=None,
+                 steps=0):
         self.stepper, self.done, self.host_state, self.host_losses = stepper, done_event, host_state, host_losses
         self.heads, self.template, self.host_avg = heads, template, host_avg
+        self.host_optim, self.steps = host_optim, steps
         self.ema_state = None
+        self.optim_state = None
 
     def resolve(self):
         self.done.synchronize()
@@ -370,6 +477,8 @@ class PendingModel:
         if self.host_avg is not None:           # loose buffers: the live model's
             avg = store.state_dict_from(store.averaged_bytes(self.host_avg, self.host_state), keys)
             self.ema_state = collections.OrderedDict((k, avg[k] if k in avg else state[k].clone()) for k in keys)
+        if self.host_optim is not None:
+            self.optim_state = self.stepper.optimizer_state_from(self.host_optim, self.steps)
         tpl.load_state_dict(state)
         tpl.eval()
         blob = pickle.dumps(tpl)
@@ -404,13 +513,20 @@ class LearnerStep:
     device: a <- a + w (x - a), w = max(1 - d, 1 / t) at optimiser step t, or 1 - d once seeded (seed_weight_ema).
     end_epoch hands it over with the model (PendingModel.ema_state); ema_state_dict() reads it now.  Training itself is
     the same with and without.
+
+    save_optimizer (default: train_args['save_optimizer'], off): end_epoch also hands over the optimiser state the next
+    step uses (Adam's moments and step count, the learning rate and the data-count average of its schedule) in the
+    OptimizerStateFormat dict (PendingModel.optim_state), by the same device-to-device snapshot and side-stream copy as the
+    model.  optimizer_state_dict() reads it now; load_optimizer_state() resumes from it.  The step itself is the same with
+    and without.
     """
 
     def __init__(self, model, args, example_batch, lr, device=None, process_group=None, use_graph=True,
                  max_norm=4.0, weight_decay=1e-5, time_loss_kernel=False, channels_last=True, cudnn_benchmark=True,
                  small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None,
-                 weight_ema=None):
+                 weight_ema=None, save_optimizer=None):
         self.weight_ema = weight_ema_decay(args.get('weight_ema') if weight_ema is None else weight_ema)
+        self.save_optimizer = bool(args.get('save_optimizer', False) if save_optimizer is None else save_optimizer)
         self.device = torch.device(device if device is not None else 'cuda')
         self.args = args
         if diagnostics is None:
@@ -458,6 +574,9 @@ class LearnerStep:
                                 grad_alloc=self.peer.alloc if self.peer is not None else None,
                                 param_storage=self.state.flat_param)
         self.state.index_params(self.model)
+        self.optim_format = OptimizerStateFormat(self.model.named_parameters(), betas=self.opt.betas, eps=self.opt.eps,
+                                                 weight_decay=weight_decay, max_norm=max_norm)
+        self.schedule_steps = 0          # the step count the current learning rate was scheduled at
         self.state_snap = torch.empty_like(self.state.bytes)
         self.avg_bytes = self.avg = self.avg_snap = None       # moving average of the fp32 state: a copy of bytes [0, i_off)
         self.avg_seeded = False
@@ -474,6 +593,10 @@ class LearnerStep:
         self.launches_per_step = 0
         self.ema = torch.full((1,), float(example_batch['action'].shape[0] * args.get('forward_steps', 1)) * self.world,
                               dtype=torch.float32, device=self.device)
+        # optimiser state of the epoch hand-off: [exp_avg | exp_avg_sq (n_pad fp32 each) | step_count (int64) | lr | ema (fp32)]
+        self.optim_snap = None
+        if self.save_optimizer:
+            self.optim_snap = torch.empty(8 * self.opt.n_pad + 16, dtype=torch.uint8, device=self.device)
 
         self.layout = BatchLayout(example_batch)
         self.dev_buffer = torch.zeros(self.layout.nbytes, dtype=torch.uint8, device=self.device)
@@ -792,6 +915,40 @@ class LearnerStep:
                 views[tag][off:off + n].copy_(src.reshape(-1).to(torch.float32))
         self.avg_seeded = True
 
+    def _optim_views(self, buf):
+        """(exp_avg, exp_avg_sq, step_count, lr, ema) views of a byte buffer in the optim_snap layout."""
+        n4 = 4 * self.opt.n_pad
+        return (buf[:n4].view(torch.float32), buf[n4:2 * n4].view(torch.float32), buf[2 * n4:2 * n4 + 8].view(torch.int64),
+                buf[2 * n4 + 8:2 * n4 + 12].view(torch.float32), buf[2 * n4 + 12:2 * n4 + 16].view(torch.float32))
+
+    def optimizer_state_from(self, host_optim, steps):
+        """The OptimizerStateFormat dict of a host copy of optim_snap, scheduled at step count `steps`."""
+        m, v, sc, lr, ema = self._optim_views(host_optim)
+        return self.optim_format.to_dict(m, v, int(sc[0]), float(lr[0]), float(ema[0]), steps)
+
+    def optimizer_state_dict(self):
+        """Blocking copy of the optimiser state the next step uses, in the OptimizerStateFormat dict (what end_epoch hands
+        over as PendingModel.optim_state)."""
+        self.stream.synchronize()
+        return self.optim_format.to_dict(self.opt.exp_avg.cpu(), self.opt.exp_avg_sq.cpu(), int(self.opt.step_count.item()),
+                                         float(self.opt.lr.item()), float(self.ema.item()), self.schedule_steps)
+
+    def load_optimizer_state(self, d):
+        """Resume from an OptimizerStateFormat dict (e.g. a <epoch>.optim.pth file): Adam's moments and step count, the
+        learning rate and the data-count average.  Call it before the first step (or warm_up), which snapshots the state
+        around the capture's warm-up steps.  A dict whose parameter names or shapes differ from the net's, or whose betas,
+        eps, weight_decay or max_norm differ from this learner's, raises KeyError / ValueError and changes nothing."""
+        if getattr(self, '_captured', False):
+            raise RuntimeError('load_optimizer_state must come before the first step / warm_up()')
+        m, v, step, lr, data_cnt_ema, steps = self.optim_format.unpack(d)
+        with torch.no_grad():
+            self.opt.exp_avg.copy_(m)
+            self.opt.exp_avg_sq.copy_(v)
+            self.opt.step_count.fill_(step)
+            self.opt.lr.fill_(lr)
+            self.ema.fill_(data_cnt_ema)
+        self.schedule_steps = steps
+
     def epoch_schedule(self, batch_cnt, steps, default_lr):
         """Device half of the epoch boundary, on the current stream: move the epoch's loss sums aside and apply the
         learning-rate schedule from the (all-reduced, hence global) data count.  Every rank of a sharded learner
@@ -802,20 +959,24 @@ class LearnerStep:
         fresh = self.ema * 0.8 + dcnt * (0.2 / (1e-2 + batch_cnt))
         self.ema.copy_(torch.where(dcnt > 0, fresh, self.ema))
         self.opt.lr.copy_(self.ema * (default_lr / (1 + steps * 1e-5)))
+        self.schedule_steps = int(steps)
 
     def end_epoch(self, batch_cnt, steps, default_lr, template, heads):
         """Epoch boundary without a host synchronisation (train.py:378-387): on the step stream, snapshot the loss
         sums and the whole model state device-to-device, apply the learning-rate schedule ON THE DEVICE
         (data_cnt_ema <- 0.8 ema + 0.2 dcnt/(0.01+batch_cnt); lr <- 3e-8 ema/(1+steps 1e-5), train.py:382-384 -- dcnt is
         the all-reduced global count) and let a side stream carry the snapshot to pinned host memory while the
-        next epoch's steps already run.  Returns a PendingModel (with the moving average of the weights, when there is one,
-        snapshot and copied the same way)."""
+        next epoch's steps already run.  Returns a PendingModel (with the moving average of the weights and the optimiser
+        state, when they are kept, snapshot and copied the same way; the optimiser state is taken after the schedule, i.e.
+        as the next step uses it)."""
         if self._handoff_slots is None:
             self._handoff_slots = [(torch.empty(self.state.bytes.numel(), dtype=torch.uint8).pin_memory(),
                                     torch.zeros(self.acc_snap.numel(), dtype=torch.float64).pin_memory(),
                                     torch.empty(self.state.bytes.numel(), dtype=torch.uint8).pin_memory()
-                                    if self.avg is not None else None) for _ in range(2)]
-        host_state, host_losses, host_avg = self._handoff_slots[self._handoff_i % 2]
+                                    if self.avg is not None else None,
+                                    torch.empty(self.optim_snap.numel(), dtype=torch.uint8).pin_memory()
+                                    if self.optim_snap is not None else None) for _ in range(2)]
+        host_state, host_losses, host_avg, host_optim = self._handoff_slots[self._handoff_i % 2]
         self._handoff_i += 1
         with torch.cuda.stream(self.stream):
             self.epoch_schedule(batch_cnt, steps, default_lr)
@@ -824,6 +985,10 @@ class LearnerStep:
             self.state_snap.copy_(self.state.bytes)
             if self.avg is not None:
                 self.avg_snap.copy_(self.avg_bytes)
+            if self.optim_snap is not None:
+                for dst, src in zip(self._optim_views(self.optim_snap),
+                                    (self.opt.exp_avg, self.opt.exp_avg_sq, self.opt.step_count, self.opt.lr, self.ema)):
+                    dst.copy_(src)
             ready = torch.cuda.Event()
             ready.record(self.stream)
         with torch.cuda.stream(self.copy_stream):
@@ -832,10 +997,13 @@ class LearnerStep:
             host_losses.copy_(self.acc_snap, non_blocking=True)
             if self.avg is not None:
                 host_avg[:self.state.i_off].copy_(self.avg_snap, non_blocking=True)
+            if self.optim_snap is not None:
+                host_optim.copy_(self.optim_snap, non_blocking=True)
             done = torch.cuda.Event()
             done.record(self.copy_stream)
         self._last_done = done
-        return PendingModel(self, done, host_state, host_losses, heads, template, host_avg=host_avg)
+        return PendingModel(self, done, host_state, host_losses, heads, template, host_avg=host_avg, host_optim=host_optim,
+                            steps=int(steps))
 
 
 # --------------------------------------------------------------------------- batcher + trainer
@@ -1148,11 +1316,21 @@ class Trainer:
     train_args['weight_ema'] = d in (0, 1): the learner also keeps a moving average of the weights (LearnerStep), and
     update() writes it to models/<epoch>.ema.pth and models/latest.ema.pth (AveragedCheckpoints) beside the Learner's
     checkpoints; a run restarted at restart_epoch resumes from models/<restart_epoch>.ema.pth when that file exists.  The
-    returned model is the live one either way."""
+    returned model is the live one either way.
+
+    train_args['save_optimizer'] = True: update() also writes the optimiser state and learning-rate schedule the next step
+    uses to models/<epoch>.optim.pth and models/latest.optim.pth (OptimizerStateFormat), numbered by the same
+    AveragedCheckpoints as the averages; a run restarted at restart_epoch resumes Adam's moments and step count, the
+    learning rate, the data-count average and `steps` from models/<restart_epoch>.optim.pth when that file exists."""
 
     def __init__(self, args, model):
         self.weight_ema = weight_ema_decay(args.get('weight_ema'))
-        self.ema_files = AveragedCheckpoints(args.get('restart_epoch', 0)) if self.weight_ema is not None else None
+        self.save_optimizer = bool(args.get('save_optimizer', False))
+        self.checkpoint_files = None         # numbers the .ema.pth and .optim.pth files of one epoch alike
+        if self.weight_ema is not None or self.save_optimizer:
+            self.checkpoint_files = AveragedCheckpoints(args.get('restart_epoch', 0))
+        self.ema_files = self.checkpoint_files if self.weight_ema is not None else None
+        self.optim_files = self.checkpoint_files if self.save_optimizer else None
         self.episodes = EpisodeDeque()
         self.args = args
         self.model = model
@@ -1191,8 +1369,13 @@ class Trainer:
             model, sums = item.resolve()
             if sums['dcnt'] > 0:           # train.py:357: an epoch needs at least one sample with a turn in it
                 break
-        if self.ema_files is not None and item.ema_state is not None:
-            self.ema_files.save(item.ema_state)
+        if self.checkpoint_files is not None:
+            files = {}
+            if self.ema_files is not None and item.ema_state is not None:
+                files['ema'] = item.ema_state
+            if self.optim_files is not None and item.optim_state is not None:
+                files['optim'] = item.optim_state
+            self.checkpoint_files.save_epoch(files)
         # host mirrors of the schedule the device applied (train.py:382-384), for inspection / logging
         self.data_cnt_ema = self.data_cnt_ema * 0.8 + sums['dcnt'] / (1e-2 + item.batch_cnt) * 0.2
         self.lr = self.default_lr * self.data_cnt_ema / (1 + steps * 1e-5)
@@ -1203,13 +1386,26 @@ class Trainer:
         batch = self._first_host_batch()
         self.cpu_template = copy.deepcopy(self.model)
         self.cpu_template.eval()
+        optim_state = None
+        if self.optim_files is not None and self.optim_files.restart_epoch > 0:
+            path = self.optim_files.seed_path('optim')
+            if path is not None:
+                optim_state = torch.load(path, map_location='cpu')
+                sched = optim_state['schedule']         # before the helper ranks spawn: they start at self.lr
+                self.steps, self.data_cnt_ema, self.lr = int(sched['steps']), float(sched['data_cnt_ema']), float(sched['lr'])
+            else:
+                print('handyrl_b200: no %s, the optimiser state starts fresh'
+                      % self.optim_files.path(self.optim_files.restart_epoch, 'optim'))
         pg = None
         if self.world > 1:
             from . import multigpu
             batch = tree_map(lambda t: t[:t.shape[0] // self.world].contiguous(), batch)
-            self.fleet = multigpu.Fleet(self.world, self.args, self.cpu_template, list(self.episodes), self.lr)
+            self.fleet = multigpu.Fleet(self.world, self.args, self.cpu_template, list(self.episodes), self.lr,
+                                        optim_state=optim_state)
             pg = self.fleet.process_group
         self.stepper = LearnerStep(self.model, self.args, batch, self.lr, process_group=pg)
+        if optim_state is not None:
+            self.stepper.load_optimizer_state(optim_state)
         seed = self.ema_files.seed_path() if self.ema_files is not None else None
         if seed is not None:
             self.stepper.seed_weight_ema(torch.load(seed, map_location='cpu'))
