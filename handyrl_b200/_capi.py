@@ -115,6 +115,7 @@ class HrlGatherArgs(C.Structure):
 SYMBOLS = {
     'hrl_loss_workspace_bytes': (C.c_size_t, [C.c_int32] * 5),
     'hrl_loss_fwd_bwd': (C.c_int, [C.POINTER(HrlLossArgs), C.c_void_p]),
+    'hrl_loss_fwd': (C.c_int, [C.POINTER(HrlLossArgs), C.c_void_p]),
     'hrl_loss_diag_workspace_bytes': (C.c_size_t, [C.c_int32] * 5),
     'hrl_loss_fwd_bwd_diag': (C.c_int, [C.POINTER(HrlLossArgs), C.c_void_p, C.c_void_p]),
     'hrl_compute_target': (C.c_int, [C.c_int32] * 6 + [C.c_void_p] * 3 + [C.c_float, C.c_float] +

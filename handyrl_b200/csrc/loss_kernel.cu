@@ -144,7 +144,9 @@ __device__ __forceinline__ void row_epilogue(const LossParams &prm, const SmemLa
 // ======================================================================== rows kernel
 // IOS: logits and action masks staged in shared memory by cp.async (rows read/written on chip only).
 // DIAG (every kernel): the learner diagnostics sums are accumulated in phase 2c and folded with the losses.
-template <int LPR, int NPL, bool VEC, bool IOS, bool DIAG>
+// GRAD (every kernel): phase 3 is compiled in.  Without it (hrl_loss_fwd) the kernel writes the loss sums and the taps only:
+// phases 0-2c, the partials and the fixed-order fold are the same code, so the sums are bit-identical.
+template <int LPR, int NPL, bool VEC, bool IOS, bool DIAG, bool GRAD>
 __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
     extern __shared__ __align__(128) float smem[];
     __shared__ bool s_last;
@@ -267,7 +269,7 @@ __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
     HRL_STAMP(5);
 
     // ---------------- phase 3: gradients w.r.t. the raw net outputs
-    for (int base = 0; base < c.nrows; base += ngrp) {
+    for (int base = 0; GRAD && base < c.nrows; base += ngrp) {
         const int r = base + grp;
         if (r >= c.nrows) continue;  // no shuffles below: divergence is harmless
         const int e = r / R, rr = r - e * R, t = rr / Pa, q = rr - t * Pa;
@@ -324,7 +326,7 @@ __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
             if (prm.has_r) a.dreturn_raw[grow] = f.gr;
         }
     }
-    if (IOS) {
+    if (IOS && GRAD) {
         __syncthreads();
         const int per_ep = R * A;
         for (int i = tid; i < c.nE * per_ep; i += nthr) {
@@ -333,7 +335,7 @@ __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
             st_stream(a.dpolicy_raw + ((size_t)(c.b0 + e) * T0 + bi) * Pa * A + rem, smem[L.z + (e * R + rr) * RS + j]);
         }
     }
-    zero_burn_in(prm, c);
+    if (GRAD) zero_burn_in(prm, c);
     __syncthreads();
     if (s_last) {
         finalize_losses(prm, L, smem, c);
@@ -347,7 +349,7 @@ __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
 // are coalesced without any staging copy, every element-wise step (masking, exp, gradient) is one short
 // dependent chain per thread, and the row-wise steps (max, sums, scalar tail) are short loops over A <= 32
 // values held in shared memory.  This is the latency-optimal mapping when a window is only a few KB.
-template <bool DIAG>
+template <bool DIAG, bool GRAD>
 __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
     extern __shared__ __align__(128) float smem[];
     __shared__ bool s_last;
@@ -425,7 +427,7 @@ __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
     HRL_STAMP(5);
 
     // ---- 3a: per-row gradient factors (reusing the se / sw slots), value / return gradients
-    for (int r = tid; r < c.nrows; r += nthr) {
+    for (int r = tid; GRAD && r < c.nrows; r += nthr) {
         const int e = (c.nE == 1) ? 0 : r / R, rr = r - e * R, t = fdiv(rr, Pa, c.shPa), q = rr - t * Pa;
         const RowFactors f = row_factors(prm, L, smem, e * Tt + t, q, P, Pa);
         smem[L.se + r] = f.w;
@@ -437,7 +439,7 @@ __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
     __syncthreads();
     HRL_STAMP(18);
     // ---- 3b: gradients, one element per thread, coalesced stores
-    for (int i = tid; i < nelem; i += nthr) {
+    for (int i = tid; GRAD && i < nelem; i += nthr) {
         const int e = (c.nE == 1) ? 0 : i / per_ep, rem = i - e * per_ep;
         const int r = i / A, j = i - r * A;
         const float scale = smem[L.scale + r];
@@ -448,7 +450,7 @@ __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
         st_stream(a.dpolicy_raw + ((size_t)(c.b0 + e) * T0 + bi) * Pa * A + rem, g);
     }
     HRL_STAMP(19);
-    zero_burn_in(prm, c);
+    if (GRAD) zero_burn_in(prm, c);
     __syncthreads();
     if (s_last) {
         finalize_losses(prm, L, smem, c);
@@ -461,7 +463,7 @@ __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
 // Same job as the element kernel with fewer barrier-separated stages: RL = 2^k >= A lanes own one row, so the row
 // maximum, the exponential sums and the gathered logit are warp shuffles inside the lane group (one fused stage
 // instead of four), and the gradient stage recomputes the row factors per lane instead of a separate row pass.
-template <int RL, bool DIAG>
+template <int RL, bool DIAG, bool GRAD>
 __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) {
     extern __shared__ __align__(128) float smem[];
     __shared__ bool s_last;
@@ -521,7 +523,7 @@ __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) 
     HRL_STAMP(5);
 
     // ---- stage 3: gradients; every lane gathers its row's factors itself (no separate row pass)
-    for (int base = 0; base < c.nrows; base += ngrp) {
+    for (int base = 0; GRAD && base < c.nrows; base += ngrp) {
         const int r = base + grp;
         if (r >= c.nrows) continue;
         const int e = (c.nE == 1) ? 0 : r / R, rr = r - e * R, t = fdiv(rr, Pa, c.shPa), q = rr - t * Pa;
@@ -540,7 +542,7 @@ __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) 
         }
     }
     HRL_STAMP(19);
-    zero_burn_in(prm, c);
+    if (GRAD) zero_burn_in(prm, c);
     __syncthreads();
     if (s_last) {
         finalize_losses(prm, L, smem, c);
@@ -559,7 +561,7 @@ __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) 
 //   * after the (redundant, cheap) recurrences each warp turns its rows into gradients in place and sends every
 //     row home with a bulk store.
 // Shared memory is zbuf + ~14 KB, so two CTAs (32 row-reducing warps) share an SM.
-template <bool DIAG>
+template <bool DIAG, bool GRAD>
 __global__ void __launch_bounds__(544, 2) loss_bulk_kernel(const LossParams prm) {
     extern __shared__ __align__(128) float smem[];
     __shared__ bool s_last;
@@ -720,7 +722,7 @@ __global__ void __launch_bounds__(544, 2) loss_bulk_kernel(const LossParams prm)
     HRL_STAMP(5);
 
     // ---------------- gradients: in place, one bulk store per row
-    for (int rr = warp; rr < R; rr += NC) {
+    for (int rr = warp; GRAD && rr < R; rr += NC) {
         const int gr = r_lo + rr;
         const int t = fdiv(gr, Pa, c.shPa), q = gr - t * Pa;
         const size_t grow = ((size_t)c.b0 * T0 + bi + t) * Pa + q;
@@ -784,8 +786,8 @@ __global__ void __launch_bounds__(544, 2) loss_bulk_kernel(const LossParams prm)
             if (prm.has_r) a.dreturn_raw[grow] = f.gr;
         }
     }
-    if (lane == 0) bulk_store_wait_all();
-    if (crank == 0) zero_burn_in(prm, c);
+    if (GRAD && lane == 0) bulk_store_wait_all();
+    if (GRAD && crank == 0) zero_burn_in(prm, c);
     __syncthreads();
     if (s_last) {
         finalize_losses(prm, L, smem, c);
@@ -804,9 +806,9 @@ static int launch_kernel(K kern, const LossParams &prm, int grid, int threads, s
     return HRL_OK;
 }
 
-template <bool DIAG>
+template <bool DIAG, bool GRAD>
 static int launch_bulk(const LossParams &prm, int grid, int threads, size_t smem_bytes, cudaStream_t stream) {
-    HRL_CUDA_CHECK(cudaFuncSetAttribute(loss_bulk_kernel<DIAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    HRL_CUDA_CHECK(cudaFuncSetAttribute(loss_bulk_kernel<DIAG, GRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(threads);
@@ -819,7 +821,7 @@ static int launch_bulk(const LossParams &prm, int grid, int threads, size_t smem
     attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    HRL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, loss_bulk_kernel<DIAG>, prm));
+    HRL_CUDA_CHECK(cudaLaunchKernelEx(&cfg, loss_bulk_kernel<DIAG, GRAD>, prm));
     return HRL_OK;
 }
 
@@ -829,9 +831,9 @@ static int pow2_ceil(int x) {
     return p;
 }
 
-// The dispatch of hrl_loss_fwd_bwd; DIAG picks the kernels with the diagnostics sums compiled in (same choice of variant,
-// launch shape and shared memory).
-template <bool DIAG>
+// The dispatch of hrl_loss_fwd_bwd; DIAG picks the kernels with the diagnostics sums compiled in, !GRAD the forward-only
+// kernels of hrl_loss_fwd (same choice of variant, launch shape and shared memory in every form).
+template <bool DIAG, bool GRAD>
 static int loss_fwd_bwd(const HrlLossArgs *args, float *diag, void *stream_) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     HRL_REQUIRE(args != nullptr, HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: args is NULL");
@@ -851,8 +853,8 @@ static int loss_fwd_bwd(const HrlLossArgs *args, float *diag, void *stream_) {
     HRL_REQUIRE(a.policy_raw && a.action_mask && a.action && a.selected_prob && a.reward && a.ret && a.turn_mask &&
                     a.observation_mask && a.episode_mask && a.progress && a.outcome,
                 HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: a required input pointer is NULL");
-    HRL_REQUIRE(a.dpolicy_raw && a.losses, HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: a required output pointer is NULL");
-    HRL_REQUIRE((a.value_raw != nullptr) == (a.dvalue_raw != nullptr) && (a.return_raw != nullptr) == (a.dreturn_raw != nullptr),
+    HRL_REQUIRE(a.losses && (a.dpolicy_raw || !GRAD), HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: a required output pointer is NULL");
+    HRL_REQUIRE(!GRAD || ((a.value_raw != nullptr) == (a.dvalue_raw != nullptr) && (a.return_raw != nullptr) == (a.dreturn_raw != nullptr)),
                 HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: each head needs both its output and its gradient buffer");
     HRL_REQUIRE(a.A <= 1024, HRL_ERR_UNSUPPORTED, "hrl_loss_fwd_bwd: A=%d > 1024 not built", a.A);
     HRL_REQUIRE(a.P <= 64, HRL_ERR_UNSUPPORTED, "hrl_loss_fwd_bwd: P=%d > 64 not built", a.P);
@@ -883,7 +885,7 @@ static int loss_fwd_bwd(const HrlLossArgs *args, float *diag, void *stream_) {
     const int NPL = LPR == 1 ? pow2_ceil(a.A) : (a.A > 512 ? 32 : 16);
     const bool aligned16 = ((reinterpret_cast<uintptr_t>(a.policy_raw) & 15) == 0) &&
                            ((reinterpret_cast<uintptr_t>(a.action_mask) & 15) == 0) &&
-                           ((reinterpret_cast<uintptr_t>(a.dpolicy_raw) & 15) == 0);
+                           (!GRAD || (reinterpret_cast<uintptr_t>(a.dpolicy_raw) & 15) == 0);   // hrl_loss_fwd never writes it
     const int mode = tune.variant - 1;               // -1 auto, 0 direct, 1 staged I/O, 2 bulk, 3 element, 4 group
 
     // ---- bulk (TMA) kernel: wide rows
@@ -922,7 +924,7 @@ static int loss_fwd_bwd(const HrlLossArgs *args, float *diag, void *stream_) {
             const int grid = a.B * best_cs;
             HRL_REQUIRE(a.workspace != nullptr && a.workspace_bytes >= 2048 + (size_t)grid * 8 * sizeof(float), HRL_ERR_WORKSPACE,
                         "hrl_loss_fwd_bwd: workspace of %zu bytes is too small", a.workspace_bytes);
-            return launch_bulk<DIAG>(prm, grid, NC * 32, best_bytes, stream);
+            return launch_bulk<DIAG, GRAD>(prm, grid, NC * 32, best_bytes, stream);
         }
         HRL_REQUIRE(mode != 2, HRL_ERR_UNSUPPORTED, "hrl_loss_fwd_bwd: bulk kernel forced but the window does not fit");
     }
@@ -953,12 +955,12 @@ static int loss_fwd_bwd(const HrlLossArgs *args, float *diag, void *stream_) {
                         "hrl_loss_fwd_bwd: workspace of %zu bytes is too small", a.workspace_bytes);
             const size_t bytes = (size_t)L.total * 4;
             switch (RL) {
-                case 1: return launch_kernel(loss_group_kernel<1, DIAG>, prm, grid0, threads, bytes, stream);
-                case 2: return launch_kernel(loss_group_kernel<2, DIAG>, prm, grid0, threads, bytes, stream);
-                case 4: return launch_kernel(loss_group_kernel<4, DIAG>, prm, grid0, threads, bytes, stream);
-                case 8: return launch_kernel(loss_group_kernel<8, DIAG>, prm, grid0, threads, bytes, stream);
-                case 16: return launch_kernel(loss_group_kernel<16, DIAG>, prm, grid0, threads, bytes, stream);
-                default: return launch_kernel(loss_group_kernel<32, DIAG>, prm, grid0, threads, bytes, stream);
+                case 1: return launch_kernel(loss_group_kernel<1, DIAG, GRAD>, prm, grid0, threads, bytes, stream);
+                case 2: return launch_kernel(loss_group_kernel<2, DIAG, GRAD>, prm, grid0, threads, bytes, stream);
+                case 4: return launch_kernel(loss_group_kernel<4, DIAG, GRAD>, prm, grid0, threads, bytes, stream);
+                case 8: return launch_kernel(loss_group_kernel<8, DIAG, GRAD>, prm, grid0, threads, bytes, stream);
+                case 16: return launch_kernel(loss_group_kernel<16, DIAG, GRAD>, prm, grid0, threads, bytes, stream);
+                default: return launch_kernel(loss_group_kernel<32, DIAG, GRAD>, prm, grid0, threads, bytes, stream);
             }
         }
     }
@@ -986,7 +988,7 @@ static int loss_fwd_bwd(const HrlLossArgs *args, float *diag, void *stream_) {
             const int grid = (a.B + EPB - 1) / EPB;
             HRL_REQUIRE(a.workspace != nullptr && a.workspace_bytes >= 2048 + (size_t)grid * 8 * sizeof(float), HRL_ERR_WORKSPACE,
                         "hrl_loss_fwd_bwd: workspace of %zu bytes is too small", a.workspace_bytes);
-            return launch_kernel(loss_elem_kernel<DIAG>, prm, grid, threads, (size_t)L.total * 4, stream);
+            return launch_kernel(loss_elem_kernel<DIAG, GRAD>, prm, grid, threads, (size_t)L.total * 4, stream);
         }
     }
 
@@ -1033,7 +1035,7 @@ static int loss_fwd_bwd(const HrlLossArgs *args, float *diag, void *stream_) {
                 2048 + (size_t)grid * 8 * sizeof(float));
 
 #define HRL_CASE(l, n, v, s) \
-    if (LPR == l && NPL == n && vec == v && ios == s) return launch_kernel(loss_rows_kernel<l, n, v, s, DIAG>, prm, grid, threads, smem_bytes, stream);
+    if (LPR == l && NPL == n && vec == v && ios == s) return launch_kernel(loss_rows_kernel<l, n, v, s, DIAG, GRAD>, prm, grid, threads, smem_bytes, stream);
 #define HRL_CASE2(l, n) HRL_CASE(l, n, false, false) HRL_CASE(l, n, false, true)
     HRL_CASE2(1, 1) HRL_CASE2(1, 2) HRL_CASE2(1, 4) HRL_CASE2(1, 8) HRL_CASE2(1, 16)
     HRL_CASE2(2, 16) HRL_CASE2(4, 16) HRL_CASE2(8, 16) HRL_CASE2(16, 16) HRL_CASE2(32, 16)
@@ -1055,8 +1057,10 @@ extern "C" size_t hrl_loss_diag_workspace_bytes(int32_t B, int32_t, int32_t, int
     return hrl::loss_diag_workspace_bytes(B);   // + the diagnostics partials of up to eight CTAs per window
 }
 
-extern "C" int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream) { return hrl::loss_fwd_bwd<false>(args, nullptr, stream); }
+extern "C" int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream) { return hrl::loss_fwd_bwd<false, true>(args, nullptr, stream); }
 
 extern "C" int hrl_loss_fwd_bwd_diag(const HrlLossArgs *args, float *diag, void *stream) {
-    return hrl::loss_fwd_bwd<true>(args, diag, stream);
+    return hrl::loss_fwd_bwd<true, true>(args, diag, stream);
 }
+
+extern "C" int hrl_loss_fwd(const HrlLossArgs *args, void *stream) { return hrl::loss_fwd_bwd<false, false>(args, nullptr, stream); }

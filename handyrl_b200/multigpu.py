@@ -138,12 +138,14 @@ def _helper_main(rank, world, port, args, model_blob, lr, conn, optim_state=None
         assert cmds.get()[0] == 'start'                # the backlog has arrived in `episodes`
         batch = Batcher(args, episodes)._make()
         batch = tree_map(lambda t: t[:t.shape[0] // world].contiguous(), batch)
-        # rank 0 averages and writes the optimiser state
-        stepper = LearnerStep(model, args, batch, lr, device=device, process_group=pg, weight_ema=0, save_optimizer=False)
+        # rank 0 averages, validates and writes the optimiser state
+        stepper = LearnerStep(model, args, batch, lr, device=device, process_group=pg, weight_ema=0, save_optimizer=False,
+                              validation=False)
         if optim_state is not None:
             stepper.load_optimizer_state(optim_state)
         stepper.warm_up()
-        gb = GpuBatcher(args, episodes, device, seed=args.get('seed', 0) * 7919 + 17 + rank)
+        # rank 0 validates: the held-out episodes (the same ones on every rank) are left out here
+        gb = GpuBatcher(args, episodes, device, seed=args.get('seed', 0) * 7919 + 17 + rank, keep_validation=False)
         gb.run()
         while not gb.ready():
             time.sleep(0.005)

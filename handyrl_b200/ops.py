@@ -51,14 +51,17 @@ def algo_id(name):
 
 
 class LossBuffers:
-    """Pre-allocated outputs of one fused loss launch (re-used across steps / graph replays)."""
+    """Pre-allocated outputs of one fused loss launch (re-used across steps / graph replays).  grads=False: the outputs of the
+    forward-only pass (loss_fwd), without gradient buffers."""
 
-    def __init__(self, B, T, P, Pa, A, has_value, has_return, device, taps=False, policy_dtype=torch.float32, diagnostics=False):
+    def __init__(self, B, T, P, Pa, A, has_value, has_return, device, taps=False, policy_dtype=torch.float32, diagnostics=False,
+                 grads=True):
         f = dict(dtype=torch.float32, device=device)
         self.dims = (B, T, P, Pa, A)
-        self.dpolicy = torch.empty((B, T, Pa, A), dtype=policy_dtype, device=device)      # bf16 logits get bf16 gradients
-        self.dvalue = torch.empty((B, T, Pa, 1), **f) if has_value else None
-        self.dreturn = torch.empty((B, T, Pa, 1), **f) if has_return else None
+        self.policy_dtype = policy_dtype
+        self.dpolicy = torch.empty((B, T, Pa, A), dtype=policy_dtype, device=device) if grads else None   # bf16 logits: bf16 gradients
+        self.dvalue = torch.empty((B, T, Pa, 1), **f) if has_value and grads else None
+        self.dreturn = torch.empty((B, T, Pa, 1), **f) if has_return and grads else None
         self.losses = torch.zeros(NUM_LOSS, **f)
         self.taps = None
         if taps:
@@ -95,6 +98,19 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None, di
              losses and gradients are bit-identical to the plain pass
     returns  LossBuffers with .losses = [p, v, r, ent, total, dcnt] and the gradients.
     """
+    return _loss_call(outputs, batch, args, buffers, taps, tuning, 'diag' if diagnostics else 'fwd_bwd')
+
+
+def loss_fwd(outputs, batch, args, buffers=None, taps=False, tuning=None):
+    """The forward half of loss_fwd_bwd (hrl_loss_fwd): the same kernel choice with the gradient phase compiled out, for losses
+    on data the optimiser does not see.  Same arguments (buffers: LossBuffers(..., grads=False), or any LossBuffers -- its
+    gradient buffers are left untouched); returns the (6,) device tensor of sums [p, v, r, ent, total, dcnt], bit-identical
+    to loss_fwd_bwd(...).losses on the same inputs."""
+    return _loss_call(outputs, batch, args, buffers, taps, tuning, 'fwd').losses
+
+
+def _loss_call(outputs, batch, args, buffers, taps, tuning, form):
+    diagnostics = form == 'diag'
     policy = outputs['policy']
     io_bf16 = policy.dtype == torch.bfloat16       # wide rows only: 8 instead of 12 bytes per action through HBM (include/hrl_b200.h)
     if io_bf16:
@@ -107,8 +123,11 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None, di
     value = _dev_f32(outputs.get('value'), 'value')
     ret_head = _dev_f32(outputs.get('return'), 'return')
     if buffers is None:
-        buffers = LossBuffers(B, T, P, Pa, A, value is not None, ret_head is not None, policy.device, taps=taps, policy_dtype=policy.dtype)
-    assert buffers.dims == (B, T, P, Pa, A) and buffers.dpolicy.dtype == policy.dtype
+        buffers = LossBuffers(B, T, P, Pa, A, value is not None, ret_head is not None, policy.device, taps=taps, policy_dtype=policy.dtype,
+                              grads=form != 'fwd')
+    assert buffers.dims == (B, T, P, Pa, A) and buffers.policy_dtype == policy.dtype
+    if form != 'fwd' and buffers.dpolicy is None:
+        raise ValueError('loss_fwd_bwd: these LossBuffers were built without gradient buffers (grads=False)')
     if diagnostics:
         buffers.enable_diagnostics()
 
@@ -119,10 +138,10 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None, di
            buffers.taps is not None, None if tuning is None else tuple(sorted((k, v if not torch.is_tensor(v) else v.data_ptr())
                                                                                  for k, v in tuning.items()))) + \
         tuple(batch[k].data_ptr() for k in _BATCH_KEYS)
-    slot = '_cached_diag' if diagnostics else '_cached'      # one argument block per form
+    slot = '_cached_' + form      # one argument block per form
     cached = getattr(buffers, slot, None)
     if cached is not None and cached[0] == key:
-        _launch(cached[1], buffers, diagnostics)
+        _launch(cached[1], buffers, form)
         return buffers
 
     a = HrlLossArgs()
@@ -147,7 +166,8 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None, di
             _dev_f32(batch['progress'], 'progress'), _dev_f32(batch['outcome'], 'outcome')]
     (a.policy_raw, a.value_raw, a.return_raw, a.action_mask, a.action, a.selected_prob, a.reward, a.ret,
      a.turn_mask, a.observation_mask, a.episode_mask, a.progress, a.outcome) = [_ptr(t) for t in keep]
-    a.dpolicy_raw, a.dvalue_raw, a.dreturn_raw = _ptr(buffers.dpolicy), _ptr(buffers.dvalue), _ptr(buffers.dreturn)
+    if form != 'fwd':
+        a.dpolicy_raw, a.dvalue_raw, a.dreturn_raw = _ptr(buffers.dpolicy), _ptr(buffers.dvalue), _ptr(buffers.dreturn)
     a.losses = _ptr(buffers.losses)
     if buffers.taps is not None:
         t = buffers.taps
@@ -169,7 +189,7 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None, di
             setattr(a.tuning, k, int(t.pop(k, 0)))
         if t:
             raise ValueError('unknown loss tuning keys: %s' % sorted(t))
-    _launch(a, buffers, diagnostics)
+    _launch(a, buffers, form)
     buffers._keep = keep  # the launch is asynchronous: keep temporaries alive
     if all(k is None or k is o for k, o in zip(keep[3:], (batch['action_mask'], batch['action'], batch['selected_prob'],
                                                           batch['reward'], batch['return'], batch['turn_mask'],
@@ -179,9 +199,11 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None, di
     return buffers
 
 
-def _launch(a, buffers, diagnostics):
-    if diagnostics:
+def _launch(a, buffers, form):
+    if form == 'diag':
         check(lib().hrl_loss_fwd_bwd_diag(C.byref(a), _ptr(buffers.diagnostics), _stream_ptr()))
+    elif form == 'fwd':
+        check(lib().hrl_loss_fwd(C.byref(a), _stream_ptr()))
     else:
         check(lib().hrl_loss_fwd_bwd(C.byref(a), _stream_ptr()))
     _count()

@@ -11,6 +11,7 @@ Store layout = include/hrl_b200.h HrlGatherArgs: one row per episode step, colum
 Nested observations are stored as the concatenation of their flattened leaves.
 """
 import ctypes as C
+import hashlib
 import random
 import threading
 
@@ -24,6 +25,19 @@ from .batch import flatten_moments, decode_moments, sample_window, tree_leaves, 
 WINDOW_DTYPE = np.dtype([('first_step', '<i8'), ('start', '<i4'), ('end', '<i4'), ('train_start', '<i4'),
                          ('total', '<i4'), ('outcome_row', '<i4'), ('player', '<i4')])
 assert WINDOW_DTYPE.itemsize == C.sizeof(HrlWindow)
+
+
+def held_out(fe, rate):
+    """True when the episode (a FlatEpisode) belongs to the held-out validation split of rate r: an 8-byte BLAKE2b digest of its
+    step arrays (action, selected prob, turn) and outcome, read as a fraction in [0, 1), is below r.  The decision depends on the
+    episode's content alone -- not on Python's salted hash(), the arrival order, the rank or the wire format it came in -- so every
+    rank and every restart splits the replay the same way.  rate None or 0: never."""
+    if not rate:
+        return False
+    h = hashlib.blake2b(digest_size=8)
+    for a in (fe.action, fe.prob, fe.turn, fe.outcome):
+        h.update(np.ascontiguousarray(a).tobytes())
+    return int.from_bytes(h.digest(), 'little') < rate * 2.0 ** 64
 
 
 class EpisodeHandle:

@@ -309,6 +309,27 @@ def weight_ema_decay(value):
     return float(value)
 
 
+def validation_rate(args):
+    """train_args['validation_rate'] -> the fraction r of episodes held out of training for the validation loss, or None when
+    validation is off (key absent, 0 or None).  Anything else outside (0, 1) raises ValueError, and so does the key together
+    with gpu_replay: False (the held-out split lives in the GPU replay)."""
+    value = args.get('validation_rate')
+    if value is None or (isinstance(value, numbers.Real) and value == 0):
+        return None
+    if isinstance(value, bool) or not isinstance(value, numbers.Real) or not 0.0 < float(value) < 1.0:
+        raise ValueError("train_args['validation_rate'] must be a fraction in (0, 1) (e.g. 0.05), or 0 / None for no validation; "
+                         "got %r" % (value,))
+    if not args.get('gpu_replay', True):
+        raise ValueError("train_args['validation_rate'] needs the GPU replay (gpu_replay: True): the held-out episodes are kept there")
+    return float(value)
+
+
+def loss_line(name, sums, heads):
+    """'<name> = p:0.512 v:0.231 ent:1.843 total:0.561': each head's sum over the sums' own sample count dcnt, as the Trainer
+    prints its training loss (train.py:392)."""
+    return '%s = %s' % (name, ' '.join([k + ':' + '%.3f' % (sums[k] / sums['dcnt']) for k in heads]))
+
+
 class AveragedCheckpoints:
     """Files written next to the Learner's checkpoints (reference train.py:441-454): models/<epoch>.<suffix>.pth and
     models/latest.<suffix>.pth, in the Learner's relative `models` directory, written with torch.save.  <epoch> is the number
@@ -446,15 +467,19 @@ class PendingModel:
     eval mode and caches its pickled bytes on it (the Learner pickles the model for every worker request,
     train.py:605-615).  With a moving average of the weights (`host_avg`), it also leaves the averaged state_dict, keyed
     like the model's, in `ema_state`; with the optimiser state (`host_optim`, LearnerStep.end_epoch's layout), it leaves
-    that state in the OptimizerStateFormat dict in `optim_state`, scheduled at step count `steps`."""
+    that state in the OptimizerStateFormat dict in `optim_state`, scheduled at step count `steps`.  With validation passes
+    (`host_val`), it prints their lines after the loss line and leaves their sums in `validation` (what
+    LearnerStep.pop_validation() returns)."""
 
     def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host_avg=None, host_optim=None,
-                 steps=0):
+                 steps=0, host_val=None):
         self.stepper, self.done, self.host_state, self.host_losses = stepper, done_event, host_state, host_losses
         self.heads, self.template, self.host_avg = heads, template, host_avg
         self.host_optim, self.steps = host_optim, steps
+        self.host_val = host_val
         self.ema_state = None
         self.optim_state = None
+        self.validation = None
 
     def resolve(self):
         self.done.synchronize()
@@ -465,9 +490,14 @@ class PendingModel:
         if len(host) > NUM_LOSS:        # the learner's diagnostics sums ride behind the loss sums
             self.diagnostics = ops.summarize_diagnostics(host[NUM_LOSS:])
         if dcnt > 0:
-            print('loss = %s' % ' '.join([k + ':' + '%.3f' % (sums[k] / dcnt) for k in self.heads]))
+            print(loss_line('loss', sums, self.heads))
             if self.diagnostics is not None:
                 print(ops.format_diagnostics(self.diagnostics))
+        if self.host_val is not None:
+            self.validation = self.stepper.validation_sums(self.host_val.tolist())
+            for name, val in self.validation.items():
+                if val['dcnt'] > 0:
+                    print(loss_line(name, val, self.heads))
         tpl = self.template
         store = self.stepper.state
         keys = list(tpl.state_dict().keys())
@@ -519,13 +549,24 @@ class LearnerStep:
     OptimizerStateFormat dict (PendingModel.optim_state), by the same device-to-device snapshot and side-stream copy as the
     model.  optimizer_state_dict() reads it now; load_optimizer_state() resumes from it.  The step itself is the same with
     and without.
+
+    validation (default: whether train_args['validation_rate'] is set, off): validate_in_place() evaluates the batch in
+    self.dev with the current weights -- net forward in training mode (BatchNorm on batch statistics, as in the step), then the
+    forward-only loss kernel (ops.loss_fwd) -- and adds the six loss sums to `val_accum`; validate_in_place(averaged=True)
+    does the same with the moving average of the weights into `val_ema_accum`.  No backward, no optimiser step, no
+    all-reduce, and the learner is left bit for bit as it was: the StateStore bytes (weights, BatchNorm running statistics,
+    num_batches_tracked) are saved and restored around the pass on the device.  In graph mode each form is one more CUDA
+    graph sharing the step graph's memory pool; `launches_per_validation` counts its launches.  end_epoch hands the sums
+    over with the loss sums (PendingModel.validation); pop_validation() reads them now.
     """
 
     def __init__(self, model, args, example_batch, lr, device=None, process_group=None, use_graph=True,
                  max_norm=4.0, weight_decay=1e-5, time_loss_kernel=False, channels_last=True, cudnn_benchmark=True,
                  small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None,
-                 weight_ema=None, save_optimizer=None):
+                 weight_ema=None, save_optimizer=None, validation=None):
         self.weight_ema = weight_ema_decay(args.get('weight_ema') if weight_ema is None else weight_ema)
+        rate = validation_rate(args)
+        self.validation = bool(rate is not None if validation is None else validation)
         self.save_optimizer = bool(args.get('save_optimizer', False) if save_optimizer is None else save_optimizer)
         self.device = torch.device(device if device is not None else 'cuda')
         self.args = args
@@ -584,6 +625,18 @@ class LearnerStep:
             self.avg_bytes = self.state.bytes[:self.state.i_off].clone()
             self.avg = self.avg_bytes.view(torch.float32)
             self.avg_snap = torch.empty_like(self.avg_bytes)
+        # validation sums [live (NUM_LOSS) | averaged (NUM_LOSS)], the epoch hand-off's copy, and the state saved around a pass
+        self.val_accum_all = self.val_accum = self.val_ema_accum = self.val_snap = self.val_saved = None
+        self.val_buf = None
+        self.val_graphs = {}
+        self.launches_per_validation = 0
+        if self.validation:
+            self.val_accum_all = torch.zeros(2 * NUM_LOSS, dtype=torch.float64, device=self.device)
+            self.val_accum = self.val_accum_all[:NUM_LOSS]
+            if self.avg is not None:
+                self.val_ema_accum = self.val_accum_all[NUM_LOSS:]
+            self.val_snap = torch.zeros_like(self.val_accum_all)
+            self.val_saved = torch.empty_like(self.state.bytes)
         self.acc_snap = torch.zeros(n_sums, dtype=torch.float64, device=self.device)
         self.copy_stream = torch.cuda.Stream(device=self.device)
         self._handoff_slots = None
@@ -703,6 +756,30 @@ class LearnerStep:
         self._part_loss()
         self._part_backward()
 
+    def _device_validate(self, averaged):
+        """The device work of one validation pass, on the current stream (inputs already in self.dev)."""
+        store = self.state
+        self.val_saved.copy_(store.bytes)          # the train-mode forward moves the BatchNorm running statistics
+        if averaged:
+            store.bytes[:store.i_off].copy_(self.avg_bytes)
+        fastnet.new_step()          # the weights differ from those the cached convolution images were packed from
+        B, T, P, Pa, A = self.dims
+        with torch.no_grad():
+            if self.engine is not None:
+                flat = self.engine.forward(self.dev['observation'].flatten(0, 2))
+                outs = {k: v.unflatten(0, (B, T, Pa)) for k, v in flat.items()}
+            else:
+                outs = forward_raw(self.model, self.hidden0, self.dev, self.args, self.memory_format)
+        if self.val_buf is None:
+            self.val_buf = ops.LossBuffers(B, T, P, Pa, A, 'value' in outs, 'return' in outs, self.device, grads=False)
+        sums = ops.loss_fwd({k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, self.dev, self.args,
+                            buffers=self.val_buf)
+        (self.val_ema_accum if averaged else self.val_accum).add_(sums)
+        store.bytes.copy_(self.val_saved)
+
+    def _validation_forms(self):
+        return [False, True] if self.val_ema_accum is not None else [False]
+
     def _capture(self):
         # warm-up on the step stream (cuDNN heuristics, lazy inits, NCCL communicator), then capture
         self.stream.wait_stream(torch.cuda.current_stream(self.device))
@@ -713,12 +790,19 @@ class LearnerStep:
                 before = ops.LAUNCHES['n']
                 self._device_step()
                 self.launches_per_step = ops.LAUNCHES['n'] - before      # this library's kernels in one step
+            if self.validation:
+                for averaged in self._validation_forms():
+                    for i in range(2):
+                        before = ops.LAUNCHES['n']
+                        self._device_validate(averaged)
+                        self.launches_per_validation = ops.LAUNCHES['n'] - before
             self.stream.synchronize()
             self._restore(state)
             if self.use_graph and not self.time_loss_kernel:
                 self.graph = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(self.graph, stream=self.stream):
                     self._device_step()
+                self._capture_validation(self.graph.pool())
                 self._restore(state)
             elif self.use_graph:
                 # the loss kernel is launched between two graphs so that CUDA events can bracket it
@@ -729,9 +813,21 @@ class LearnerStep:
                 self.graph_bwd = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(self.graph_bwd, pool=self.graph_fwd.pool(), stream=self.stream):
                     self._part_backward()
+                self._capture_validation(self.graph_fwd.pool())
                 self._restore(state)
             self.stream.synchronize()
         self._captured = True
+
+    def _capture_validation(self, pool):
+        """One CUDA graph per validation form, after the step graph and in its memory pool: the graphs never run concurrently,
+        so the pass reuses the step's activation memory instead of doubling it."""
+        if not self.validation:
+            return
+        for averaged in self._validation_forms():
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, pool=pool, stream=self.stream):
+                self._device_validate(averaged)
+            self.val_graphs[averaged] = g
 
     def _snapshot(self):
         bufs = {k: v.clone() for k, v in self.model.state_dict().items()}
@@ -739,6 +835,8 @@ class LearnerStep:
                 self.accum.clone(), self.avg.clone() if self.avg is not None else None)
 
     def _restore(self, state):
+        if self.val_accum_all is not None:
+            self.val_accum_all.zero_()
         bufs, m, v, sc, acc, avg = state
         with torch.no_grad():
             for k, t in self.model.state_dict().items():
@@ -813,6 +911,40 @@ class LearnerStep:
                 self.graph_bwd.replay()
         self.steps += 1
 
+    def validate_in_place(self, averaged=False):
+        """Enqueue one validation pass on the batch in self.dev (written there by GpuBatcher.fill_validation on the step
+        stream): the six loss sums of the current weights -- or of their moving average when `averaged` -- are added to
+        val_accum (val_ema_accum).  Returns without waiting for the GPU; the learner's state is left as it was.  The first step
+        (or warm_up) runs the capture, which uses self.dev: write the batch after it."""
+        if not self.validation:
+            raise RuntimeError('LearnerStep was built without validation (train_args["validation_rate"] / validation=True)')
+        if averaged:
+            self._require_average()
+        if not getattr(self, '_captured', False):
+            self._capture()
+        with torch.cuda.stream(self.stream):
+            if self.use_graph:
+                self.val_graphs[averaged].replay()
+            else:
+                self._device_validate(averaged)
+
+    def validation_sums(self, values):
+        """{'validation': {LOSS_KEYS: sum}[, 'validation_ema': ...]} of a host list in val_accum_all's layout."""
+        out = {'validation': dict(zip(LOSS_KEYS, values[:NUM_LOSS]))}
+        if self.val_ema_accum is not None:
+            out['validation_ema'] = dict(zip(LOSS_KEYS, values[NUM_LOSS:2 * NUM_LOSS]))
+        return out
+
+    def pop_validation(self):
+        """Validation sums accumulated since the last call or epoch boundary (one host sync): {'validation': {p, v, r, ent,
+        total, dcnt}} and, with a moving average of the weights, 'validation_ema'; divide by dcnt for the printed means."""
+        if not self.validation:
+            raise RuntimeError('LearnerStep was built without validation (train_args["validation_rate"] / validation=True)')
+        self.stream.synchronize()
+        vals = self.val_accum_all.cpu().tolist()
+        self.val_accum_all.zero_()
+        return self.validation_sums(vals)
+
     def loss_kernel_ms(self):
         """Average device time of the fused loss kernel over the steps since the last call
         (needs time_loss_kernel=True)."""
@@ -861,6 +993,7 @@ class LearnerStep:
         """Release the captured graphs (they pin NCCL kernels: destroy them before the process group)."""
         self.stream.synchronize()
         self.graph = self.graph_fwd = self.graph_bwd = None
+        self.val_graphs = {}
         self._outs = None
         self._captured = False
         import gc
@@ -975,8 +1108,10 @@ class LearnerStep:
                                     torch.empty(self.state.bytes.numel(), dtype=torch.uint8).pin_memory()
                                     if self.avg is not None else None,
                                     torch.empty(self.optim_snap.numel(), dtype=torch.uint8).pin_memory()
-                                    if self.optim_snap is not None else None) for _ in range(2)]
-        host_state, host_losses, host_avg, host_optim = self._handoff_slots[self._handoff_i % 2]
+                                    if self.optim_snap is not None else None,
+                                    torch.zeros(self.val_snap.numel(), dtype=torch.float64).pin_memory()
+                                    if self.val_snap is not None else None) for _ in range(2)]
+        host_state, host_losses, host_avg, host_optim, host_val = self._handoff_slots[self._handoff_i % 2]
         self._handoff_i += 1
         with torch.cuda.stream(self.stream):
             self.epoch_schedule(batch_cnt, steps, default_lr)
@@ -989,6 +1124,9 @@ class LearnerStep:
                 for dst, src in zip(self._optim_views(self.optim_snap),
                                     (self.opt.exp_avg, self.opt.exp_avg_sq, self.opt.step_count, self.opt.lr, self.ema)):
                     dst.copy_(src)
+            if self.val_snap is not None:
+                self.val_snap.copy_(self.val_accum_all)
+                self.val_accum_all.zero_()
             ready = torch.cuda.Event()
             ready.record(self.stream)
         with torch.cuda.stream(self.copy_stream):
@@ -999,11 +1137,13 @@ class LearnerStep:
                 host_avg[:self.state.i_off].copy_(self.avg_snap, non_blocking=True)
             if self.optim_snap is not None:
                 host_optim.copy_(self.optim_snap, non_blocking=True)
+            if self.val_snap is not None:
+                host_val.copy_(self.val_snap, non_blocking=True)
             done = torch.cuda.Event()
             done.record(self.copy_stream)
         self._last_done = done
         return PendingModel(self, done, host_state, host_losses, heads, template, host_avg=host_avg, host_optim=host_optim,
-                            steps=int(steps))
+                            steps=int(steps), host_val=host_val)
 
 
 # --------------------------------------------------------------------------- batcher + trainer
@@ -1146,14 +1286,20 @@ class GpuBatcher:
     Feeder and learner never wait for each other's GPU work on the host: the upload stream waits (on the device) for
     the last gather that may read rows it overwrites, the step stream waits for the last upload; the only shared
     host lock covers "sample + enqueue gather" on one side and "update directory + enqueue copies" on the other
-    (microseconds each: staging into pinned memory happens outside it)."""
+    (microseconds each: staging into pinned memory happens outside it).
+
+    With train_args['validation_rate'] = r, the episodes replay.held_out() picks (a fraction r, decided from their content)
+    never enter the training ring: they go to a second DeviceReplay, `val_replay`, of r times the ring's steps and
+    r * maximum_episodes episodes, that fill_validation() samples from -- or, with keep_validation=False (helper ranks, which
+    do not validate), nowhere."""
 
     DESC_SLOTS = 4        # pinned descriptor buffers in rotation: bounds how far the host runs ahead of the GPU
 
-    def __init__(self, args, episodes, device, seed=None, forward=None):
+    def __init__(self, args, episodes, device, seed=None, forward=None, keep_validation=True):
         from .replay import DeviceReplay
         from .wire import episode_to_flat
         self.args = args
+        self.validation = validation_rate(args)
         self.device = device
         self.forward = forward              # multi-GPU: callable(list of episodes) that ships them to the other ranks
         self.pending = queue.Queue()
@@ -1162,7 +1308,9 @@ class GpuBatcher:
         self.last_gather = None
         self.order_lock = threading.Lock()
         self.stop_event = threading.Event()
-        self.rng = np.random.default_rng(seed if seed is not None else args.get('seed', 0) * 7919 + 17)
+        seed = seed if seed is not None else args.get('seed', 0) * 7919 + 17
+        self.rng = np.random.default_rng(seed)
+        self.val_rng = np.random.default_rng(seed + 1)      # validation draws leave the training stream alone
         self.fed = 0
         self._slots = None
         self._slot_i = 0
@@ -1192,9 +1340,9 @@ class GpuBatcher:
         # ring capacity from the observed episode lengths and the free HBM (the reference bounds episodes, not steps)
         fe0 = episode_to_flat(backlog[0]) if backlog else None
         cap = int(args.get('replay_capacity_steps', 0))
+        lens = [e['steps'] for e in backlog] or [64]
+        mean_len, max_len = sum(lens) / len(lens), max(lens)
         if not cap:
-            lens = [e['steps'] for e in backlog] or [64]
-            mean_len, max_len = sum(lens) / len(lens), max(lens)
             want = int(args['maximum_episodes'] * mean_len * 1.25) + 4 * max_len
             budget = want
             if fe0 is not None and torch.device(device).type == 'cuda':
@@ -1206,6 +1354,11 @@ class GpuBatcher:
                 print('handyrl_b200: the GPU replay holds about %d episodes (%d steps), fewer than maximum_episodes=%d'
                       % (est, cap, args['maximum_episodes']))
         self.replay = DeviceReplay(cap, args['maximum_episodes'], device=device)
+        self.val_replay = None
+        if self.validation is not None and keep_validation:
+            r = self.validation
+            self.val_replay = DeviceReplay(max(int(r * cap), 2 * max_len), max(1, int(round(r * args['maximum_episodes']))),
+                                           device=device)
         self.thread = threading.Thread(target=self._feed, daemon=True)
 
     def run(self):
@@ -1213,6 +1366,7 @@ class GpuBatcher:
             self.thread.start()
 
     def _feed(self):
+        from .replay import held_out
         from .wire import episode_to_flat
         while not self.stop_event.is_set():
             try:
@@ -1227,12 +1381,20 @@ class GpuBatcher:
             try:
                 if self.forward is not None:
                     self.forward(eps)
-                staged = self.replay.stage([episode_to_flat(ep) for ep in eps])
+                fes = [episode_to_flat(ep) for ep in eps]
+                held = [held_out(fe, self.validation) for fe in fes]
+                train = [fe for fe, h in zip(fes, held) if not h]
+                val = [fe for fe, h in zip(fes, held) if h] if self.val_replay is not None else []
+                staged = self.replay.stage(train) if train else None
+                val_staged = self.val_replay.stage(val) if val else None
                 with self.order_lock:
                     if self.last_gather is not None:   # device-side: never overwrite rows an enqueued gather reads
                         self.upload_stream.wait_event(self.last_gather)
                     with torch.cuda.stream(self.upload_stream):
-                        self.replay.commit(staged)
+                        if staged is not None:
+                            self.replay.commit(staged)
+                        if val_staged is not None:
+                            self.val_replay.commit(val_staged)
                         ev = torch.cuda.Event()
                         ev.record(self.upload_stream)
                         self.last_upload = ev
@@ -1258,12 +1420,24 @@ class GpuBatcher:
             slot['event'].synchronize()      # the gather that read this slot DESC_SLOTS steps ago
         return slot
 
+    def validation_ready(self):
+        """True once the held-out ring holds an episode."""
+        return self.val_replay is not None and len(self.val_replay) > 0
+
     def fill(self, stepper):
         """Sample a batch and gather it into stepper.dev (on the step stream)."""
+        self._fill(stepper, self.replay, self.rng)
+
+    def fill_validation(self, stepper):
+        """Sample a batch of held-out windows (the same sampling law) and gather it into stepper.dev (on the step stream), for
+        LearnerStep.validate_in_place."""
+        self._fill(stepper, self.val_replay, self.val_rng)
+
+    def _fill(self, stepper, replay, rng):
         B = stepper.dims[0]
         slot = self._descriptor_slot(B)
         with self.order_lock:
-            win = self.replay.sample_windows(B, self.args, self.rng)
+            win = replay.sample_windows(B, self.args, rng)
             slot['host'].numpy()[:] = win.view(np.uint8)
             with torch.cuda.stream(stepper.stream):
                 if self.last_upload is not None:
@@ -1276,9 +1450,9 @@ class GpuBatcher:
                 else:
                     out['observation'] = self._flat_obs(stepper)
                 out['value'] = self._value_sink(stepper)
-                self.replay.gather(slot['dev'], self.args, out=out)
+                replay.gather(slot['dev'], self.args, out=out)
                 if not single_leaf:
-                    nested = self.replay.split_observation(out['observation'])
+                    nested = replay.split_observation(out['observation'])
                     for d, s_ in zip(tree_leaves(stepper.dev['observation']), tree_leaves(nested)):
                         d.copy_(s_)
                 ev = torch.cuda.Event()
@@ -1289,7 +1463,7 @@ class GpuBatcher:
     def _flat_obs(self, stepper):
         if not hasattr(self, '_obs_buf'):
             B, T, Pa = stepper.dev['action'].shape[:3]
-            self._obs_buf = torch.empty((B, T, Pa, self.replay.OE), device=self.device)
+            self._obs_buf = torch.empty((B, T, Pa, self.replay.OE), device=self.device)   # both rings hold one kind of episode
         return self._obs_buf
 
     def _value_sink(self, stepper):
@@ -1321,10 +1495,18 @@ class Trainer:
     train_args['save_optimizer'] = True: update() also writes the optimiser state and learning-rate schedule the next step
     uses to models/<epoch>.optim.pth and models/latest.optim.pth (OptimizerStateFormat), numbered by the same
     AveragedCheckpoints as the averages; a run restarted at restart_epoch resumes Adam's moments and step count, the
-    learning rate, the data-count average and `steps` from models/<restart_epoch>.optim.pth when that file exists."""
+    learning rate, the data-count average and `steps` from models/<restart_epoch>.optim.pth when that file exists.
+
+    train_args['validation_rate'] = r in (0, 1): a fraction r of the episodes (replay.held_out) is held out of training, and
+    after every round(1 / r)-th step one batch of held-out windows is evaluated with the live weights (and with their moving
+    average under weight_ema) without an update (LearnerStep.validate_in_place).  Each epoch prints 'validation = ...' (and
+    'validation_ema = ...') after the loss line, in its format, once the held-out ring holds an episode.  Only rank 0
+    validates; every rank leaves the held-out episodes out of its training ring."""
 
     def __init__(self, args, model):
         self.weight_ema = weight_ema_decay(args.get('weight_ema'))
+        self.validation = validation_rate(args)
+        self.validate_every = max(1, int(round(1.0 / self.validation))) if self.validation is not None else 0
         self.save_optimizer = bool(args.get('save_optimizer', False))
         self.checkpoint_files = None         # numbers the .ema.pth and .optim.pth files of one epoch alike
         if self.weight_ema is not None or self.save_optimizer:
@@ -1439,6 +1621,11 @@ class Trainer:
                     self.fleet.run_steps(chunk)          # every rank runs exactly the steps rank 0 runs
                 self.gpu_batcher.fill(self.stepper)
                 self.stepper.step_in_place()
+                if self.validate_every and (batch_cnt + 1) % self.validate_every == 0 and self.gpu_batcher.validation_ready():
+                    self.gpu_batcher.fill_validation(self.stepper)
+                    self.stepper.validate_in_place()
+                    if self.stepper.avg is not None:
+                        self.stepper.validate_in_place(averaged=True)
             else:
                 batch = self.batcher.batch()
                 if batch is None:           # stop() was called

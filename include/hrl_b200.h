@@ -11,7 +11,8 @@
  *                            + the autograd pass of train.py:369 restricted to those ops
  *   hrl_loss_fwd_bwd_diag <- the same pass + learner diagnostics sums (importance ratios, advantages, value fit);
  *                            no reference counterpart
- *   hrl_compute_target    <- handyrl/losses.py:63-80  (compute_target, stand-alone)
+ *   hrl_loss_fwd          <- the forward half alone: compute_loss (train.py:189-267) on held-out data, no update
+ *   hrl_compute_target   <- handyrl/losses.py:63-80  (compute_target, stand-alone)
  *   hrl_peer_allreduce_sumsq <- the gradient exchange nn.DataParallel does implicitly (train.py:339-340), as a
  *                            fused peer-memory kernel
  *   hrl_grad_sumsq /
@@ -140,6 +141,11 @@ size_t hrl_loss_workspace_bytes(int32_t B, int32_t T, int32_t P, int32_t Pa, int
 
 /* Enqueue the fused loss pass.  `stream` is a cudaStream_t. */
 int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream);
+
+/* The forward half of hrl_loss_fwd_bwd (held-out validation losses): the same struct, workspace, shapes (bf16 logits included)
+ * and choice of kernel, with the gradient phase compiled out.  Writes `losses` (bit-identical to hrl_loss_fwd_bwd on the
+ * same inputs) and the taps that are given; dpolicy_raw, dvalue_raw and dreturn_raw may be NULL and are never written. */
+int hrl_loss_fwd(const HrlLossArgs *args, void *stream);
 
 /*
  * Learner diagnostics (opt-in): additive sums, so that shards add up and the sums can ride the gradient all-reduce.
