@@ -126,7 +126,13 @@ SYMBOLS = {
                            [C.c_double] * 5 + [C.c_void_p, C.c_void_p]),
     'hrl_clip_adam_step_diag': (C.c_int, [C.c_void_p] * 4 + [C.c_int64] + [C.c_void_p] * 3 +
                                 [C.c_double] * 5 + [C.c_void_p, C.c_void_p, C.c_void_p]),
+    'hrl_clip_adam_step_guarded': (C.c_int, [C.c_void_p] * 4 + [C.c_int64] + [C.c_void_p] * 3 + [C.c_double] * 5 +
+                                   [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'hrl_step_commit': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                  C.c_void_p]),
     'hrl_weight_ema': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_int32, C.c_void_p]),
+    'hrl_weight_ema_guarded': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_int32, C.c_void_p,
+                                         C.c_void_p]),
     'hrl_peer_allreduce_sumsq': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int64,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'hrl_bn_workspace_floats': (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),

@@ -36,16 +36,20 @@ __global__ void __launch_bounds__(kOptThreads) grad_sumsq_kernel(const float *__
 }
 
 // DIAG: block 0 also adds g, g^2, [g > max_norm], 1 to diag[0..3] (learner diagnostics, include/hrl_b200.h)
-template <bool DIAG>
+// GUARD: the step is rejected when the fp64 fold of the partials or one of tail[0..n_tail) is not finite.  Every block
+// folds the same partials in the same order and reads the same tail, so every block reaches the same decision on its
+// own; a rejected step writes neither param, the moments nor diag.  Block 0 writes the decision to *skip.
+template <bool DIAG, bool GUARD>
 __global__ void __launch_bounds__(kOptThreads) clip_adam_kernel(
     float *__restrict__ param, const float *__restrict__ grad, float *__restrict__ exp_avg,
     float *__restrict__ exp_avg_sq, int64_t n, const float *__restrict__ partials, const float *__restrict__ lr_p,
     int64_t *step_p, double max_norm_d, double beta1_d, double beta2_d, double eps_d, double wd_d,
-    float *grad_norm_out, double *diag) {
+    float *grad_norm_out, double *diag, const float *__restrict__ tail, int n_tail, int32_t *skip) {
     const float max_norm = (float)max_norm_d, beta2 = (float)beta2_d, eps = (float)eps_d, wd = (float)wd_d;
     // every block folds the partial sums in the same order -> identical clip coefficient everywhere
     __shared__ double red[kOptThreads / 32];
     __shared__ float s_coef;
+    __shared__ int s_reject;
     double acc = 0.0;
     for (int i = threadIdx.x; i < kPartials; i += blockDim.x) acc += (double)partials[i];
     acc = warp_sum_d(acc);
@@ -58,7 +62,14 @@ __global__ void __launch_bounds__(kOptThreads) clip_adam_kernel(
         float coef = max_norm / (total_norm + 1e-6f);  // torch clip_grad_norm_
         s_coef = fminf(coef, 1.0f);
         if (blockIdx.x == 0 && grad_norm_out) *grad_norm_out = total_norm;
-        if (DIAG && blockIdx.x == 0) {
+        bool reject = false;
+        if (GUARD) {
+            reject = !isfinite(s);                      // also a finite gradient whose fp32 sum of squares overflowed
+            for (int i = 0; i < n_tail; i++) reject |= !isfinite(tail[i]);
+            s_reject = reject ? 1 : 0;
+            if (blockIdx.x == 0) *skip = reject ? 1 : 0;
+        }
+        if (DIAG && blockIdx.x == 0 && !reject) {
             diag[0] += (double)total_norm;
             diag[1] += (double)total_norm * (double)total_norm;
             diag[2] += total_norm > max_norm ? 1.0 : 0.0;
@@ -66,6 +77,7 @@ __global__ void __launch_bounds__(kOptThreads) clip_adam_kernel(
         }
     }
     __syncthreads();
+    if (GUARD && s_reject) return;
     const float coef = s_coef;
     const int64_t t = *step_p + 1;
     const float lr = *lr_p;
@@ -179,6 +191,27 @@ __global__ void __launch_bounds__(kOptThreads) peer_allreduce_sumsq_kernel(
 // the step counter is bumped by a 1-thread epilogue so that every block of clip_adam_kernel
 // reads the same value regardless of scheduling
 __global__ void bump_step_kernel(int64_t *step_p) { *step_p += 1; }
+// guarded form: a rejected step is not counted
+__global__ void bump_step_guarded_kernel(int64_t *step_p, const int32_t *skip) { *step_p += *skip ? 0 : 1; }
+
+// After a guarded optimiser step.  Accepted: accum[i] += (double)tail[i], i < n_tail (one rounding, as ATen's fp64 add_
+// of an fp32 tensor).  Rejected: *skip_count += 1, and the saved bytes go back to `state` (the buffers the forward moved).
+__global__ void __launch_bounds__(kOptThreads) step_commit_kernel(const int32_t *__restrict__ skip, const float *__restrict__ tail,
+                                                                  int n_tail, double *__restrict__ accum, double *__restrict__ skip_count,
+                                                                  uint8_t *__restrict__ state, const uint8_t *__restrict__ saved,
+                                                                  int64_t nbytes) {
+    if (*skip == 0) {
+        if (blockIdx.x == 0)
+            for (int i = threadIdx.x; i < n_tail; i += blockDim.x) accum[i] = accum[i] + (double)tail[i];
+        return;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) *skip_count += 1.0;
+    const int64_t n16 = nbytes >> 4;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += (int64_t)gridDim.x * blockDim.x)
+        reinterpret_cast<uint4 *>(state)[i] = reinterpret_cast<const uint4 *>(saved)[i];
+    if (blockIdx.x == 0)
+        for (int64_t i = (n16 << 4) + threadIdx.x; i < nbytes; i += blockDim.x) state[i] = saved[i];
+}
 
 // moving average of the learner's state after the optimiser step: a <- fmaf(w, x - a, a),
 // w = 1 - decay once seeded, else max(1 - decay, 1 / t) with t = *step_p.  w == 1 (the first step)
@@ -186,8 +219,12 @@ __global__ void bump_step_kernel(int64_t *step_p) { *step_p += 1; }
 // the same arithmetic whatever the grid.
 __device__ __forceinline__ float ema_update(float a, float x, float w) { return w == 1.f ? x : fmaf(w, x - a, a); }
 
+// GUARD: nothing happens when *skip says the optimiser step was rejected
+template <bool GUARD>
 __global__ void __launch_bounds__(kOptThreads) weight_ema_kernel(float *__restrict__ avg, const float *__restrict__ state, int64_t n,
-                                                                 const int64_t *__restrict__ step_p, float decay, int seeded) {
+                                                                 const int64_t *__restrict__ step_p, float decay, int seeded,
+                                                                 const int32_t *__restrict__ skip) {
+    if (GUARD && *skip) return;
     const float keep = 1.f - decay;
     const int64_t t = *step_p;
     const float w = seeded ? keep : fmaxf(keep, 1.f / (float)(t > 1 ? t : 1));
@@ -236,20 +273,27 @@ extern "C" int hrl_grad_sumsq(const float *grad, int64_t n, float *partials, voi
 }
 
 namespace hrl {
-template <bool DIAG>
+template <bool DIAG, bool GUARD>
 static int clip_adam_step(const char *name, float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
                           const float *partials, const float *lr, int64_t *step, double max_norm, double beta1, double beta2,
-                          double eps, double weight_decay, float *grad_norm_out, double *diag, void *stream) {
+                          double eps, double weight_decay, float *grad_norm_out, double *diag, const float *tail, int32_t n_tail,
+                          int32_t *skip, void *stream) {
     HRL_REQUIRE(param && grad && exp_avg && exp_avg_sq && partials && lr && step && n > 0, HRL_ERR_BAD_ARG,
                 "%s: NULL pointer or n <= 0", name);
     HRL_REQUIRE(!DIAG || diag, HRL_ERR_BAD_ARG, "%s: diag_accum is NULL", name);
+    HRL_REQUIRE(!GUARD || (skip && n_tail >= 0 && (tail || n_tail == 0)), HRL_ERR_BAD_ARG,
+                "%s: skip is NULL, or tail is NULL with n_tail > 0, or n_tail < 0", name);
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     int grid = (int)((n + kOptThreads - 1) / kOptThreads);
     if (grid > kPartials) grid = kPartials;
-    clip_adam_kernel<DIAG><<<grid, kOptThreads, 0, s>>>(param, grad, exp_avg, exp_avg_sq, n, partials, lr, step, max_norm,
-                                                        beta1, beta2, eps, weight_decay, grad_norm_out, diag);
+    clip_adam_kernel<DIAG, GUARD><<<grid, kOptThreads, 0, s>>>(param, grad, exp_avg, exp_avg_sq, n, partials, lr, step, max_norm,
+                                                               beta1, beta2, eps, weight_decay, grad_norm_out, diag, tail,
+                                                               n_tail, skip);
     HRL_CUDA_CHECK(cudaGetLastError());
-    bump_step_kernel<<<1, 1, 0, s>>>(step);
+    if (GUARD)
+        bump_step_guarded_kernel<<<1, 1, 0, s>>>(step, skip);
+    else
+        bump_step_kernel<<<1, 1, 0, s>>>(step);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
 }
@@ -258,31 +302,76 @@ static int clip_adam_step(const char *name, float *param, const float *grad, flo
 extern "C" int hrl_clip_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
                                   const float *partials, const float *lr, int64_t *step, double max_norm, double beta1,
                                   double beta2, double eps, double weight_decay, float *grad_norm_out, void *stream) {
-    return hrl::clip_adam_step<false>("hrl_clip_adam_step", param, grad, exp_avg, exp_avg_sq, n, partials, lr, step, max_norm,
-                                      beta1, beta2, eps, weight_decay, grad_norm_out, nullptr, stream);
+    return hrl::clip_adam_step<false, false>("hrl_clip_adam_step", param, grad, exp_avg, exp_avg_sq, n, partials, lr, step,
+                                             max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, nullptr, nullptr, 0,
+                                             nullptr, stream);
 }
 
 extern "C" int hrl_clip_adam_step_diag(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
                                        const float *partials, const float *lr, int64_t *step, double max_norm, double beta1,
                                        double beta2, double eps, double weight_decay, float *grad_norm_out, double *diag_accum,
                                        void *stream) {
-    return hrl::clip_adam_step<true>("hrl_clip_adam_step_diag", param, grad, exp_avg, exp_avg_sq, n, partials, lr, step,
-                                     max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, diag_accum, stream);
+    return hrl::clip_adam_step<true, false>("hrl_clip_adam_step_diag", param, grad, exp_avg, exp_avg_sq, n, partials, lr, step,
+                                            max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, diag_accum, nullptr, 0,
+                                            nullptr, stream);
 }
 
-extern "C" int hrl_weight_ema(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
-                              void *stream) {
+extern "C" int hrl_clip_adam_step_guarded(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
+                                          const float *partials, const float *lr, int64_t *step, double max_norm, double beta1,
+                                          double beta2, double eps, double weight_decay, float *grad_norm_out,
+                                          const float *tail, int32_t n_tail, double *diag_accum, int32_t *skip, void *stream) {
+    if (diag_accum)
+        return hrl::clip_adam_step<true, true>("hrl_clip_adam_step_guarded", param, grad, exp_avg, exp_avg_sq, n, partials, lr,
+                                               step, max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, diag_accum, tail,
+                                               n_tail, skip, stream);
+    return hrl::clip_adam_step<false, true>("hrl_clip_adam_step_guarded", param, grad, exp_avg, exp_avg_sq, n, partials, lr,
+                                            step, max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, nullptr, tail,
+                                            n_tail, skip, stream);
+}
+
+extern "C" int hrl_step_commit(const int32_t *skip, const float *tail, int32_t n_tail, double *accum, double *skip_count,
+                               void *state, const void *saved, int64_t nbytes, void *stream) {
     using namespace hrl;
-    HRL_REQUIRE(avg && state && step && n > 0, HRL_ERR_BAD_ARG, "hrl_weight_ema: NULL pointer or n <= 0");
+    HRL_REQUIRE(skip && skip_count && n_tail >= 0 && nbytes >= 0, HRL_ERR_BAD_ARG,
+                "hrl_step_commit: skip or skip_count is NULL, or a negative size");
+    HRL_REQUIRE(n_tail == 0 || (tail && accum), HRL_ERR_BAD_ARG, "hrl_step_commit: tail or accum is NULL with n_tail > 0");
+    HRL_REQUIRE(nbytes == 0 || (state && saved), HRL_ERR_BAD_ARG, "hrl_step_commit: state or saved is NULL with nbytes > 0");
+    HRL_REQUIRE(((reinterpret_cast<uintptr_t>(state) | reinterpret_cast<uintptr_t>(saved)) & 15) == 0, HRL_ERR_BAD_ARG,
+                "hrl_step_commit: state and saved must be 16-byte aligned");
+    int64_t grid = ((nbytes >> 4) + kOptThreads - 1) / kOptThreads;
+    if (grid < 1) grid = 1;
+    if (grid > 4 * kNumSM) grid = 4 * kNumSM;
+    step_commit_kernel<<<(int)grid, kOptThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
+        skip, tail, n_tail, accum, skip_count, static_cast<uint8_t *>(state), static_cast<const uint8_t *>(saved), nbytes);
+    HRL_CUDA_CHECK(cudaGetLastError());
+    return HRL_OK;
+}
+
+namespace hrl {
+template <bool GUARD>
+static int weight_ema(const char *name, float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
+                      const int32_t *skip, void *stream) {
+    HRL_REQUIRE(avg && state && step && n > 0 && (!GUARD || skip), HRL_ERR_BAD_ARG, "%s: NULL pointer or n <= 0", name);
     HRL_REQUIRE(((reinterpret_cast<uintptr_t>(avg) | reinterpret_cast<uintptr_t>(state)) & 15) == 0, HRL_ERR_BAD_ARG,
-                "hrl_weight_ema: avg and state must be 16-byte aligned");
-    HRL_REQUIRE(decay > 0.f && decay < 1.f, HRL_ERR_BAD_ARG, "hrl_weight_ema: decay must lie in (0, 1), got %g", (double)decay);
+                "%s: avg and state must be 16-byte aligned", name);
+    HRL_REQUIRE(decay > 0.f && decay < 1.f, HRL_ERR_BAD_ARG, "%s: decay must lie in (0, 1), got %g", name, (double)decay);
     const int64_t n4 = n >> 2;
     int64_t grid = (n4 + kOptThreads - 1) / kOptThreads;
     if (grid < 1) grid = 1;                     // n < 4: block 0 does the tail alone
     if (grid > 4 * kNumSM) grid = 4 * kNumSM;
-    weight_ema_kernel<<<(int)grid, kOptThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(avg, state, n, step, decay,
-                                                                                             seeded ? 1 : 0);
+    weight_ema_kernel<GUARD><<<(int)grid, kOptThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(avg, state, n, step, decay,
+                                                                                                    seeded ? 1 : 0, skip);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
+}
+}  // namespace hrl
+
+extern "C" int hrl_weight_ema(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
+                              void *stream) {
+    return hrl::weight_ema<false>("hrl_weight_ema", avg, state, n, step, decay, seeded, nullptr, stream);
+}
+
+extern "C" int hrl_weight_ema_guarded(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
+                                      const int32_t *skip, void *stream) {
+    return hrl::weight_ema<true>("hrl_weight_ema_guarded", avg, state, n, step, decay, seeded, skip, stream);
 }

@@ -332,6 +332,11 @@ class FlatAdam:
         # diagnostics: a float64 CUDA tensor of 4 (the gnorm, gnorm2, gclip, steps entries of a DIAG_KEYS accumulator) that
         # every step adds its pre-clip norm statistics to, in the step's own launch; None = off
         self.diag = None
+        # guard against non-finite steps: a one-element int32 CUDA tensor the step sets to 1 when it rejected itself (the
+        # pre-clip norm or one of the first `guard_tail` extra slots of the bucket not finite; hrl_clip_adam_step_guarded),
+        # else 0; None = off
+        self.skip = None
+        self.guard_tail = 0
 
     @property
     def extra_slots(self):
@@ -355,6 +360,12 @@ class FlatAdam:
                  _ptr(self.grad_norm))
         if self.diag is not None:
             assert self.diag.is_cuda and self.diag.dtype == torch.float64 and self.diag.numel() == 4 and self.diag.is_contiguous()
+        if self.skip is not None:
+            assert self.skip.is_cuda and self.skip.dtype == torch.int32 and self.skip.numel() == 1
+            assert 0 <= self.guard_tail <= self.extra and grad.numel() >= self.n_pad + self.extra
+            check(lib().hrl_clip_adam_step_guarded(*fixed, _ptr(grad[self.n_pad:]), self.guard_tail, _ptr(self.diag),
+                                                   _ptr(self.skip), s))
+        elif self.diag is not None:
             check(lib().hrl_clip_adam_step_diag(*fixed, _ptr(self.diag), s))
         else:
             check(lib().hrl_clip_adam_step(*fixed, s))
@@ -368,9 +379,15 @@ class FlatAdam:
         fastnet.new_step()          # cached adjoint weights of the convolutions are stale now
 
 
-def weight_ema_update(avg, state_f32, step_count, decay, seeded):
+def _check_skip(skip):
+    if not (skip.is_cuda and skip.dtype == torch.int32 and skip.numel() == 1):
+        raise _capi.HrlError('handyrl_b200: skip must be a one-element int32 CUDA tensor')
+
+
+def weight_ema_update(avg, state_f32, step_count, decay, seeded, skip=None):
     """avg <- fmaf(w, state_f32 - avg, avg) in place, w = max(1 - decay, 1 / t) (1 - decay when `seeded`), t = the int64 device
-    counter `step_count` as it stands when the launch runs (hrl_weight_ema, csrc/optim_kernel.cu).  One launch, graph-capturable."""
+    counter `step_count` as it stands when the launch runs (hrl_weight_ema, csrc/optim_kernel.cu).  One launch, graph-capturable.
+    `skip` (FlatAdam.skip of a guarded optimiser): the launch changes nothing when that step was rejected (hrl_weight_ema_guarded)."""
     for t, name in ((avg, 'avg'), (state_f32, 'state_f32')):
         if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
             raise _capi.HrlError('handyrl_b200: %s must be a contiguous float32 CUDA tensor' % name)
@@ -378,8 +395,44 @@ def weight_ema_update(avg, state_f32, step_count, decay, seeded):
         raise _capi.HrlError('handyrl_b200: avg (%d) and state_f32 (%d) differ in size' % (avg.numel(), state_f32.numel()))
     if not (step_count.is_cuda and step_count.dtype == torch.int64 and step_count.numel() == 1):
         raise _capi.HrlError('handyrl_b200: step_count must be a one-element int64 CUDA tensor')
-    check(lib().hrl_weight_ema(_ptr(avg), _ptr(state_f32), avg.numel(), _ptr(step_count), float(decay), int(bool(seeded)),
-                               _stream_ptr()))
+    if skip is None:
+        check(lib().hrl_weight_ema(_ptr(avg), _ptr(state_f32), avg.numel(), _ptr(step_count), float(decay), int(bool(seeded)),
+                                   _stream_ptr()))
+    else:
+        _check_skip(skip)
+        check(lib().hrl_weight_ema_guarded(_ptr(avg), _ptr(state_f32), avg.numel(), _ptr(step_count), float(decay),
+                                           int(bool(seeded)), _ptr(skip), _stream_ptr()))
+    _count()
+
+
+def step_commit(skip, tail, accum, skip_count, state=None, saved=None):
+    """What follows a guarded optimiser step (hrl_step_commit, one launch reading the device flag `skip`): when the step was
+    accepted, accum[:tail.numel()] += tail (float32 sums into the float64 accumulator, as ATen's add_ does); when it was
+    rejected, skip_count += 1 and the bytes of `saved` go back to `state` (both uint8 CUDA tensors of one size, or None)."""
+    _check_skip(skip)
+    if not (tail.is_cuda and tail.dtype == torch.float32 and tail.is_contiguous()):
+        raise _capi.HrlError('handyrl_b200: tail must be a contiguous float32 CUDA tensor')
+    for t, name in ((accum, 'accum'), (skip_count, 'skip_count')):
+        if not (t.is_cuda and t.dtype == torch.float64 and t.is_contiguous()):
+            raise _capi.HrlError('handyrl_b200: %s must be a contiguous float64 CUDA tensor' % name)
+    if accum.numel() < tail.numel() or skip_count.numel() != 1:
+        raise _capi.HrlError('handyrl_b200: accum holds %d of the %d tail sums, or skip_count is not one element'
+                             % (accum.numel(), tail.numel()))
+    lo, hi = skip_count.data_ptr(), skip_count.data_ptr() + 8
+    if tail.numel() and lo < accum.data_ptr() + 8 * tail.numel() and accum.data_ptr() < hi:
+        raise _capi.HrlError('handyrl_b200: skip_count lies inside the accumulated sums')
+    nbytes = 0
+    if state is not None or saved is not None:
+        if state is None or saved is None:
+            raise _capi.HrlError('handyrl_b200: state and saved come in pairs')
+        for t, name in ((state, 'state'), (saved, 'saved')):
+            if not (t.is_cuda and t.dtype == torch.uint8 and t.is_contiguous()):
+                raise _capi.HrlError('handyrl_b200: %s must be a contiguous uint8 CUDA tensor' % name)
+        if state.numel() != saved.numel():
+            raise _capi.HrlError('handyrl_b200: state (%d) and saved (%d) differ in size' % (state.numel(), saved.numel()))
+        nbytes = state.numel()
+    check(lib().hrl_step_commit(_ptr(skip), _ptr(tail), tail.numel(), _ptr(accum), _ptr(skip_count),
+                                _ptr(state) if nbytes else None, _ptr(saved) if nbytes else None, nbytes, _stream_ptr()))
     _count()
 
 

@@ -324,6 +324,23 @@ def validation_rate(args):
     return float(value)
 
 
+def nonfinite_guard(args):
+    """train_args['skip_nonfinite'] -> whether optimiser steps whose loss or gradient is not finite are rejected on the device
+    (key absent, False or None: off)."""
+    return bool(args.get('skip_nonfinite'))
+
+
+def accum_slots(diagnostics, skip_nonfinite):
+    """Float64 slots of the learner's epoch accumulator (LearnerStep.accum): the NUM_LOSS loss sums, then the NUM_DIAG
+    diagnostics sums when diagnostics are on, then the count of rejected steps when the guard is on."""
+    return NUM_LOSS + (NUM_DIAG if diagnostics else 0) + (1 if skip_nonfinite else 0)
+
+
+def skipped_line(skipped, steps):
+    """'skipped = 3 of 1200 steps: non-finite loss or gradient': the steps of an epoch the guard rejected."""
+    return 'skipped = %d of %d steps: non-finite loss or gradient' % (skipped, steps)
+
+
 def loss_line(name, sums, heads):
     """'<name> = p:0.512 v:0.231 ent:1.843 total:0.561': each head's sum over the sums' own sample count dcnt, as the Trainer
     prints its training loss (train.py:392)."""
@@ -469,35 +486,50 @@ class PendingModel:
     like the model's, in `ema_state`; with the optimiser state (`host_optim`, LearnerStep.end_epoch's layout), it leaves
     that state in the OptimizerStateFormat dict in `optim_state`, scheduled at step count `steps`.  With validation passes
     (`host_val`), it prints their lines after the loss line and leaves their sums in `validation` (what
-    LearnerStep.pop_validation() returns)."""
+    LearnerStep.pop_validation() returns).  `host_losses` holds the learner's accumulator in the layout `diagnostics` and
+    `skip_nonfinite` give (accum_slots); with the guard, the number of the epoch's `batch_cnt` steps that were rejected is left
+    in `skipped` and, when it is not zero, printed (skipped_line) after the loss and diagnostics lines."""
 
     def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host_avg=None, host_optim=None,
-                 steps=0, host_val=None):
+                 steps=0, host_val=None, diagnostics=False, skip_nonfinite=False, batch_cnt=0):
         self.stepper, self.done, self.host_state, self.host_losses = stepper, done_event, host_state, host_losses
         self.heads, self.template, self.host_avg = heads, template, host_avg
         self.host_optim, self.steps = host_optim, steps
         self.host_val = host_val
+        self.has_diagnostics, self.skip_nonfinite, self.batch_cnt = bool(diagnostics), bool(skip_nonfinite), batch_cnt
         self.ema_state = None
         self.optim_state = None
         self.validation = None
+        self.skipped = 0
 
-    def resolve(self):
-        self.done.synchronize()
+    def report(self):
+        """Read the epoch's sums from the host copy (already arrived) and print the epoch's lines; returns the loss sums."""
         host = self.host_losses.tolist()
+        if len(host) != accum_slots(self.has_diagnostics, self.skip_nonfinite):
+            raise ValueError('PendingModel: %d accumulator slots, the layout has %d'
+                             % (len(host), accum_slots(self.has_diagnostics, self.skip_nonfinite)))
         sums = dict(zip(LOSS_KEYS, host[:NUM_LOSS]))
         dcnt = sums['dcnt']
         self.diagnostics = None
-        if len(host) > NUM_LOSS:        # the learner's diagnostics sums ride behind the loss sums
-            self.diagnostics = ops.summarize_diagnostics(host[NUM_LOSS:])
+        if self.has_diagnostics:        # the learner's diagnostics sums ride behind the loss sums
+            self.diagnostics = ops.summarize_diagnostics(host[NUM_LOSS:NUM_LOSS + NUM_DIAG])
+        self.skipped = int(host[-1]) if self.skip_nonfinite else 0
         if dcnt > 0:
             print(loss_line('loss', sums, self.heads))
             if self.diagnostics is not None:
                 print(ops.format_diagnostics(self.diagnostics))
+        if self.skipped:
+            print(skipped_line(self.skipped, self.batch_cnt))
         if self.host_val is not None:
             self.validation = self.stepper.validation_sums(self.host_val.tolist())
             for name, val in self.validation.items():
                 if val['dcnt'] > 0:
                     print(loss_line(name, val, self.heads))
+        return sums
+
+    def resolve(self):
+        self.done.synchronize()
+        sums = self.report()
         tpl = self.template
         store = self.stepper.state
         keys = list(tpl.state_dict().keys())
@@ -558,22 +590,32 @@ class LearnerStep:
     num_batches_tracked) are saved and restored around the pass on the device.  In graph mode each form is one more CUDA
     graph sharing the step graph's memory pool; `launches_per_validation` counts its launches.  end_epoch hands the sums
     over with the loss sums (PendingModel.validation); pop_validation() reads them now.
+
+    skip_nonfinite (default: train_args['skip_nonfinite'], off): a step whose pre-clip gradient norm or one of whose six loss
+    sums is not finite is rejected on the device (ops.FlatAdam.skip, hrl_clip_adam_step_guarded), and the learner is left
+    bit for bit as if its batch had never been drawn: weights, Adam's moments and step count, the BatchNorm buffers (saved by
+    one device-to-device copy at the start of every step and put back by hrl_step_commit), the epoch's loss and diagnostics
+    sums and the weight average.  Only the count of rejected steps (`skipped`, the accumulator's last slot; handed over as
+    PendingModel.skipped) goes up, and last_losses still holds the rejected step's sums.  `steps` and the host's batch counts
+    keep counting batches drawn; a rejected batch adds nothing to dcnt.  One more launch per step.  Validation passes are not
+    guarded.
     """
 
     def __init__(self, model, args, example_batch, lr, device=None, process_group=None, use_graph=True,
                  max_norm=4.0, weight_decay=1e-5, time_loss_kernel=False, channels_last=True, cudnn_benchmark=True,
                  small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None,
-                 weight_ema=None, save_optimizer=None, validation=None):
+                 weight_ema=None, save_optimizer=None, validation=None, skip_nonfinite=None):
         self.weight_ema = weight_ema_decay(args.get('weight_ema') if weight_ema is None else weight_ema)
         rate = validation_rate(args)
         self.validation = bool(rate is not None if validation is None else validation)
         self.save_optimizer = bool(args.get('save_optimizer', False) if save_optimizer is None else save_optimizer)
+        self.skip_nonfinite = nonfinite_guard(args) if skip_nonfinite is None else bool(skip_nonfinite)
         self.device = torch.device(device if device is not None else 'cuda')
         self.args = args
         if diagnostics is None:
             diagnostics = bool(args.get('diagnostics', False))
         self.diagnostics = diagnostics
-        n_sums = NUM_LOSS + (NUM_DIAG if diagnostics else 0)                # accumulator: loss sums [+ diagnostics sums]
+        n_sums = accum_slots(diagnostics, self.skip_nonfinite)             # accumulator: loss sums [+ diagnostics] [+ skips]
         n_tail = NUM_LOSS + (NUM_LOSS_DIAG if diagnostics else 0)           # bucket tail: [+ the loss pass's diagnostics]
         # the learner owns its precision contract (1e-5 of the reference's fp32 arithmetic): PyTorch's default lets
         # cuDNN convolutions run on TF32 tensor cores (10-bit mantissa).  train_args['allow_tf32'] = True opts out.
@@ -671,8 +713,17 @@ class LearnerStep:
         self.loss_accum = self.accum[:NUM_LOSS]
         self.diag_accum = None
         if diagnostics:
-            self.diag_accum = self.accum[NUM_LOSS:]
+            self.diag_accum = self.accum[NUM_LOSS:NUM_LOSS + NUM_DIAG]
             self.opt.diag = self.diag_accum[NUM_LOSS_DIAG:]        # the optimiser's entries: accumulated by its own kernel
+        # guard against non-finite steps: the count of rejected steps is the accumulator's last slot; the buffers the forward
+        # moves (StateStore bytes [f_off, nbytes)) are saved at the start of every step and put back when it is rejected
+        self.skipped = self.guard_saved = None
+        if self.skip_nonfinite:
+            self.skipped = self.accum[n_sums - 1:]
+            self.opt.skip = torch.zeros(1, dtype=torch.int32, device=self.device)
+            self.opt.guard_tail = NUM_LOSS
+            if self.state.nbytes > self.state.f_off:
+                self.guard_saved = torch.empty(self.state.nbytes - self.state.f_off, dtype=torch.uint8, device=self.device)
         self.host_slots = torch.zeros((8, NUM_LOSS)).pin_memory()
         self._slot = 0
         self.graph = self.graph_fwd = self.graph_bwd = None
@@ -698,6 +749,8 @@ class LearnerStep:
 
     # -- the device work of one step, on the current stream (inputs already in self.dev)
     def _part_forward(self):
+        if self.guard_saved is not None:        # one device-to-device copy: what a rejected step puts back
+            self.guard_saved.copy_(self._guarded_buffers())
         fastnet.new_step()          # adjoint-weight copies of the previous step are stale: the optimiser has run
         self.opt.zero_grad()
         if self.engine is not None:
@@ -744,12 +797,22 @@ class LearnerStep:
             self.opt.step()
             tail = self.opt.extra_slots
             self.last_losses.copy_(tail[:NUM_LOSS])
-        self.loss_accum.add_(self.last_losses)
-        if self.diagnostics:
-            self.diag_accum[:NUM_LOSS_DIAG].add_(tail[NUM_LOSS:NUM_LOSS + NUM_LOSS_DIAG])
+        if self.skip_nonfinite:         # one launch: accumulate an accepted step, or count a rejected one and restore its buffers
+            n_tail = NUM_LOSS + (NUM_LOSS_DIAG if self.diagnostics else 0)
+            ops.step_commit(self.opt.skip, tail[:n_tail], self.accum, self.skipped,
+                            self._guarded_buffers() if self.guard_saved is not None else None, self.guard_saved)
+        else:
+            self.loss_accum.add_(self.last_losses)
+            if self.diagnostics:
+                self.diag_accum[:NUM_LOSS_DIAG].add_(tail[NUM_LOSS:NUM_LOSS + NUM_LOSS_DIAG])
         if self.avg is not None:        # after the optimiser: step_count already counts this step
             ops.weight_ema_update(self.avg, self.state.bytes[:self.state.i_off].view(torch.float32), self.opt.step_count,
-                                  self.weight_ema, self.avg_seeded)
+                                  self.weight_ema, self.avg_seeded, skip=self.opt.skip)
+
+    def _guarded_buffers(self):
+        """The buffers a step's forward moves (BatchNorm running statistics, num_batches_tracked): StateStore bytes
+        [f_off, nbytes)."""
+        return self.state.bytes[self.state.f_off:self.state.nbytes]
 
     def _device_step(self):
         self._part_forward()
@@ -831,13 +894,16 @@ class LearnerStep:
 
     def _snapshot(self):
         bufs = {k: v.clone() for k, v in self.model.state_dict().items()}
+        guard = None
+        if self.skip_nonfinite:         # (the skip count rides in accum)
+            guard = (self.opt.skip.clone(), self.guard_saved.clone() if self.guard_saved is not None else None)
         return (bufs, self.opt.exp_avg.clone(), self.opt.exp_avg_sq.clone(), self.opt.step_count.clone(),
-                self.accum.clone(), self.avg.clone() if self.avg is not None else None)
+                self.accum.clone(), self.avg.clone() if self.avg is not None else None, guard)
 
     def _restore(self, state):
         if self.val_accum_all is not None:
             self.val_accum_all.zero_()
-        bufs, m, v, sc, acc, avg = state
+        bufs, m, v, sc, acc, avg, guard = state
         with torch.no_grad():
             for k, t in self.model.state_dict().items():
                 t.copy_(bufs[k])
@@ -847,6 +913,10 @@ class LearnerStep:
             self.accum.copy_(acc)
             if avg is not None:
                 self.avg.copy_(avg)
+            if guard is not None:
+                self.opt.skip.copy_(guard[0])
+                if guard[1] is not None:
+                    self.guard_saved.copy_(guard[1])
 
     def new_packed(self):
         return PackedBatch(self.layout)
@@ -1143,7 +1213,8 @@ class LearnerStep:
             done.record(self.copy_stream)
         self._last_done = done
         return PendingModel(self, done, host_state, host_losses, heads, template, host_avg=host_avg, host_optim=host_optim,
-                            steps=int(steps), host_val=host_val)
+                            steps=int(steps), host_val=host_val, diagnostics=self.diagnostics,
+                            skip_nonfinite=self.skip_nonfinite, batch_cnt=batch_cnt)
 
 
 # --------------------------------------------------------------------------- batcher + trainer
@@ -1501,7 +1572,13 @@ class Trainer:
     after every round(1 / r)-th step one batch of held-out windows is evaluated with the live weights (and with their moving
     average under weight_ema) without an update (LearnerStep.validate_in_place).  Each epoch prints 'validation = ...' (and
     'validation_ema = ...') after the loss line, in its format, once the held-out ring holds an episode.  Only rank 0
-    validates; every rank leaves the held-out episodes out of its training ring."""
+    validates; every rank leaves the held-out episodes out of its training ring.
+
+    train_args['skip_nonfinite'] = True: a step whose loss or gradient is not finite (a NaN or Inf from an environment's
+    observation, reward or outcome) is rejected on the device and leaves the learner as it was (LearnerStep).  Each epoch
+    that rejected a step prints 'skipped = <n> of <steps> steps: non-finite loss or gradient' after the loss (and
+    diagnostics) line, even when update() drops the epoch.  `steps` keeps counting batches drawn.  Every rank sees the same
+    all-reduced bucket, so all ranks reject alike."""
 
     def __init__(self, args, model):
         self.weight_ema = weight_ema_decay(args.get('weight_ema'))

@@ -18,6 +18,9 @@
  *   hrl_grad_sumsq /
  *   hrl_clip_adam_step    <- handyrl/train.py:370-371 (clip_grad_norm_(params, 4.0) + Adam.step,
  *                            Adam(lr, weight_decay=1e-5) of train.py:331)
+ *   hrl_clip_adam_step_guarded /
+ *   hrl_step_commit       <- the same step, rejected on the device when its loss or gradient is not finite; no
+ *                            reference counterpart
  *   hrl_weight_ema        <- a per-step moving average of the weights; no reference counterpart (scripts/aux_swa.py
  *                            averages epoch checkpoints)
  *   hrl_gather_pad        <- handyrl/train.py:33-124  (make_batch: window slice + pad + collate)
@@ -216,6 +219,32 @@ int hrl_clip_adam_step_diag(float *param, const float *grad, float *exp_avg, flo
                             float *grad_norm_out /* may be NULL */, double *diag_accum, void *stream);
 
 /*
+ * Guarded form of the same step (opt-in; a batch carrying a NaN or Inf must not poison the learner).  The step is rejected
+ * when the pre-clip norm -- the fp64 fold of the fp32 partials -- is not finite, or when one of tail[0 .. n_tail) is not
+ * finite (tail: the loss sums in the reduced bucket).  A finite gradient whose fp32 sum of squares overflows makes a
+ * partial Inf, so it is rejected too.  Every block folds the same partials and reads the same tail, so all blocks (and all
+ * ranks of a sharded learner, which see the same reduced bucket) decide alike without communicating.
+ *   accepted: the arithmetic of hrl_clip_adam_step (hrl_clip_adam_step_diag when diag_accum != NULL), bit for bit;
+ *   rejected: param, exp_avg, exp_avg_sq and diag_accum are not written, and *step is not incremented.
+ * *grad_norm_out is written either way.  *skip (device int32) is set to 1 when rejected, 0 when accepted.
+ */
+int hrl_clip_adam_step_guarded(float *param, const float *grad, float *exp_avg, float *exp_avg_sq,
+                               int64_t n, const float *partials, const float *lr, int64_t *step,
+                               double max_norm, double beta1, double beta2, double eps, double weight_decay,
+                               float *grad_norm_out /* may be NULL */, const float *tail, int32_t n_tail,
+                               double *diag_accum /* may be NULL */, int32_t *skip, void *stream);
+
+/*
+ * The accumulation that follows a guarded step, in one launch that reads *skip:
+ *   accepted: accum[i] += (double)tail[i] for i < n_tail (the epoch's loss sums, then the loss pass's diagnostics sums);
+ *   rejected: *skip_count += 1, and nbytes bytes of `saved` are copied back to `state` (the buffers -- BatchNorm running
+ *             statistics, num_batches_tracked -- as they were before the step's forward moved them).
+ * skip_count must not lie in accum[0 .. n_tail).  state and saved are 16-byte aligned; nbytes may be 0.
+ */
+int hrl_step_commit(const int32_t *skip, const float *tail, int32_t n_tail, double *accum, double *skip_count,
+                    void *state, const void *saved, int64_t nbytes, void *stream);
+
+/*
  * Moving average of the learner's weights (opt-in, no reference counterpart; reference scripts/aux_swa.py averages
  * epoch checkpoints instead).  Enqueued after the optimiser step, on the n fp32 words of the learner's state -- the
  * parameters (zero pad included) and the fp32 buffers (BatchNorm running statistics):
@@ -226,6 +255,9 @@ int hrl_clip_adam_step_diag(float *param, const float *grad, float *exp_avg, flo
  * deterministic; avg and state 16-byte aligned, any n > 0, decay in (0, 1).
  */
 int hrl_weight_ema(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded, void *stream);
+/* The same after a guarded step: nothing is written when *skip (hrl_clip_adam_step_guarded) says the step was rejected. */
+int hrl_weight_ema_guarded(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
+                           const int32_t *skip, void *stream);
 
 /*
  * Multi-GPU form of the same step: one-shot all-reduce (SUM) of the flat gradient bucket over NVLink peer
