@@ -139,6 +139,7 @@ SYMBOLS = {
     'hrl_bn_train_fwd': (C.c_int, [C.c_void_p] * 8 + [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_float, C.c_float, C.c_void_p, C.c_void_p]),
     'hrl_bn_train_bwd': (C.c_int, [C.c_void_p] * 8 + [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     'hrl_gather_pad': (C.c_int, [C.POINTER(HrlGatherArgs), C.c_void_p]),
+    'hrl_gather_pad_sym': (C.c_int, [C.POINTER(HrlGatherArgs)] + [C.c_void_p] * 4 + [C.c_int32, C.c_void_p]),
     'hrl_gemm_workspace_floats': (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64, C.c_int32]),
     'hrl_gemm_tf32x3': (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
                                    C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),

@@ -267,9 +267,13 @@ class DeviceReplay:
                 win[b]['player'] = rng.choice(range(self.Ps))
         return win
 
-    def gather(self, windows, args, out=None):
+    def gather(self, windows, args, out=None, sym=None, tables=None):
         """Run the gather/pad kernel for an array of WINDOW_DTYPE descriptors; returns the batch dict
-        (observation as the concatenated-leaf tensor; see split_observation)."""
+        (observation as the concatenated-leaf tensor; see split_observation).
+
+        sym (with tables, a symmetry.SymmetryTables): the transform of each window, an int32 array of B values in [0, K)
+        (checked here) or an int32 device tensor the caller has checked; the batch is then gathered through those
+        transforms (hrl_gather_pad_sym).  sym=None: the plain gather (hrl_gather_pad)."""
         B = len(windows)
         T, P, Pa, alternating = self.batch_shapes(args)
         if out is None:
@@ -293,7 +297,27 @@ class DeviceReplay:
         g.outcome, g.reward, g.ret = ptr(out['outcome']), ptr(out['reward']), ptr(out['return'])
         g.episode_mask, g.turn_mask, g.observation_mask = ptr(out['episode_mask']), ptr(out['turn_mask']), ptr(out['observation_mask'])
         g.action_mask, g.progress = ptr(out['action_mask']), ptr(out['progress'])
-        check(lib().hrl_gather_pad(C.byref(g), C.c_void_p(torch.cuda.current_stream().cuda_stream)))
+        stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        if sym is None:
+            check(lib().hrl_gather_pad(C.byref(g), stream))
+        else:
+            if tables is None:
+                raise ValueError('gather: sym needs the transform tables')
+            if not torch.is_tensor(sym):
+                sym = np.ascontiguousarray(sym, np.int32)
+                if sym.shape != (B,):
+                    raise ValueError('gather: sym must hold one transform per window (%d); got shape %s' % (B, sym.shape))
+                tables.check_sym(sym)
+                sym = torch.from_numpy(sym).to(self.device, non_blocking=True)
+            elif sym.dtype != torch.int32 or sym.numel() != B or not sym.is_contiguous():
+                raise ValueError('gather: sym must be a contiguous int32 tensor of %d transforms' % B)
+            if tables.OE != self.OE or tables.A != self.A:
+                raise ValueError('gather: the tables are for OE=%d, A=%d; the replay stores OE=%d, A=%d'
+                                 % (tables.OE, tables.A, self.OE, self.A))
+            t = tables.device(self.device)
+            check(lib().hrl_gather_pad_sym(C.byref(g), ptr(sym), ptr(t['obs_src']), ptr(t['act_src']), ptr(t['act_dst']),
+                                           tables.K, stream))
+            out['_sym'] = sym       # keep the transform buffer alive until the kernel has run
         from . import ops
         ops._count()
         out['_windows'] = wdev      # keep the descriptor buffer alive until the kernel has run

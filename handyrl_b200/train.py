@@ -27,7 +27,7 @@ from collections import deque
 import numpy as np
 import torch
 
-from . import ops, fastnet
+from . import ops, fastnet, symmetry
 from .batch import tree_map, tree_leaves, make_batch, gather_windows, sample_window
 from ._capi import DIAG_KEYS, LOSS_KEYS, NUM_DIAG, NUM_LOSS, NUM_LOSS_DIAG
 
@@ -607,6 +607,7 @@ class LearnerStep:
                  weight_ema=None, save_optimizer=None, validation=None, skip_nonfinite=None):
         self.weight_ema = weight_ema_decay(args.get('weight_ema') if weight_ema is None else weight_ema)
         rate = validation_rate(args)
+        symmetry.config(args)           # malformed train_args['symmetry'] fails here; the gather applies it, not the step
         self.validation = bool(rate is not None if validation is None else validation)
         self.save_optimizer = bool(args.get('save_optimizer', False) if save_optimizer is None else save_optimizer)
         self.skip_nonfinite = nonfinite_guard(args) if skip_nonfinite is None else bool(skip_nonfinite)
@@ -1348,6 +1349,20 @@ class EpisodeDeque(deque):
             self.append(ep)
 
 
+def sample_batch(replay, B, args, rng, sym_rng=None, K=0):
+    """The draws of one GPU-replay batch: B window descriptors from `rng` (DeviceReplay.sample_windows) and, with sym_rng,
+    the transform of each window, uniform in [0, K), from that generator alone -- so the descriptors are the same with and
+    without augmentation.  Returns (windows, transforms or None); the transforms are checked here, on the host, because
+    the gather kernel trusts them."""
+    win = replay.sample_windows(B, args, rng)
+    if sym_rng is None:
+        return win, None
+    sym = symmetry.draw(sym_rng, B, K)
+    if sym.size and (sym.min() < 0 or sym.max() >= K):
+        raise ValueError('sample_batch: transform outside [0, %d)' % K)
+    return win, sym
+
+
 class GpuBatcher:
     """Batcher on the GPU-resident replay (replay.py + the gather/pad kernel): arriving episodes are decoded once
     by a feeder thread and uploaded into the device ring; a batch is B window descriptors (drawn with array
@@ -1362,7 +1377,12 @@ class GpuBatcher:
     With train_args['validation_rate'] = r, the episodes replay.held_out() picks (a fraction r, decided from their content)
     never enter the training ring: they go to a second DeviceReplay, `val_replay`, of r times the ring's steps and
     r * maximum_episodes episodes, that fill_validation() samples from -- or, with keep_validation=False (helper ranks, which
-    do not validate), nowhere."""
+    do not validate), nowhere.
+
+    With train_args['symmetry'] set (symmetry.py), fill() gathers every window through a transform drawn uniformly from the
+    group by its own generator (symmetry.sampler_rng(seed)): the window descriptors are those drawn without the key.  The
+    tables are built once from the first episode's leaf shapes and uploaded once; the transforms ride in the pinned
+    descriptor slot behind the descriptors, in the same copy.  fill_validation() never augments."""
 
     DESC_SLOTS = 4        # pinned descriptor buffers in rotation: bounds how far the host runs ahead of the GPU
 
@@ -1382,6 +1402,9 @@ class GpuBatcher:
         seed = seed if seed is not None else args.get('seed', 0) * 7919 + 17
         self.rng = np.random.default_rng(seed)
         self.val_rng = np.random.default_rng(seed + 1)      # validation draws leave the training stream alone
+        self.symmetry = symmetry.config(args)
+        self.sym_rng = symmetry.sampler_rng(seed) if self.symmetry is not None else None
+        self.sym_tables = None
         self.fed = 0
         self._slots = None
         self._slot_i = 0
@@ -1410,6 +1433,9 @@ class GpuBatcher:
 
         # ring capacity from the observed episode lengths and the free HBM (the reference bounds episodes, not steps)
         fe0 = episode_to_flat(backlog[0]) if backlog else None
+        if self.symmetry is not None and fe0 is not None:      # malformed tables raise here, before any upload
+            self.sym_tables = symmetry.build_tables(self.symmetry, [l.shape[2:] for l in tree_leaves(fe0.obs)],
+                                                    fe0.amask.shape[-1])
         cap = int(args.get('replay_capacity_steps', 0))
         lens = [e['steps'] for e in backlog] or [64]
         mean_len, max_len = sum(lens) / len(lens), max(lens)
@@ -1482,9 +1508,18 @@ class GpuBatcher:
         from .replay import WINDOW_DTYPE
         if self._slots is None:
             nb = B * WINDOW_DTYPE.itemsize
-            self._slots = [{'host': torch.empty(nb, dtype=torch.uint8).pin_memory(),
-                            'dev': torch.empty((B, WINDOW_DTYPE.itemsize), dtype=torch.uint8, device=self.device),
-                            'event': None} for _ in range(self.DESC_SLOTS)]
+            if self.symmetry is None:
+                self._slots = [{'host': torch.empty(nb, dtype=torch.uint8).pin_memory(),
+                                'dev': torch.empty((B, WINDOW_DTYPE.itemsize), dtype=torch.uint8, device=self.device),
+                                'event': None} for _ in range(self.DESC_SLOTS)]
+            else:       # descriptors, then B int32 transforms: one buffer, one copy
+                self._slots = []
+                for _ in range(self.DESC_SLOTS):
+                    host = torch.empty(nb + 4 * B, dtype=torch.uint8).pin_memory()
+                    dev = torch.empty(nb + 4 * B, dtype=torch.uint8, device=self.device)
+                    self._slots.append({'host': host, 'host_sym': host[nb:].view(torch.int32),
+                                        'dev': dev[:nb].view(B, WINDOW_DTYPE.itemsize), 'dev_all': dev,
+                                        'sym': dev[nb:].view(torch.int32), 'event': None})
         slot = self._slots[self._slot_i % self.DESC_SLOTS]
         self._slot_i += 1
         if slot['event'] is not None:
@@ -1496,24 +1531,32 @@ class GpuBatcher:
         return self.val_replay is not None and len(self.val_replay) > 0
 
     def fill(self, stepper):
-        """Sample a batch and gather it into stepper.dev (on the step stream)."""
-        self._fill(stepper, self.replay, self.rng)
+        """Sample a batch and gather it into stepper.dev (on the step stream); augmented under train_args['symmetry']."""
+        self._fill(stepper, self.replay, self.rng, self.symmetry is not None)
 
     def fill_validation(self, stepper):
         """Sample a batch of held-out windows (the same sampling law) and gather it into stepper.dev (on the step stream), for
-        LearnerStep.validate_in_place."""
-        self._fill(stepper, self.val_replay, self.val_rng)
+        LearnerStep.validate_in_place.  Never augmented: validation measures the real data."""
+        self._fill(stepper, self.val_replay, self.val_rng, False)
 
-    def _fill(self, stepper, replay, rng):
+    def _tables(self):
+        if self.sym_tables is None:         # no backlog at construction: the first stored episode fixes the shapes
+            self.sym_tables = symmetry.build_tables(self.symmetry, self.replay.leaf_shapes, self.replay.A)
+        return self.sym_tables
+
+    def _fill(self, stepper, replay, rng, augment):
         B = stepper.dims[0]
         slot = self._descriptor_slot(B)
         with self.order_lock:
-            win = replay.sample_windows(B, self.args, rng)
-            slot['host'].numpy()[:] = win.view(np.uint8)
+            win, sym = sample_batch(replay, B, self.args, rng, self.sym_rng if augment else None,
+                                    self._tables().K if augment else 0)
+            slot['host'][:win.nbytes].numpy()[:] = win.view(np.uint8)
+            if sym is not None:
+                slot['host_sym'].numpy()[:] = sym
             with torch.cuda.stream(stepper.stream):
                 if self.last_upload is not None:
                     stepper.stream.wait_event(self.last_upload)
-                slot['dev'].view(-1).copy_(slot['host'], non_blocking=True)
+                slot.get('dev_all', slot['dev']).view(-1).copy_(slot['host'], non_blocking=True)
                 out = dict(stepper.dev)
                 single_leaf = torch.is_tensor(stepper.dev['observation'])
                 if single_leaf:
@@ -1521,7 +1564,10 @@ class GpuBatcher:
                 else:
                     out['observation'] = self._flat_obs(stepper)
                 out['value'] = self._value_sink(stepper)
-                replay.gather(slot['dev'], self.args, out=out)
+                if sym is not None:
+                    replay.gather(slot['dev'], self.args, out=out, sym=slot['sym'], tables=self.sym_tables)
+                else:
+                    replay.gather(slot['dev'], self.args, out=out)
                 if not single_leaf:
                     nested = replay.split_observation(out['observation'])
                     for d, s_ in zip(tree_leaves(stepper.dev['observation']), tree_leaves(nested)):
@@ -1578,11 +1624,16 @@ class Trainer:
     observation, reward or outcome) is rejected on the device and leaves the learner as it was (LearnerStep).  Each epoch
     that rejected a step prints 'skipped = <n> of <steps> steps: non-finite loss or gradient' after the loss (and
     diagnostics) line, even when update() drops the epoch.  `steps` keeps counting batches drawn.  Every rank sees the same
-    all-reduced bucket, so all ranks reject alike."""
+    all-reduced bucket, so all ranks reject alike.
+
+    train_args['symmetry'] = {'group': ..., 'board': [H, W]} or {'tables': 'module:function'} (symmetry.py): every training
+    window is gathered through a board transform drawn uniformly per window (GpuBatcher); the printed lines, the step and
+    the validation batches are unchanged.  Needs gpu_replay."""
 
     def __init__(self, args, model):
         self.weight_ema = weight_ema_decay(args.get('weight_ema'))
         self.validation = validation_rate(args)
+        self.symmetry = symmetry.config(args)
         self.validate_every = max(1, int(round(1.0 / self.validation))) if self.validation is not None else 0
         self.save_optimizer = bool(args.get('save_optimizer', False))
         self.checkpoint_files = None         # numbers the .ema.pth and .optim.pth files of one epoch alike

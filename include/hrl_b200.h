@@ -24,6 +24,8 @@
  *   hrl_weight_ema        <- a per-step moving average of the weights; no reference counterpart (scripts/aux_swa.py
  *                            averages epoch checkpoints)
  *   hrl_gather_pad        <- handyrl/train.py:33-124  (make_batch: window slice + pad + collate)
+ *   hrl_gather_pad_sym    <- the same gather with each window rotated / mirrored by a board-symmetry table; no
+ *                            reference counterpart
  *   hrl_gemm_tf32x3       <- the Linear/Conv contractions of the user's net inside train.py:142-146 (+ autograd, :369)
  *
  * Conventions
@@ -550,6 +552,26 @@ typedef struct HrlGatherArgs {
 } HrlGatherArgs;
 
 int hrl_gather_pad(const HrlGatherArgs *args, void *stream);
+
+/*
+ * Replay gather/pad with board-symmetry augmentation: hrl_gather_pad, with window b written through transform sym[b]
+ * of K permutation tables.  For a live cell of window b, with k = sym[b]:
+ *   observation[e]  = stored observation[obs_src[k][e]]     e < obs_elems (the concatenated flat leaves)
+ *   action_mask[a]  = stored action_mask[act_src[k][a]]     a < A
+ *   action          = act_dst[k][stored action]             (an action outside [0, A) is copied unchanged)
+ * act_src[k] is the inverse permutation of act_dst[k].  Pad cells and every other batch tensor are bit-identical to
+ * hrl_gather_pad's; every batch byte is still written exactly once, and copies are exact.
+ *
+ * The kernel trusts the tables and sym: every row must be a permutation of [0, obs_elems) / [0, A), and
+ * 0 <= sym[b] < K (the caller checks the values on the host before uploading them).  1 <= K <= HRL_SYM_MAX_TRANSFORMS.
+ */
+#define HRL_SYM_MAX_TRANSFORMS 64
+int hrl_gather_pad_sym(const HrlGatherArgs *args,
+                       const int32_t *sym,      /* [B] device: transform of each window, 0 <= sym[b] < K */
+                       const int32_t *obs_src,  /* [K][obs_elems] device (may be NULL when obs_elems == 0) */
+                       const int32_t *act_src,  /* [K][A] device: new action-mask slot <- stored slot */
+                       const int32_t *act_dst,  /* [K][A] device: stored action -> new action */
+                       int32_t K, void *stream);
 
 /* Text of the last error raised on the calling thread ("" if none). */
 const char *hrl_last_error(void);
