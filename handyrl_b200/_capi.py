@@ -52,7 +52,7 @@ class HrlLossArgs(C.Structure):
         ('tap_target_value', C.c_void_p), ('tap_target_return', C.c_void_p), ('tap_advantage', C.c_void_p),
         ('tap_logp', C.c_void_p), ('tap_rho', C.c_void_p), ('tap_entropy', C.c_void_p),
         ('workspace', C.c_void_p), ('workspace_bytes', C.c_size_t),
-        ('tuning', HrlLossTuning), ('io_bf16', C.c_int32),
+        ('tuning', HrlLossTuning), ('io_bf16', C.c_int32), ('window_weight', C.c_void_p),
     ]
 
 
@@ -111,6 +111,17 @@ class HrlGatherArgs(C.Structure):
     ]
 
 
+class HrlReplaySampleArgs(C.Structure):
+    _fields_ = [
+        ('B', C.c_int32), ('ring', C.c_int32), ('head', C.c_int32), ('count', C.c_int32),
+        ('burn_in', C.c_int32), ('forward_steps', C.c_int32), ('Ps', C.c_int32), ('solo', C.c_int32),
+        ('alpha', C.c_float), ('beta', C.c_float), ('seed', C.c_uint64), ('counter', C.c_uint64),
+        ('dir', C.c_void_p), ('prio', C.c_void_p), ('prio_serial', C.c_void_p), ('max_prio', C.c_void_p),
+        ('workspace', C.c_void_p), ('windows', C.c_void_p), ('win_slot', C.c_void_p), ('win_serial', C.c_void_p),
+        ('win_weight', C.c_void_p),
+    ]
+
+
 # every symbol include/hrl_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     'hrl_loss_workspace_bytes': (C.c_size_t, [C.c_int32] * 5),
@@ -140,6 +151,8 @@ SYMBOLS = {
     'hrl_bn_train_bwd': (C.c_int, [C.c_void_p] * 8 + [C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     'hrl_gather_pad': (C.c_int, [C.POINTER(HrlGatherArgs), C.c_void_p]),
     'hrl_gather_pad_sym': (C.c_int, [C.POINTER(HrlGatherArgs)] + [C.c_void_p] * 4 + [C.c_int32, C.c_void_p]),
+    'hrl_replay_sample': (C.c_int, [C.POINTER(HrlReplaySampleArgs), C.c_void_p]),
+    'hrl_replay_priority_update': (C.c_int, [C.c_int32] * 4 + [C.c_void_p] * 2 + [C.c_float] + [C.c_void_p] * 7),
     'hrl_gemm_workspace_floats': (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64, C.c_int32]),
     'hrl_gemm_tf32x3': (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p, C.c_int64,
                                    C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),

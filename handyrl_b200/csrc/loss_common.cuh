@@ -301,8 +301,9 @@ __device__ __forceinline__ void baselines(const LossParams &prm, const SmemLayou
 // phases 2b/2c: from per-row statistics (logp, rho, ent in smem) and the baselines of phase 2a to per-cell gradient
 // factors and the six loss partial sums of this thread.  Caller must __syncthreads() before (statistics and
 // baselines visible) and after.  DIAG: also the HRL_NUM_LOSS_DIAG diagnostics partial sums of this thread in dpart
-// (separate accumulators: the order of every loss sum is that of the plain kernels).
-template <bool DIAG>
+// (separate accumulators: the order of every loss sum is that of the plain kernels).  GRAD: the training pass, which applies
+// HrlLossArgs.window_weight; the forward-only pass (held-out losses) is never weighted and compiles the weight out.
+template <bool DIAG, bool GRAD>
 __device__ __forceinline__ void targets_and_losses(const LossParams &prm, const SmemLayout &L, float *smem, const CtaCtx &c,
                                                    float part[6], float *dpart) {
     const HrlLossArgs &a = prm.a;
@@ -435,24 +436,28 @@ __device__ __forceinline__ void targets_and_losses(const LossParams &prm, const 
         }
         const float tot_adv = rho * (ad[0] + ad[1]);                            // train.py:265
         const float own = (t >= c.t_lo && t < c.t_hi) ? 1.0f : 0.0f;            // cluster: each cell is summed once
+        // importance weight of the window (prioritised replay): it scales each loss term once, after the term is formed,
+        // so a weight of exactly 1 changes no bit; dcnt and the diagnostics stay unweighted.  The gradient factors take it
+        // in row_factors.
+        const float wb = (GRAD && a.window_weight) ? __ldg(a.window_weight + c.b0 + e) : 1.0f;
         smem[L.wterm + i] = tot_adv * tm;
-        Lp += own * (-smem[L.logp + row] * tot_adv * tm);                       // train.py:202
+        Lp += own * (-smem[L.logp + row] * tot_adv * tm * wb);                  // train.py:202
         float dv = 0.f, dr = 0.f;
         if (prm.has_v) {                                                        // train.py:204
             const float d = smem[L.vraw + row] * om - tg[0];
-            Lv += own * (d * d * om);
+            Lv += own * (d * d * om * wb);
             dv = d * om * om;
         }
         if (prm.has_r) {                                                        // train.py:206 smooth_l1, beta 1
             const float d = smem[L.rout + i] - tg[1], adf = fabsf(d);
-            Lr += own * ((adf < 1.0f ? 0.5f * d * d : adf - 0.5f) * om);
+            Lr += own * ((adf < 1.0f ? 0.5f * d * d : adf - 0.5f) * om * wb);
             dr = fminf(fmaxf(d, -1.0f), 1.0f) * om * om;
         }
         smem[L.dv + i] = dv;
         smem[L.dr + i] = dr;
         const float h = smem[L.ent + row] * tm;                                 // train.py:208
-        Lent += own * h;
-        Lreg += own * (h * (1.0f - smem[L.prog + cell] * (1.0f - a.entropy_regularization_decay)));   // train.py:212
+        Lent += own * (h * wb);
+        Lreg += own * (h * (1.0f - smem[L.prog + cell] * (1.0f - a.entropy_regularization_decay)) * wb);   // train.py:212
         dcnt += own * tm;
         if (DIAG && own != 0.0f) {
             // the log ratio exactly as row_epilogue forms it before the exp and the clip (train.py:231-238)
@@ -624,12 +629,13 @@ __device__ __forceinline__ void finalize_diag(const LossParams &prm, const SmemL
     if (c.tid < HRL_NUM_DIAG - HRL_NUM_LOSS_DIAG) prm.diag[HRL_NUM_LOSS_DIAG + c.tid] = 0.0f;   // the optimiser's entries
 }
 
-// per-row gradient factors gathered from the per-cell terms (sum over players when Pa == 1)
+// per-row gradient factors gathered from the per-cell terms (sum over players when Pa == 1), times the importance weight
+// of window b (the global window index: `cell` is CTA-local -- e * Tt + t, or t alone where a window spans a cluster)
 struct RowFactors {
     float w, k, gv, gr;
 };
-__device__ __forceinline__ RowFactors row_factors(const LossParams &prm, const SmemLayout &L, const float *smem, int cell, int q,
-                                                  int P, int Pa) {
+__device__ __forceinline__ RowFactors row_factors(const LossParams &prm, const SmemLayout &L, const float *smem, int b, int cell,
+                                                  int q, int P, int Pa) {
     RowFactors f = {0.f, 0.f, 0.f, 0.f};
     if (Pa == P) {
         f.w = smem[L.wterm + cell * P + q];
@@ -646,6 +652,13 @@ __device__ __forceinline__ RowFactors row_factors(const LossParams &prm, const S
     }
     f.w *= smem[L.emask + cell];
     f.k *= prm.a.entropy_regularization * (1.0f - smem[L.prog + cell] * (1.0f - prm.a.entropy_regularization_decay));
+    if (prm.a.window_weight) {
+        const float wb = __ldg(prm.a.window_weight + b);
+        f.w *= wb;
+        f.k *= wb;
+        f.gv *= wb;
+        f.gr *= wb;
+    }
     return f;
 }
 

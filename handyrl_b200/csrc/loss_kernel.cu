@@ -261,7 +261,7 @@ __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
 
     // ---------------- phase 2: targets, recurrences, per-cell terms; one warp publishes the scalars
     float part[6], dpart[DIAG ? HRL_NUM_LOSS_DIAG : 1];
-    targets_and_losses<DIAG>(prm, L, smem, c, part, dpart);
+    targets_and_losses<DIAG, GRAD>(prm, L, smem, c, part, dpart);
     HRL_STAMP(4);
     if (DIAG) reduce_diag(prm, L, smem, c, dpart);
     reduce_partials(L, smem, c, part);
@@ -275,7 +275,7 @@ __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
         const int e = r / R, rr = r - e * R, t = rr / Pa, q = rr - t * Pa;
         const int cell = e * Tt + t;
         const size_t grow = ((size_t)(c.b0 + e) * T0 + bi + t) * Pa + q;
-        const RowFactors f = row_factors(prm, L, smem, cell, q, P, Pa);
+        const RowFactors f = row_factors(prm, L, smem, c.b0 + e, cell, q, P, Pa);
         const float scale = smem[L.scale + r], m = smem[L.mx + r], lsum = smem[L.lsum + r], h = smem[L.ent + r];
         const int act = (int)s_act[r];
         float *outp = a.dpolicy_raw + grow * A;
@@ -419,7 +419,7 @@ __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
     HRL_STAMP(3);
 
     float part[6], dpart[DIAG ? HRL_NUM_LOSS_DIAG : 1];
-    targets_and_losses<DIAG>(prm, L, smem, c, part, dpart);
+    targets_and_losses<DIAG, GRAD>(prm, L, smem, c, part, dpart);
     HRL_STAMP(4);
     if (DIAG) reduce_diag(prm, L, smem, c, dpart);
     reduce_partials(L, smem, c, part);
@@ -429,7 +429,7 @@ __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
     // ---- 3a: per-row gradient factors (reusing the se / sw slots), value / return gradients
     for (int r = tid; GRAD && r < c.nrows; r += nthr) {
         const int e = (c.nE == 1) ? 0 : r / R, rr = r - e * R, t = fdiv(rr, Pa, c.shPa), q = rr - t * Pa;
-        const RowFactors f = row_factors(prm, L, smem, e * Tt + t, q, P, Pa);
+        const RowFactors f = row_factors(prm, L, smem, c.b0 + e, e * Tt + t, q, P, Pa);
         smem[L.se + r] = f.w;
         smem[L.sw + r] = f.k;
         const size_t grow = ((size_t)(c.b0 + e) * T0 + bi) * Pa + rr;
@@ -515,7 +515,7 @@ __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) 
     HRL_STAMP(3);
 
     float part[6], dpart[DIAG ? HRL_NUM_LOSS_DIAG : 1];
-    targets_and_losses<DIAG>(prm, L, smem, c, part, dpart);
+    targets_and_losses<DIAG, GRAD>(prm, L, smem, c, part, dpart);
     HRL_STAMP(4);
     if (DIAG) reduce_diag(prm, L, smem, c, dpart);
     reduce_partials(L, smem, c, part);
@@ -527,7 +527,7 @@ __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) 
         const int r = base + grp;
         if (r >= c.nrows) continue;
         const int e = (c.nE == 1) ? 0 : r / R, rr = r - e * R, t = fdiv(rr, Pa, c.shPa), q = rr - t * Pa;
-        const RowFactors f = row_factors(prm, L, smem, e * Tt + t, q, P, Pa);
+        const RowFactors f = row_factors(prm, L, smem, c.b0 + e, e * Tt + t, q, P, Pa);
         const size_t grow = ((size_t)(c.b0 + e) * T0 + bi) * Pa + rr;
         if (lane < A) {
             const float scale = smem[L.scale + r];
@@ -714,7 +714,7 @@ __global__ void __launch_bounds__(544, 2) loss_bulk_kernel(const LossParams prm)
     HRL_STAMP(3);
 
     float part[6], dpart[DIAG ? HRL_NUM_LOSS_DIAG : 1];
-    targets_and_losses<DIAG>(prm, L, smem, c, part, dpart);
+    targets_and_losses<DIAG, GRAD>(prm, L, smem, c, part, dpart);
     HRL_STAMP(4);
     if (DIAG) reduce_diag(prm, L, smem, c, dpart);
     reduce_partials(L, smem, c, part);
@@ -726,7 +726,7 @@ __global__ void __launch_bounds__(544, 2) loss_bulk_kernel(const LossParams prm)
         const int gr = r_lo + rr;
         const int t = fdiv(gr, Pa, c.shPa), q = gr - t * Pa;
         const size_t grow = ((size_t)c.b0 * T0 + bi + t) * Pa + q;
-        const RowFactors f = row_factors(prm, L, smem, t, q, P, Pa);
+        const RowFactors f = row_factors(prm, L, smem, c.b0, t, q, P, Pa);
         const float scale = smem[L.scale + gr], m = smem[L.mx + gr], lsum = smem[L.lsum + gr], h = smem[L.ent + gr];
         const int act = (int)s_act[gr];
         float *zrow = smem + L.z + (size_t)rr * A;

@@ -55,7 +55,7 @@ class LossBuffers:
     forward-only pass (loss_fwd), without gradient buffers."""
 
     def __init__(self, B, T, P, Pa, A, has_value, has_return, device, taps=False, policy_dtype=torch.float32, diagnostics=False,
-                 grads=True):
+                 grads=True, advantage=False):
         f = dict(dtype=torch.float32, device=device)
         self.dims = (B, T, P, Pa, A)
         self.policy_dtype = policy_dtype
@@ -70,6 +70,8 @@ class LossBuffers:
                 'advantage': torch.zeros((B, T, P, 1), **f), 'logp': torch.zeros((B, T, Pa, 1), **f),
                 'rho': torch.zeros((B, T, Pa, 1), **f), 'entropy': torch.zeros((B, T, Pa), **f),
             }
+        # advantage=True: the advantage tap alone (B, T, P, 1), which the priority update of prioritised replay reduces
+        self.advantage = torch.zeros((B, T, P, 1), **f) if advantage and not taps else None
         self.workspace = torch.zeros(lib().hrl_loss_workspace_bytes(B, T, P, Pa, A), dtype=torch.uint8, device=device)
         self.diagnostics = self.diag_workspace = None
         if diagnostics:
@@ -84,7 +86,7 @@ class LossBuffers:
             self.diag_workspace = torch.zeros(lib().hrl_loss_diag_workspace_bytes(*self.dims), dtype=torch.uint8, device=device)
 
 
-def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None, diagnostics=False):
+def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None, diagnostics=False, window_weight=None):
     """Fused mask epilogue + compute_loss + closed-form backward (reference train.py:176-267).
 
     outputs: raw net outputs {'policy': (B,T,Pa,A), 'value': (B,T,Pa,1)?, 'return': (B,T,Pa,1)?}
@@ -96,9 +98,12 @@ def loss_fwd_bwd(outputs, batch, args, buffers=None, taps=False, tuning=None, di
              cluster, consumers, threads, unstaged, trace (an int64 CUDA tensor of >= 32 elements)
     diagnostics: also accumulate the learner diagnostics sums (hrl_loss_fwd_bwd_diag) into .diagnostics, in DIAG_KEYS order;
              losses and gradients are bit-identical to the plain pass
+    window_weight: None, or a (B,) float32 CUDA tensor of importance weights (prioritised replay): every per-cell loss term of
+             window b and its gradients are scaled by window_weight[b]; dcnt and the diagnostics are not.  Weights of exactly 1
+             give the bits of window_weight=None.
     returns  LossBuffers with .losses = [p, v, r, ent, total, dcnt] and the gradients.
     """
-    return _loss_call(outputs, batch, args, buffers, taps, tuning, 'diag' if diagnostics else 'fwd_bwd')
+    return _loss_call(outputs, batch, args, buffers, taps, tuning, 'diag' if diagnostics else 'fwd_bwd', window_weight)
 
 
 def loss_fwd(outputs, batch, args, buffers=None, taps=False, tuning=None):
@@ -109,7 +114,7 @@ def loss_fwd(outputs, batch, args, buffers=None, taps=False, tuning=None):
     return _loss_call(outputs, batch, args, buffers, taps, tuning, 'fwd').losses
 
 
-def _loss_call(outputs, batch, args, buffers, taps, tuning, form):
+def _loss_call(outputs, batch, args, buffers, taps, tuning, form, window_weight=None):
     diagnostics = form == 'diag'
     policy = outputs['policy']
     io_bf16 = policy.dtype == torch.bfloat16       # wide rows only: 8 instead of 12 bytes per action through HBM (include/hrl_b200.h)
@@ -130,12 +135,15 @@ def _loss_call(outputs, batch, args, buffers, taps, tuning, form):
         raise ValueError('loss_fwd_bwd: these LossBuffers were built without gradient buffers (grads=False)')
     if diagnostics:
         buffers.enable_diagnostics()
+    if window_weight is not None and not (window_weight.is_cuda and window_weight.dtype == torch.float32 and
+                                          window_weight.is_contiguous() and window_weight.numel() == B):
+        raise _capi.HrlError('handyrl_b200: window_weight must be a contiguous float32 CUDA tensor of B=%d weights' % B)
 
     # static buffers (CUDA-graph replays): the argument block of the previous call is still valid
     key = (policy.data_ptr(), 0 if value is None else value.data_ptr(), 0 if ret_head is None else ret_head.data_ptr(),
            args['value_target'], args['policy_target'], bool(args['turn_based_training']), args.get('burn_in_steps', 0),
            args['lambda'], args['gamma'], args['entropy_regularization'], args['entropy_regularization_decay'],
-           buffers.taps is not None, None if tuning is None else tuple(sorted((k, v if not torch.is_tensor(v) else v.data_ptr())
+           buffers.taps is not None, 0 if window_weight is None else window_weight.data_ptr(), None if tuning is None else tuple(sorted((k, v if not torch.is_tensor(v) else v.data_ptr())
                                                                                  for k, v in tuning.items()))) + \
         tuple(batch[k].data_ptr() for k in _BATCH_KEYS)
     slot = '_cached_' + form      # one argument block per form
@@ -173,6 +181,9 @@ def _loss_call(outputs, batch, args, buffers, taps, tuning, form):
         t = buffers.taps
         a.tap_target_value, a.tap_target_return, a.tap_advantage = _ptr(t['target_value']), _ptr(t['target_return']), _ptr(t['advantage'])
         a.tap_logp, a.tap_rho, a.tap_entropy = _ptr(t['logp']), _ptr(t['rho']), _ptr(t['entropy'])
+    elif getattr(buffers, 'advantage', None) is not None:
+        a.tap_advantage = _ptr(buffers.advantage)
+    a.window_weight = _ptr(window_weight)
     a.io_bf16 = int(io_bf16)
     ws = buffers.diag_workspace if diagnostics else buffers.workspace
     a.workspace = _ptr(ws)
@@ -433,6 +444,48 @@ def step_commit(skip, tail, accum, skip_count, state=None, saved=None):
         nbytes = state.numel()
     check(lib().hrl_step_commit(_ptr(skip), _ptr(tail), tail.numel(), _ptr(accum), _ptr(skip_count),
                                 _ptr(state) if nbytes else None, _ptr(saved) if nbytes else None, nbytes, _stream_ptr()))
+    _count()
+
+
+def replay_sample(state, replay, head, count, args, windows, seed, counter, solo):
+    """Launch hrl_replay_sample (one kernel on the current stream): draw state.B windows of the replay `replay` (a
+    DeviceReplay keeping its directory mirror) by prioritised replay, into `windows` (a (B, 32) uint8 CUDA tensor, the
+    gather's descriptor buffer) and state.win_slot / win_serial / win_weight.  head, count: the directory snapshot the host
+    took under the replay lock; seed, counter: the Philox key and this batch's counter."""
+    if replay.dir_dev is None:
+        raise _capi.HrlError('handyrl_b200: the replay keeps no device directory (DeviceReplay(..., mirror=True))')
+    if replay.dir_dev.shape[0] != state.ring:
+        raise _capi.HrlError('handyrl_b200: the replay directory has %d slots, the priorities %d' % (replay.dir_dev.shape[0], state.ring))
+    if not (windows.is_cuda and windows.dtype == torch.uint8 and windows.is_contiguous() and windows.numel() == 32 * state.B):
+        raise _capi.HrlError('handyrl_b200: windows must be a contiguous uint8 CUDA buffer of %d descriptors' % state.B)
+    g = _capi.HrlReplaySampleArgs()
+    g.B, g.ring, g.head, g.count = state.B, state.ring, int(head), int(count)
+    g.burn_in, g.forward_steps = int(args.get('burn_in_steps', 0)), int(args['forward_steps'])
+    g.Ps, g.solo = int(replay.Ps), int(bool(solo))
+    g.alpha, g.beta = state.alpha, state.beta
+    g.seed, g.counter = int(seed) % (1 << 64), int(counter) % (1 << 64)
+    g.dir, g.prio, g.prio_serial, g.max_prio = _ptr(replay.dir_dev), _ptr(state.prio), _ptr(state.prio_serial), _ptr(state.max_prio)
+    g.workspace, g.windows = _ptr(state.cdf), _ptr(windows)
+    g.win_slot, g.win_serial, g.win_weight = _ptr(state.win_slot), _ptr(state.win_serial), _ptr(state.win_weight)
+    check(lib().hrl_replay_sample(C.byref(g), _stream_ptr()))
+    _count()
+
+
+def priority_update(state, advantage, turn_mask, burn_in, skip=None):
+    """Launch hrl_replay_priority_update (one kernel on the current stream): the window priorities of this step's
+    advantage tap and turn mask ((B, T, P[, 1]) float32 CUDA tensors) go to state.prio where the windows' serials still
+    match, and raise state.max_prio.  skip: the guarded optimiser's flag (nothing is written when it is set), or None."""
+    for t, name in ((advantage, 'advantage'), (turn_mask, 'turn_mask')):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous() and t.shape[0] == state.B):
+            raise _capi.HrlError('handyrl_b200: %s must be a contiguous float32 CUDA tensor of %d windows' % (name, state.B))
+    if advantage.shape[:3] != turn_mask.shape[:3]:
+        raise _capi.HrlError('handyrl_b200: advantage %s and turn_mask %s differ in shape' % (tuple(advantage.shape), tuple(turn_mask.shape)))
+    if skip is not None:
+        _check_skip(skip)
+    B, T, P = turn_mask.shape[:3]
+    check(lib().hrl_replay_priority_update(B, T, P, int(burn_in), _ptr(advantage), _ptr(turn_mask), float(state.epsilon),
+                                           _ptr(state.win_slot), _ptr(state.win_serial), _ptr(state.prio), _ptr(state.prio_serial),
+                                           _ptr(state.max_prio), _ptr(skip), _stream_ptr()))
     _count()
 
 

@@ -63,7 +63,7 @@ class DeviceReplay:
     are drawn with array operations instead of a Python loop per window.
     """
 
-    def __init__(self, capacity_steps, max_episodes, device='cuda'):
+    def __init__(self, capacity_steps, max_episodes, device='cuda', mirror=False):
         self.device = torch.device(device)
         self.capacity = int(capacity_steps)
         self.max_episodes = int(max_episodes)
@@ -74,6 +74,12 @@ class DeviceReplay:
         self.ready = False
         self.next_outcome_row = 0
         self.lock = threading.Lock()       # guards the directory (feeder thread appends, learner thread samples)
+        # every stored episode gets the next serial, so a directory slot that is reused is told apart from its old episode
+        self._serial = np.full(self.max_episodes + 1, -1, np.int64)
+        self.next_serial = 0
+        # mirror=True (prioritised replay): a device copy of the directory, [slot] = (first_step, steps, outcome_row, serial),
+        # which commit() updates on its stream for the slots it appends; the device sampler reads it
+        self.dir_dev = (torch.full((self.max_episodes + 1, 4), -1, dtype=torch.int64, device=self.device) if mirror else None)
 
     # ------------------------------------------------------------------ directory
     def __len__(self):
@@ -92,8 +98,16 @@ class DeviceReplay:
         self._count -= 1
 
     def _append(self, first_step, steps, row):
-        self._dir[(self._head + self._count) % self._dir.shape[0]] = (first_step, steps, row)
+        slot = (self._head + self._count) % self._dir.shape[0]
+        self._dir[slot] = (first_step, steps, row)
+        self._serial[slot] = self.next_serial
+        self.next_serial += 1
         self._count += 1
+        return slot
+
+    def snapshot(self, max_count):
+        """(head slot, count) of the directory now, count capped at max_count (the sampler's view; take it under self.lock)."""
+        return self._head, min(self._count, int(max_count))
 
     def _allocate(self, fe):
         S, dev = self.capacity, self.device
@@ -168,7 +182,7 @@ class DeviceReplay:
         oldest episodes beyond max_episodes) and enqueue the copies on the current stream.  Rows are placed back to
         back, so every run of episodes that does not cross the end of the ring is ONE copy per store column."""
         handles, segments = [], []        # segments: [dst_lo, src_lo, n]
-        rows = []
+        rows, appended = [], []
         with self.lock:
             src = 0
             for n in staged['steps']:
@@ -192,7 +206,7 @@ class DeviceReplay:
                 else:
                     segments.append([lo, src, n])
                 rows.append(row)
-                self._append(lo, n, row)
+                appended.append(self._append(lo, n, row))
                 handles.append(EpisodeHandle(lo, n, row))
                 self.write = hi
                 src += n
@@ -205,6 +219,12 @@ class DeviceReplay:
             idx = torch.tensor(rows, dtype=torch.long)
             self.st_outcome.index_copy_(0, idx.to(self.device, non_blocking=True),
                                         staged['outcome'].to(self.device, non_blocking=True))
+            if self.dir_dev is not None and appended:
+                # a slot reused inside one upload is copied once, with its final episode
+                slots = np.unique(np.asarray(appended, np.int64))
+                ent = np.concatenate([self._dir[slots], self._serial[slots, None]], axis=1)
+                self.dir_dev.index_copy_(0, torch.from_numpy(slots).to(self.device, non_blocking=True),
+                                         torch.from_numpy(np.ascontiguousarray(ent)).to(self.device, non_blocking=True))
         return handles
 
     # ------------------------------------------------------------------ batches

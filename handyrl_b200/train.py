@@ -27,7 +27,7 @@ from collections import deque
 import numpy as np
 import torch
 
-from . import ops, fastnet, symmetry
+from . import ops, fastnet, priority, symmetry
 from .batch import tree_map, tree_leaves, make_batch, gather_windows, sample_window
 from ._capi import DIAG_KEYS, LOSS_KEYS, NUM_DIAG, NUM_LOSS, NUM_LOSS_DIAG
 
@@ -591,6 +591,13 @@ class LearnerStep:
     graph sharing the step graph's memory pool; `launches_per_validation` counts its launches.  end_epoch hands the sums
     over with the loss sums (PendingModel.validation); pop_validation() reads them now.
 
+    train_args['prioritized_replay'] (priority.py): the step owns the priority state (`prio_state`, a priority.PriorityState:
+    the per-slot priorities and the per-window slot, serial and weight buffers the sampler fills), because the captured graph
+    bakes in its pointers.  The loss pass scales window b's terms and gradients by prio_state.win_weight[b] and writes the
+    advantage tap, and the step ends with one more launch (ops.priority_update, after the optimiser: it reads the guard's flag)
+    that stores the windows' priorities.  With the weights at 1 and the serials at -1 (as built, and so during the warm-up and
+    capture steps) the weights train exactly as without the key and no priority moves.
+
     skip_nonfinite (default: train_args['skip_nonfinite'], off): a step whose pre-clip gradient norm or one of whose six loss
     sums is not finite is rejected on the device (ops.FlatAdam.skip, hrl_clip_adam_step_guarded), and the learner is left
     bit for bit as if its batch had never been drawn: weights, Adam's moments and step count, the BatchNorm buffers (saved by
@@ -608,6 +615,7 @@ class LearnerStep:
         self.weight_ema = weight_ema_decay(args.get('weight_ema') if weight_ema is None else weight_ema)
         rate = validation_rate(args)
         symmetry.config(args)           # malformed train_args['symmetry'] fails here; the gather applies it, not the step
+        self.priority = priority.config(args)
         self.validation = bool(rate is not None if validation is None else validation)
         self.save_optimizer = bool(args.get('save_optimizer', False) if save_optimizer is None else save_optimizer)
         self.skip_nonfinite = nonfinite_guard(args) if skip_nonfinite is None else bool(skip_nonfinite)
@@ -701,6 +709,9 @@ class LearnerStep:
         B, T, Pa, A = example_batch['action_mask'].shape
         P = example_batch['turn_mask'].shape[2]
         self.dims = (B, T, P, Pa, A)
+        self.prio_state = None
+        if self.priority is not None:
+            self.prio_state = priority.PriorityState(self.priority, priority.ring_slots(args), B, self.device)
         self.hidden0 = None
         if hasattr(self.model, 'init_hidden'):
             self.hidden0 = tree_map(lambda h: h.to(self.device), self.model.init_hidden([B, P]))
@@ -762,12 +773,14 @@ class LearnerStep:
             self._outs = forward_raw(self.model, self.hidden0, self.dev, self.args, self.memory_format)
         if self.loss_buf is None:
             B, T, P, Pa, A = self.dims
-            self.loss_buf = ops.LossBuffers(B, T, P, Pa, A, 'value' in self._outs, 'return' in self._outs, self.device)
+            self.loss_buf = ops.LossBuffers(B, T, P, Pa, A, 'value' in self._outs, 'return' in self._outs, self.device,
+                                            advantage=self.prio_state is not None)
 
     def _part_loss(self):
         outs = self._outs
         ops.loss_fwd_bwd({k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, self.dev, self.args,
-                         buffers=self.loss_buf, diagnostics=self.diagnostics)
+                         buffers=self.loss_buf, diagnostics=self.diagnostics,
+                         window_weight=self.prio_state.win_weight if self.prio_state is not None else None)
 
     def _part_backward(self):
         outs, buf = self._outs, self.loss_buf
@@ -809,6 +822,9 @@ class LearnerStep:
         if self.avg is not None:        # after the optimiser: step_count already counts this step
             ops.weight_ema_update(self.avg, self.state.bytes[:self.state.i_off].view(torch.float32), self.opt.step_count,
                                   self.weight_ema, self.avg_seeded, skip=self.opt.skip)
+        if self.prio_state is not None:     # after the optimiser: a rejected step stores no priority
+            ops.priority_update(self.prio_state, self.loss_buf.advantage, self.dev['turn_mask'], self.args.get('burn_in_steps', 0),
+                                skip=self.opt.skip if self.skip_nonfinite else None)
 
     def _guarded_buffers(self):
         """The buffers a step's forward moves (BatchNorm running statistics, num_batches_tracked): StateStore bytes
@@ -1382,7 +1398,14 @@ class GpuBatcher:
     With train_args['symmetry'] set (symmetry.py), fill() gathers every window through a transform drawn uniformly from the
     group by its own generator (symmetry.sampler_rng(seed)): the window descriptors are those drawn without the key.  The
     tables are built once from the first episode's leaf shapes and uploaded once; the transforms ride in the pinned
-    descriptor slot behind the descriptors, in the same copy.  fill_validation() never augments."""
+    descriptor slot behind the descriptors, in the same copy.  fill_validation() never augments.
+
+    With train_args['prioritized_replay'] set (priority.py), fill() draws the windows on the device instead: the replay keeps a
+    device mirror of its directory, and hrl_replay_sample reads it with the stepper's priority state (LearnerStep.prio_state)
+    and writes the descriptors and the importance weights straight into the buffers the gather and the step read.  The host
+    only snapshots (head, count) under the locks, as it does to sample; the Philox key comes from the seed
+    (priority.sampler_key) and the counter is the number of batches drawn.  Symmetry transforms are still drawn on the host.
+    fill_validation() keeps the host sampler."""
 
     DESC_SLOTS = 4        # pinned descriptor buffers in rotation: bounds how far the host runs ahead of the GPU
 
@@ -1405,6 +1428,9 @@ class GpuBatcher:
         self.symmetry = symmetry.config(args)
         self.sym_rng = symmetry.sampler_rng(seed) if self.symmetry is not None else None
         self.sym_tables = None
+        self.priority = priority.config(args)
+        self.prio_key = priority.sampler_key(seed)
+        self.prio_batches = 0               # the Philox counter of the next prioritised batch
         self.fed = 0
         self._slots = None
         self._slot_i = 0
@@ -1450,7 +1476,7 @@ class GpuBatcher:
             if est < args['maximum_episodes']:
                 print('handyrl_b200: the GPU replay holds about %d episodes (%d steps), fewer than maximum_episodes=%d'
                       % (est, cap, args['maximum_episodes']))
-        self.replay = DeviceReplay(cap, args['maximum_episodes'], device=device)
+        self.replay = DeviceReplay(cap, args['maximum_episodes'], device=device, mirror=self.priority is not None)
         self.val_replay = None
         if self.validation is not None and keep_validation:
             r = self.validation
@@ -1531,8 +1557,9 @@ class GpuBatcher:
         return self.val_replay is not None and len(self.val_replay) > 0
 
     def fill(self, stepper):
-        """Sample a batch and gather it into stepper.dev (on the step stream); augmented under train_args['symmetry']."""
-        self._fill(stepper, self.replay, self.rng, self.symmetry is not None)
+        """Sample a batch and gather it into stepper.dev (on the step stream); augmented under train_args['symmetry'], drawn by
+        the device sampler under train_args['prioritized_replay']."""
+        self._fill(stepper, self.replay, self.rng, self.symmetry is not None, self.priority is not None)
 
     def fill_validation(self, stepper):
         """Sample a batch of held-out windows (the same sampling law) and gather it into stepper.dev (on the step stream), for
@@ -1544,19 +1571,39 @@ class GpuBatcher:
             self.sym_tables = symmetry.build_tables(self.symmetry, self.replay.leaf_shapes, self.replay.A)
         return self.sym_tables
 
-    def _fill(self, stepper, replay, rng, augment):
+    def _fill(self, stepper, replay, rng, augment, prioritized=False):
         B = stepper.dims[0]
+        if prioritized and stepper.prio_state is None:
+            raise ValueError("GpuBatcher: train_args['prioritized_replay'] needs a LearnerStep built with the key")
         slot = self._descriptor_slot(B)
         with self.order_lock:
-            win, sym = sample_batch(replay, B, self.args, rng, self.sym_rng if augment else None,
-                                    self._tables().K if augment else 0)
-            slot['host'][:win.nbytes].numpy()[:] = win.view(np.uint8)
+            if prioritized:         # the device draws the windows: the host takes the directory snapshot only
+                with replay.lock:
+                    head, count = replay.snapshot(self.args['maximum_episodes'])
+                if count <= 0:
+                    raise IndexError('the replay is empty')
+                sym = None
+                if augment:
+                    K = self._tables().K
+                    sym = symmetry.draw(self.sym_rng, B, K)
+                    self._tables().check_sym(sym)
+            else:
+                win, sym = sample_batch(replay, B, self.args, rng, self.sym_rng if augment else None,
+                                        self._tables().K if augment else 0)
+                slot['host'][:win.nbytes].numpy()[:] = win.view(np.uint8)
             if sym is not None:
                 slot['host_sym'].numpy()[:] = sym
             with torch.cuda.stream(stepper.stream):
                 if self.last_upload is not None:
                     stepper.stream.wait_event(self.last_upload)
-                slot.get('dev_all', slot['dev']).view(-1).copy_(slot['host'], non_blocking=True)
+                if not prioritized:
+                    slot.get('dev_all', slot['dev']).view(-1).copy_(slot['host'], non_blocking=True)
+                else:
+                    if sym is not None:
+                        slot['sym'].copy_(slot['host_sym'], non_blocking=True)
+                    ops.replay_sample(stepper.prio_state, replay, head, count, self.args, slot['dev'], self.prio_key,
+                                      self.prio_batches, solo=not self.args['turn_based_training'])
+                    self.prio_batches += 1
                 out = dict(stepper.dev)
                 single_leaf = torch.is_tensor(stepper.dev['observation'])
                 if single_leaf:
@@ -1628,12 +1675,20 @@ class Trainer:
 
     train_args['symmetry'] = {'group': ..., 'board': [H, W]} or {'tables': 'module:function'} (symmetry.py): every training
     window is gathered through a board transform drawn uniformly per window (GpuBatcher); the printed lines, the step and
-    the validation batches are unchanged.  Needs gpu_replay."""
+    the validation batches are unchanged.  Needs gpu_replay.
+
+    train_args['prioritized_replay'] = True or {'alpha': a, 'beta': b, 'epsilon': e} (priority.py): training windows are drawn
+    on the device with probability proportional to the recency law times a per-episode priority from the fused loss's
+    advantages, and weighted to correct the bias (LearnerStep, GpuBatcher).  The printed lines keep their format; the loss
+    line reports the weighted objective.  Validation batches use the host sampler and no weights.  Each rank keeps the
+    priorities of its own shard.  Priorities are not saved: after a restart every episode starts at max_prio.  Needs
+    gpu_replay."""
 
     def __init__(self, args, model):
         self.weight_ema = weight_ema_decay(args.get('weight_ema'))
         self.validation = validation_rate(args)
         self.symmetry = symmetry.config(args)
+        self.priority = priority.config(args)
         self.validate_every = max(1, int(round(1.0 / self.validation))) if self.validation is not None else 0
         self.save_optimizer = bool(args.get('save_optimizer', False))
         self.checkpoint_files = None         # numbers the .ema.pth and .optim.pth files of one epoch alike

@@ -26,6 +26,9 @@
  *   hrl_gather_pad        <- handyrl/train.py:33-124  (make_batch: window slice + pad + collate)
  *   hrl_gather_pad_sym    <- the same gather with each window rotated / mirrored by a board-symmetry table; no
  *                            reference counterpart
+ *   hrl_replay_sample /
+ *   hrl_replay_priority_update <- prioritised replay: Batcher.select_episode's recency law (train.py:291-315) times a
+ *                            per-episode priority, with importance weights; no reference counterpart
  *   hrl_gemm_tf32x3       <- the Linear/Conv contractions of the user's net inside train.py:142-146 (+ autograd, :369)
  *
  * Conventions
@@ -139,6 +142,10 @@ typedef struct HrlLossArgs {
                                     move through HBM.  Wide rows only (256 < A <= 512, A % 8 == 0); everything in between --
                                     masks, softmax statistics, targets, the gradient before its final rounding -- stays fp32, so
                                     the losses equal those of the fp32 call on the widened logits bit for bit              */
+    const float *window_weight;  /* (B) importance weight of each window (prioritised replay), or NULL = 1.  It multiplies every
+                                    per-cell loss term of window b (policy, value, return, entropy, entropy regulariser) and
+                                    their gradients; dcnt and the diagnostics sums stay unweighted.  Weights of exactly 1
+                                    give losses and gradients bit-identical to NULL                                       */
 } HrlLossArgs;
 
 /* Bytes of workspace hrl_loss_fwd_bwd needs for these dimensions (host call, no GPU work). */
@@ -149,7 +156,8 @@ int hrl_loss_fwd_bwd(const HrlLossArgs *args, void *stream);
 
 /* The forward half of hrl_loss_fwd_bwd (held-out validation losses): the same struct, workspace, shapes (bf16 logits included)
  * and choice of kernel, with the gradient phase compiled out.  Writes `losses` (bit-identical to hrl_loss_fwd_bwd on the
- * same inputs) and the taps that are given; dpolicy_raw, dvalue_raw and dreturn_raw may be NULL and are never written. */
+ * same inputs) and the taps that are given; dpolicy_raw, dvalue_raw and dreturn_raw may be NULL and are never written.
+ * window_weight is ignored: held-out losses are never weighted. */
 int hrl_loss_fwd(const HrlLossArgs *args, void *stream);
 
 /*
@@ -572,6 +580,55 @@ int hrl_gather_pad_sym(const HrlGatherArgs *args,
                        const int32_t *act_src,  /* [K][A] device: new action-mask slot <- stored slot */
                        const int32_t *act_dst,  /* [K][A] device: stored action -> new action */
                        int32_t K, void *stream);
+
+/*
+ * Prioritised replay (opt-in, no reference counterpart).  Every slot of the replay's episode directory (a ring of `ring`
+ * slots; the live episodes are slots (head + i) % ring, i = 0 the oldest of `count`) holds a priority prio[s] and the serial
+ * of the episode that priority belongs to, prio_serial[s].
+ *
+ * hrl_replay_sample draws B windows on the device, in one launch:
+ *   - a live slot whose directory serial differs from prio_serial is a new episode: prio = *max_prio, prio_serial = its serial;
+ *   - episode i is drawn with probability (i+1) * prio^alpha / sum (fp64 prefix sum in a fixed order, binary search);
+ *   - inside it the window is placed as the host sampler places it: train_start uniform on [0, 1 + max(0, steps - forward)),
+ *     start = max(0, train_start - burn_in), end = min(train_start + forward, steps), a uniform player when solo != 0;
+ *   - windows[b], win_slot[b], win_serial[b] and win_weight[b] = B * p_b^(-alpha*beta) / sum_b' p_b'^(-alpha*beta).
+ * The random numbers are Philox4x32-10 (curand) with key `seed`, one 128-bit block per window at counter
+ * (b, counter_lo, counter_hi, 0): the same seed, counter and priorities give the same windows.
+ */
+typedef struct HrlReplaySampleArgs {
+    int32_t B;                    /* windows to draw                                                            */
+    int32_t ring;                 /* directory slots                                                            */
+    int32_t head, count;          /* oldest live slot and live episodes (count >= 1, count < ring)              */
+    int32_t burn_in, forward_steps;
+    int32_t Ps;                   /* players per step in the store                                              */
+    int32_t solo;                 /* 1: draw HrlWindow.player uniformly in [0, Ps); 0: player = 0               */
+    float alpha, beta;            /* alpha >= 0, 0 <= beta <= 1                                                  */
+    uint64_t seed;                /* Philox key                                                                 */
+    uint64_t counter;             /* Philox counter of this batch (one per batch)                               */
+    const int64_t *dir;           /* [ring][4] device mirror of the directory: first_step, steps, outcome_row, serial */
+    float *prio;                  /* [ring]                                                                     */
+    int64_t *prio_serial;         /* [ring]                                                                     */
+    const float *max_prio;        /* [1]                                                                        */
+    double *workspace;            /* [ring] prefix sums                                                         */
+    HrlWindow *windows;           /* [B] out: the gather's descriptors                                          */
+    int32_t *win_slot;            /* [B] out: directory slot of each window                                     */
+    int64_t *win_serial;          /* [B] out: episode serial of each window                                     */
+    float *win_weight;            /* [B] out: importance weights, mean 1                                        */
+} HrlReplaySampleArgs;
+
+int hrl_replay_sample(const HrlReplaySampleArgs *args, void *stream);
+
+/*
+ * The priority update that ends a prioritised step, in one launch.  Window b's priority over its trained cells
+ * (t >= burn_in), tm = turn_mask (B,T,P), adv = the loss pass's tap_advantage (B,T,P):
+ *     q_b = sum(tm * |adv|) / sum(tm) + epsilon      (fp32, fixed order; no priority when sum(tm) == 0)
+ * prio[win_slot[b]] becomes the largest q_b of the windows on that slot -- only where prio_serial[slot] == win_serial[b]
+ * (win_serial < 0: the window is ignored) -- and *max_prio rises to the largest q_b written.  skip (the guarded optimiser's
+ * flag, or NULL): when *skip != 0 nothing is written.
+ */
+int hrl_replay_priority_update(int32_t B, int32_t T, int32_t P, int32_t burn_in, const float *tap_advantage,
+                               const float *turn_mask, float epsilon, const int32_t *win_slot, const int64_t *win_serial,
+                               float *prio, const int64_t *prio_serial, float *max_prio, const int32_t *skip, void *stream);
 
 /* Text of the last error raised on the calling thread ("" if none). */
 const char *hrl_last_error(void);
