@@ -90,14 +90,20 @@ __device__ __forceinline__ void stage_small(const LossParams &prm, const SmemLay
     for (int i = c.tid; i < c.nE * c.P; i += c.nthr) cp_async4(smem + L.outcome + i, a.outcome + (size_t)c.b0 * c.P + i);
 }
 
-// burn-in steps take no part in the loss: zero gradients (train.py:220-222)
+// burn-in steps take no part in the loss: zero gradients (train.py:220-222).  With io_bf16 the policy gradient holds bf16
+// elements: zeroed as 16-bit words (zero in bf16 too), or the stores would land at twice the offset.
 __device__ __forceinline__ void zero_burn_in(const LossParams &prm, const CtaCtx &c) {
     const HrlLossArgs &a = prm.a;
     if (c.bi <= 0) return;
     const int nz = c.bi * c.Pa * c.A, nzr = c.bi * c.Pa;
     for (int e = 0; e < c.nE; e++) {
         const size_t g0 = (size_t)(c.b0 + e) * c.T0 * c.Pa;
-        for (int i = c.tid; i < nz; i += c.nthr) a.dpolicy_raw[g0 * c.A + i] = 0.0f;
+        if (a.io_bf16) {
+            uint16_t *d16 = reinterpret_cast<uint16_t *>(a.dpolicy_raw) + g0 * c.A;
+            for (int i = c.tid; i < nz; i += c.nthr) d16[i] = 0;
+        } else {
+            for (int i = c.tid; i < nz; i += c.nthr) a.dpolicy_raw[g0 * c.A + i] = 0.0f;
+        }
         for (int i = c.tid; i < nzr; i += c.nthr) {
             if (prm.has_v) a.dvalue_raw[g0 + i] = 0.0f;
             if (prm.has_r) a.dreturn_raw[g0 + i] = 0.0f;
