@@ -324,6 +324,107 @@ def validation_rate(args):
     return float(value)
 
 
+def replay_ratio(args):
+    """train_args['replay_ratio'] -> the cap r on samples trained per step stored in the training replay, or None when the
+    limit is off (key absent, 0 or None).  A negative, NaN or infinite value, True and anything that is not a number raise
+    ValueError."""
+    value = args.get('replay_ratio')
+    if value is None or (isinstance(value, numbers.Real) and value == 0):
+        return None
+    if isinstance(value, bool) or not isinstance(value, numbers.Real) or not 0.0 < float(value) < float('inf'):
+        raise ValueError("train_args['replay_ratio'] must be a positive number of samples trained per stored step (e.g. 32), "
+                         "or 0 / None for no limit; got %r" % (value,))
+    return float(value)
+
+
+class ReplayRatioLimiter:
+    """The Trainer's samples-per-insert limit (train_args['replay_ratio'] = r), counted on the host from numbers it already
+    has: `trained`, the samples of the batches drawn (drew(): batch_size * forward_steps each, the global batch without
+    burn-in), and `stored`, the steps of the episodes that entered the training replay (store(), called by the feeder after
+    each commit).  Evictions never lower `stored`: it counts inserts.  acquire(n) holds the trainer thread until n more
+    batches fit,
+
+        trained + n * samples_per_batch <= r * stored,
+
+    on a condition that store() signals (and a short poll), so it never touches the device and never blocks the feeder.
+    Both counts start at zero with the object, and the per-epoch figures of the printed line come from end_epoch()."""
+
+    def __init__(self, ratio, samples_per_batch, poll=0.05, clock=time.monotonic):
+        self.ratio, self.samples_per_batch = float(ratio), int(samples_per_batch)
+        self.poll, self.clock = poll, clock
+        self.cond = threading.Condition()
+        self.trained = self.stored = 0
+        self.waited = 0.0                 # seconds the trainer thread spent in acquire() without credit
+        self.waiting = False
+        self._mark = None                 # (trained, stored, waited, clock) at the start of the running epoch
+
+    def allows(self, n=1):
+        return self.trained + n * self.samples_per_batch <= self.ratio * self.stored
+
+    def store(self, steps):
+        with self.cond:
+            self.stored += int(steps)
+            self.cond.notify_all()
+
+    def drew(self, batches=1):
+        with self.cond:
+            self.trained += batches * self.samples_per_batch
+
+    def wake(self):
+        """Make a waiting acquire() look at its interrupt() now (the Trainer calls it from update() and stop())."""
+        with self.cond:
+            self.cond.notify_all()
+
+    def acquire(self, n, interrupt):
+        """Wait until n more batches fit (returns True) or, without that credit, until interrupt() is true (returns False)."""
+        with self.cond:
+            if self.allows(n):
+                return True
+            t0 = self.clock()
+            self.waiting = True
+            try:
+                while not self.allows(n):
+                    if interrupt():
+                        return False
+                    self.cond.wait(self.poll)
+                return True
+            finally:
+                self.waiting = False
+                self.waited += self.clock() - t0
+
+    def start_epoch(self):
+        """Start the first epoch's clock (later epochs start where the previous one ended); its counts start at zero, so the
+        first epoch's stored steps include the backlog."""
+        with self.cond:
+            if self._mark is None:
+                self._mark = (0, 0, 0.0, self.clock())
+
+    def end_epoch(self):
+        """The running epoch's figures, and start the next: {'trained': samples, 'stored': steps, 'ratio': trained / stored
+        (None when nothing was stored), 'limit': r, 'waited': the fraction of the epoch's wall time spent waiting for credit,
+        'wall': the epoch's wall time in seconds}."""
+        with self.cond:
+            now = self.clock()
+            trained0, stored0, waited0, t0 = self._mark if self._mark is not None else (0, 0, 0.0, now)
+            self._mark = (self.trained, self.stored, self.waited, now)
+            trained, stored, waited = self.trained - trained0, self.stored - stored0, self.waited - waited0
+        wall = now - t0
+        return {'trained': trained, 'stored': stored, 'ratio': trained / stored if stored else None, 'limit': self.ratio,
+                'waited': min(1.0, waited / wall) if wall > 0 else 0.0, 'wall': wall}
+
+    def snapshot(self):
+        with self.cond:
+            return {'limit': self.ratio, 'trained': self.trained, 'stored': self.stored, 'waited': self.waited,
+                    'waiting': self.waiting}
+
+
+def replay_ratio_line(stats):
+    """'replay_ratio = 31.7 limit:32 waited:0.43': an epoch's trained samples over the steps stored during it (left out when
+    nothing was stored), the limit, and the fraction of its wall time the trainer waited for credit (ReplayRatioLimiter.end_epoch)."""
+    head = '%.1f ' % stats['ratio'] if stats['ratio'] is not None else ''
+    return 'replay_ratio = %slimit:%g waited:%.2f' % (head, stats['limit'], stats['waited'])
+
+
 def nonfinite_guard(args):
     """train_args['skip_nonfinite'] -> whether optimiser steps whose loss or gradient is not finite are rejected on the device
     (key absent, False or None: off)."""
@@ -488,7 +589,9 @@ class PendingModel:
     (`host_val`), it prints their lines after the loss line and leaves their sums in `validation` (what
     LearnerStep.pop_validation() returns).  `host_losses` holds the learner's accumulator in the layout `diagnostics` and
     `skip_nonfinite` give (accum_slots); with the guard, the number of the epoch's `batch_cnt` steps that were rejected is left
-    in `skipped` and, when it is not zero, printed (skipped_line) after the loss and diagnostics lines."""
+    in `skipped` and, when it is not zero, printed (skipped_line) after the loss and diagnostics lines.  The Trainer sets
+    `replay_ratio` to the epoch's ReplayRatioLimiter.end_epoch() figures under train_args['replay_ratio'], and report() prints
+    them (replay_ratio_line) after those lines and before the validation lines."""
 
     def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host_avg=None, host_optim=None,
                  steps=0, host_val=None, diagnostics=False, skip_nonfinite=False, batch_cnt=0):
@@ -501,6 +604,7 @@ class PendingModel:
         self.optim_state = None
         self.validation = None
         self.skipped = 0
+        self.replay_ratio = None
 
     def report(self):
         """Read the epoch's sums from the host copy (already arrived) and print the epoch's lines; returns the loss sums."""
@@ -520,6 +624,8 @@ class PendingModel:
                 print(ops.format_diagnostics(self.diagnostics))
         if self.skipped:
             print(skipped_line(self.skipped, self.batch_cnt))
+        if self.replay_ratio is not None:
+            print(replay_ratio_line(self.replay_ratio))
         if self.host_val is not None:
             self.validation = self.stepper.validation_sums(self.host_val.tolist())
             for name, val in self.validation.items():
@@ -1405,17 +1511,21 @@ class GpuBatcher:
     and writes the descriptors and the importance weights straight into the buffers the gather and the step read.  The host
     only snapshots (head, count) under the locks, as it does to sample; the Philox key comes from the seed
     (priority.sampler_key) and the counter is the number of batches drawn.  Symmetry transforms are still drawn on the host.
-    fill_validation() keeps the host sampler."""
+    fill_validation() keeps the host sampler.
+
+    With a `limiter` (a ReplayRatioLimiter, train_args['replay_ratio']), the feeder adds the steps of the episodes it committed
+    to the training ring after each commit; held-out episodes add nothing."""
 
     DESC_SLOTS = 4        # pinned descriptor buffers in rotation: bounds how far the host runs ahead of the GPU
 
-    def __init__(self, args, episodes, device, seed=None, forward=None, keep_validation=True):
+    def __init__(self, args, episodes, device, seed=None, forward=None, keep_validation=True, limiter=None):
         from .replay import DeviceReplay
         from .wire import episode_to_flat
         self.args = args
         self.validation = validation_rate(args)
         self.device = device
         self.forward = forward              # multi-GPU: callable(list of episodes) that ships them to the other ranks
+        self.limiter = limiter
         self.pending = queue.Queue()
         self.upload_stream = torch.cuda.Stream(device=device)
         self.last_upload = None
@@ -1521,6 +1631,8 @@ class GpuBatcher:
                         ev = torch.cuda.Event()
                         ev.record(self.upload_stream)
                         self.last_upload = ev
+                if self.limiter is not None and train:       # before `fed` moves: a ready() replay has its credit
+                    self.limiter.store(sum(fe.steps for fe in train))
             except Exception:
                 traceback.print_exc()
             self.fed += len(eps)
@@ -1682,9 +1794,17 @@ class Trainer:
     advantages, and weighted to correct the bias (LearnerStep, GpuBatcher).  The printed lines keep their format; the loss
     line reports the weighted objective.  Validation batches use the host sampler and no weights.  Each rank keeps the
     priorities of its own shard.  Priorities are not saved: after a restart every episode starts at max_prio.  Needs
-    gpu_replay."""
+    gpu_replay.
+
+    train_args['replay_ratio'] = r > 0: before each batch (each chunk with several GPUs) the trainer thread waits until the
+    samples trained since this Trainer started, that batch included, are at most r times the steps stored in the training
+    replay since then (ReplayRatioLimiter; the backlog counts, held-out episodes and validation batches do not).  So that
+    update() cannot deadlock the Learner, an epoch that has not taken a step yet when update() waits lets one step (chunk)
+    through: each epoch exceeds the limit by at most that.  Each epoch prints 'replay_ratio = <ratio> limit:<r>
+    waited:<fraction>' after the loss, diagnostics and skipped lines; replay_ratio_stats() returns the counts."""
 
     def __init__(self, args, model):
+        ratio = replay_ratio(args)
         self.weight_ema = weight_ema_decay(args.get('weight_ema'))
         self.validation = validation_rate(args)
         self.symmetry = symmetry.config(args)
@@ -1703,6 +1823,12 @@ class Trainer:
         self.gpu_batcher = None
         self.default_lr = 3e-8
         self.data_cnt_ema = self.args['batch_size'] * self.args['forward_steps']
+        self.limiter = None
+        self.replay_ratio_epoch = None       # the figures of the last epoch update() handed over
+        if ratio is not None:
+            self.limiter = ReplayRatioLimiter(ratio, self.data_cnt_ema)
+            if not self.gpu_replay:          # the host batcher samples this deque: what it appends is stored
+                self.episodes.listener = lambda ep: self.limiter.store(ep['steps'])
         self.params = list(self.model.parameters())
         self.lr = self.default_lr * self.data_cnt_ema
         self.steps = 0
@@ -1728,10 +1854,14 @@ class Trainer:
         state_dict rebuild and the pickling happen here, on the caller's thread."""
         while True:
             self.update_flag = True
+            if self.limiter is not None:
+                self.limiter.wake()          # a trainer waiting for credit ends its epoch now
             item, steps = self.update_queue.get()
             if not isinstance(item, PendingModel):
                 return item, steps
             model, sums = item.resolve()
+            if self.limiter is not None:
+                self.replay_ratio_epoch = item.replay_ratio
             if sums['dcnt'] > 0:           # train.py:357: an epoch needs at least one sample with a turn in it
                 break
         if self.checkpoint_files is not None:
@@ -1745,6 +1875,15 @@ class Trainer:
         self.data_cnt_ema = self.data_cnt_ema * 0.8 + sums['dcnt'] / (1e-2 + item.batch_cnt) * 0.2
         self.lr = self.default_lr * self.data_cnt_ema / (1 + steps * 1e-5)
         return model, steps
+
+    def replay_ratio_stats(self):
+        """None without train_args['replay_ratio']; otherwise the limiter's counts since this Trainer started: {'limit': r,
+        'trained': samples trained, 'stored': steps stored in the training replay, 'waited': seconds the trainer thread spent
+        waiting for credit, 'waiting': whether it waits now, 'epoch': the figures of the last epoch update() handed over (what
+        its replay_ratio line printed: ReplayRatioLimiter.end_epoch), or None before the first}."""
+        if self.limiter is None:
+            return None
+        return dict(self.limiter.snapshot(), epoch=self.replay_ratio_epoch)
 
     def _start_stepper(self):
         # the first batch is built on the host: it fixes every shape of the captured step
@@ -1778,7 +1917,8 @@ class Trainer:
         self.batcher.pool = [self.stepper.new_packed() for _ in range(4)]
         if self.gpu_replay:
             self.gpu_batcher = GpuBatcher(self.args, self.episodes, self.stepper.device,
-                                          forward=self.fleet.send_episodes if self.fleet is not None else None)
+                                          forward=self.fleet.send_episodes if self.fleet is not None else None,
+                                          limiter=self.limiter)
             self.gpu_batcher.run()
         loss_buf = self.stepper.loss_buf
         self.heads = ['p'] + (['v'] if loss_buf.dvalue is not None else []) + \
@@ -1790,6 +1930,8 @@ class Trainer:
             return self.model
         batch_cnt = 0
         chunk = int(self.args.get('multi_gpu_chunk', 8))
+        if self.limiter is not None:
+            self.limiter.start_epoch()
         while True:
             if self.stop_event.is_set() and (self.fleet is None or batch_cnt % chunk == 0):
                 return None                 # (sharded: only between chunks -- the other ranks run whole chunks)
@@ -1800,6 +1942,15 @@ class Trainer:
                     if self.stop_event.is_set():
                         return None
                     time.sleep(0.01)
+            if self.limiter is not None and (self.fleet is None or batch_cnt % chunk == 0):
+                if not self.limiter.acquire(1 if self.fleet is None else chunk,
+                                            lambda: self.stop_event.is_set() or self.update_flag):
+                    if self.stop_event.is_set():
+                        return None
+                    if batch_cnt > 0:
+                        break               # update() waits: end the epoch without another step
+                    # update() waits for an epoch that has no step yet: this step (chunk) goes through over the limit
+            if self.gpu_batcher is not None:
                 if self.fleet is not None and batch_cnt % chunk == 0:
                     self.fleet.run_steps(chunk)          # every rank runs exactly the steps rank 0 runs
                 self.gpu_batcher.fill(self.stepper)
@@ -1819,6 +1970,8 @@ class Trainer:
                 self.stepper.step(packed)
             batch_cnt += 1
             self.steps += 1
+            if self.limiter is not None:
+                self.limiter.drew()
             if self.update_flag and (self.fleet is None or batch_cnt % chunk == 0):
                 break
         # epoch boundary: nothing here waits for the GPU (LearnerStep.end_epoch)
@@ -1826,6 +1979,8 @@ class Trainer:
             self.fleet.end_epoch(batch_cnt, self.steps, self.default_lr)
         pending = self.stepper.end_epoch(batch_cnt, self.steps, self.default_lr, self.cpu_template, self.heads)
         pending.batch_cnt = batch_cnt
+        if self.limiter is not None:
+            pending.replay_ratio = self.limiter.end_epoch()
         return pending
 
     def _first_host_batch(self):
@@ -1858,6 +2013,8 @@ class Trainer:
         """Not in the reference (its threads die with the process): lets tests and embedders shut the
         trainer down cleanly -- stops the batcher threads, the helper ranks, and ends run()."""
         self.stop_event.set()
+        if self.limiter is not None:
+            self.limiter.wake()
         self.batcher.stop()
         if self.gpu_batcher is not None:
             self.gpu_batcher.stop()
