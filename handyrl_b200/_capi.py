@@ -174,6 +174,7 @@ SYMBOLS = {
     'hrl_conv_wgrad_reduce2': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p]),
     'hrl_conv_wgrad_reduce': (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     'hrl_board_pack_many': (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
+    'hrl_board_pack_many_pivot': (C.c_int, [C.c_void_p, C.c_int32] + [C.c_void_p] * 3 + [C.c_int32] * 3 + [C.c_void_p]),
     'hrl_board_fold_many': (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),
     'hrl_board_fold': (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p] + [C.c_int32] * 6 + [C.c_void_p]),
     'hrl_gemm_effective_splits': (C.c_int32, [C.c_int64, C.c_int32]),

@@ -5,6 +5,9 @@
 // matrix, CTA = (256 columns) x (a slab of rows).
 //   forward : stats partials -> per-channel mean / rstd (+ running stats, as nn.BatchNorm2d) -> normalise
 //   backward: partials of sum(dy), sum(dy * xhat) -> per-channel dbeta / dgamma -> dx
+// The forward sums are shifted by a per-channel pivot K_c = the channel's value in row 0: var = E[(x-K)^2] - E[x-K]^2.
+// Unshifted fp32 sums of x and x^2 lose the variance to cancellation once |mean| / std reaches the hundreds; shifted, the
+// sums are of size std and the variance keeps fp32 accuracy whatever the mean (DESIGN.md, "BatchNorm statistics").
 #include "common.cuh"
 
 namespace hrl {
@@ -15,20 +18,21 @@ __global__ void __launch_bounds__(kBnCols) bn_partials_kernel(const float *__res
                                                               const float *__restrict__ mean, const float *__restrict__ rstd,
                                                               int64_t N, int CHW, int HW, int rows_per_slab,
                                                               float *__restrict__ p0, float *__restrict__ p1, int C) {
-    // forward (dy == nullptr): p0 = sum x, p1 = sum x^2;  backward: p0 = sum dy, p1 = sum dy * xhat
+    // forward (dy == nullptr): p0 = sum (x-K), p1 = sum (x-K)^2;  backward: p0 = sum dy, p1 = sum dy * xhat
     const int j = blockIdx.x * kBnCols + threadIdx.x;
     if (j >= CHW) return;
     const int64_t r0 = (int64_t)blockIdx.y * rows_per_slab, r1 = min(N, r0 + rows_per_slab);
+    const int c = (j / HW) % C;              // NCHW: j = c*HW + h;  channels-last (HW passed as 1): j = f*C + c
     float a = 0.f, b = 0.f;
     if (dy == nullptr) {
+        const float K = __ldg(x + c * HW);   // the pivot: row 0, the channel's first column
 #pragma unroll 4
         for (int64_t r = r0; r < r1; r++) {
-            const float v = __ldg(x + r * CHW + j);
+            const float v = __ldg(x + r * CHW + j) - K;
             a += v;
             b = fmaf(v, v, b);
         }
     } else {
-        const int c = (j / HW) % C;          // NCHW: j = c*HW + h;  channels-last (HW passed as 1): j = f*C + c
         const float m = mean[c], rs = rstd[c];
 #pragma unroll 4
         for (int64_t r = r0; r < r1; r++) {
@@ -42,8 +46,8 @@ __global__ void __launch_bounds__(kBnCols) bn_partials_kernel(const float *__res
     p1[(int64_t)blockIdx.y * CHW + j] = b;
 }
 
-// one CTA per channel folds the partials (slabs x HW columns) in fp64
-__global__ void __launch_bounds__(256) bn_finalize_fwd_kernel(const float *__restrict__ p0, const float *__restrict__ p1, int slabs,
+// one CTA per channel folds the partials (slabs x HW columns) in fp64 and adds the pivot x[c * cmul] back to the mean
+__global__ void __launch_bounds__(256) bn_finalize_fwd_kernel(const float *__restrict__ x, const float *__restrict__ p0, const float *__restrict__ p1, int slabs,
                                                               int CHW, int reps, int cmul, int istride, double count, float eps, float momentum,
                                                               float *__restrict__ mean, float *__restrict__ rstd,
                                                               float *__restrict__ running_mean, float *__restrict__ running_var) {
@@ -62,8 +66,8 @@ __global__ void __launch_bounds__(256) bn_finalize_fwd_kernel(const float *__res
     if (threadIdx.x == 0) {
         s = 0.0; q = 0.0;
         for (int w = 0; w < 8; w++) { s += rs_[w]; q += rq_[w]; }
-        const double m = s / count;
-        double var = q / count - m * m;          // biased, as F.batch_norm normalises with
+        const double d = s / count, m = (double)x[c * cmul] + d;
+        double var = q / count - d * d;          // biased, as F.batch_norm normalises with
         if (var < 0.0) var = 0.0;
         mean[c] = (float)m;
         rstd[c] = (float)(1.0 / sqrt(var + (double)eps));
@@ -97,7 +101,8 @@ __global__ void __launch_bounds__(256) bn_finalize_bwd_kernel(const float *__res
     }
 }
 
-// forward: y = (x - mean) * rstd * gamma + beta;  backward: dx = gamma * rstd * (dy - dbeta/M - xhat * dgamma/M)
+// forward: y = (x - mean) * rstd * gamma + beta  (x - mean first: x * scale + (beta - mean * scale) cancels when |mean| >> std)
+// backward: dx = gamma * rstd * (dy - dbeta/M - xhat * dgamma/M)
 __global__ void __launch_bounds__(kBnCols) bn_apply_kernel(const float *__restrict__ x, const float *__restrict__ dy,
                                                            const float *__restrict__ gamma, const float *__restrict__ beta,
                                                            const float *__restrict__ mean, const float *__restrict__ rstd,
@@ -110,9 +115,9 @@ __global__ void __launch_bounds__(kBnCols) bn_apply_kernel(const float *__restri
     const int64_t r0 = (int64_t)blockIdx.y * rows_per_slab, r1 = min(N, r0 + rows_per_slab);
     const float m = mean[c], rs = rstd[c], g = gamma ? gamma[c] : 1.0f;
     if (dy == nullptr) {
-        const float scale = rs * g, shift = (beta ? beta[c] : 0.0f) - m * scale;
+        const float scale = rs * g, b = beta ? beta[c] : 0.0f;
 #pragma unroll 4
-        for (int64_t r = r0; r < r1; r++) __stcs(out + r * CHW + j, fmaf(__ldg(x + r * CHW + j), scale, shift));
+        for (int64_t r = r0; r < r1; r++) __stcs(out + r * CHW + j, fmaf(__ldg(x + r * CHW + j) - m, scale, b));
     } else {
         const float k = g * rs, mb = dbeta[c] * inv_count, mg = dgamma[c] * inv_count;
 #pragma unroll 4
@@ -178,7 +183,7 @@ extern "C" int hrl_bn_train_fwd(const float *x, const float *gamma, const float 
     bn_grid(b.rows, b.cols, slabs, rps, grid);
     float *p0 = workspace, *p1 = workspace + (size_t)slabs * b.cols;
     bn_partials_kernel<<<grid, kBnCols, 0, s>>>(x, nullptr, nullptr, nullptr, b.rows, b.cols, b.cdiv, rps, p0, p1, C);
-    bn_finalize_fwd_kernel<<<C, 256, 0, s>>>(p0, p1, slabs, b.cols, b.reps, b.cmul, b.istride, (double)N * HW, eps, momentum, mean, rstd,
+    bn_finalize_fwd_kernel<<<C, 256, 0, s>>>(x, p0, p1, slabs, b.cols, b.reps, b.cmul, b.istride, (double)N * HW, eps, momentum, mean, rstd,
                                              running_mean, running_var);
     bn_apply_kernel<<<grid, kBnCols, 0, s>>>(x, nullptr, gamma, beta, mean, rstd, nullptr, nullptr, 0.0f, b.rows, b.cols, b.cdiv, rps, y, C);
     HRL_CUDA_CHECK(cudaGetLastError());

@@ -740,7 +740,8 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
     // ---- epilogue: registers -> shared-memory tile (padded rows) -> coalesced global stores.
     // (a thread holds 2 columns of 2 rows per 8-column group: storing from registers would scatter every warp instruction)
     //   HRL_GEMM_EP_RELU        C = max(acc, 0)
-    //   HRL_GEMM_EP_STATS       C = acc, plus per-column sum and sum of squares over the tile's rows
+    //   HRL_GEMM_EP_STATS       C = acc, plus per-column sum and sum of squares of acc - mean over the tile's rows (mean = the
+    //                           pivot ep_mean, or 0: shifted sums keep the variance when |mean| >> std)
     //   HRL_GEMM_EP_MASK_STATS  C = acc * (z > 0) with z = y*scale+shift of the pre-activation tile y (the ReLU
     //                           backward), plus per-column sums of C and of C * xhat, xhat = (y - mean) * rstd
     //                           (the two batch sums the BatchNorm backward needs)
@@ -796,7 +797,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
         float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
         if (mine) {
             float k_sc[4] = {1.f, 1.f, 1.f, 1.f}, k_sh[4] = {0.f, 0.f, 0.f, 0.f}, k_mu[4] = {0.f, 0.f, 0.f, 0.f}, k_rs[4] = {1.f, 1.f, 1.f, 1.f};
-            if (masked) {
+            if (masked || ep == HRL_GEMM_EP_STATS) {
 #pragma unroll
                 for (int e = 0; e < 4; e++) {
                     const int col = n0 + 4 * my_c4 + e;
@@ -815,9 +816,12 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
                     if (ep == HRL_GEMM_EP_RELU) {
                         v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
                     } else if (ep == HRL_GEMM_EP_STATS) {
-                        s1[0] += v.x; s1[1] += v.y; s1[2] += v.z; s1[3] += v.w;
-                        s2[0] = fmaf(v.x, v.x, s2[0]); s2[1] = fmaf(v.y, v.y, s2[1]);
-                        s2[2] = fmaf(v.z, v.z, s2[2]); s2[3] = fmaf(v.w, v.w, s2[3]);
+                        const float d[4] = {v.x - k_mu[0], v.y - k_mu[1], v.z - k_mu[2], v.w - k_mu[3]};
+#pragma unroll
+                        for (int e = 0; e < 4; e++) {
+                            s1[e] += d[e];
+                            s2[e] = fmaf(d[e], d[e], s2[e]);
+                        }
                     } else if (masked) {
                         const float4 y = yq[u];
                         const int rn = r + kAhead * rpp;

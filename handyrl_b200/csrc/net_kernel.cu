@@ -68,9 +68,23 @@ struct PackJobs {
     HrlPackJob job[HRL_MAX_BOARD_JOBS];
     int first_block[HRL_MAX_BOARD_JOBS + 1];
     int n;
+    // BatchNorm statistics pivots (hrl_board_pack_many_pivot), in the blocks after the jobs' blocks
+    const float *rm[HRL_MAX_BOARD_JOBS], *rv[HRL_MAX_BOARD_JOBS];
+    float *pivot[HRL_MAX_BOARD_JOBS];
+    int layers, C, HW;
 };
 
 __global__ void board_pack_kernel(const PackJobs jobs) {
+    if ((int)blockIdx.x >= jobs.first_block[jobs.n]) {
+        // pivot = the running mean where |running mean| > 32 running std, else 0 (unshifted sums, bit for bit)
+        const int per_layer = (jobs.C * jobs.HW + 255) / 256, b = blockIdx.x - jobs.first_block[jobs.n];
+        const int l = b / per_layer, i = (b - l * per_layer) * 256 + threadIdx.x;
+        if (i < jobs.C * jobs.HW) {
+            const float m = jobs.rm[l][i / jobs.HW], v = jobs.rv[l][i / jobs.HW];
+            jobs.pivot[l][i] = m * m > 1024.f * v ? m : 0.f;
+        }
+        return;
+    }
     int k = 0;
     while (k + 1 < jobs.n && (int)blockIdx.x >= jobs.first_block[k + 1]) k++;
     board_pack_body(jobs.job[k], blockIdx.x - jobs.first_block[k], jobs.first_block[k + 1] - jobs.first_block[k]);
@@ -385,10 +399,20 @@ extern "C" int hrl_conv_wgrad_reduce(const float *partials, int32_t splits, floa
     return hrl_conv_wgrad_reduce2(partials, splits, taps * Cin, dw, nullptr, Cout, Cin, taps, 0, stream);
 }
 
-extern "C" int hrl_board_pack_many(const HrlPackJob *jobs, int32_t n_jobs, void *stream) {
-    HRL_REQUIRE(jobs && n_jobs >= 1 && n_jobs <= HRL_MAX_BOARD_JOBS, HRL_ERR_BAD_ARG, "hrl_board_pack_many: 1..%d jobs", HRL_MAX_BOARD_JOBS);
+extern "C" int hrl_board_pack_many_pivot(const HrlPackJob *jobs, int32_t n_jobs, const float *const *running_mean, const float *const *running_var,
+                                         float *const *pivot_col, int32_t layers, int32_t C, int32_t HW, void *stream) {
+    HRL_REQUIRE((jobs || n_jobs == 0) && n_jobs >= 0 && n_jobs <= HRL_MAX_BOARD_JOBS && layers >= 0 && layers <= HRL_MAX_BOARD_JOBS &&
+                    n_jobs + layers >= 1,
+                HRL_ERR_BAD_ARG, "hrl_board_pack_many: 1..%d jobs and 0..%d pivot layers", HRL_MAX_BOARD_JOBS, HRL_MAX_BOARD_JOBS);
+    HRL_REQUIRE(layers == 0 || (running_mean && running_var && pivot_col && C > 0 && HW > 0), HRL_ERR_BAD_ARG,
+                "hrl_board_pack_many_pivot: NULL pointer or bad shape");
     PackJobs pj;
     pj.n = n_jobs;
+    pj.layers = layers; pj.C = C; pj.HW = HW;
+    for (int l = 0; l < layers; l++) {
+        HRL_REQUIRE(running_mean[l] && running_var[l] && pivot_col[l], HRL_ERR_BAD_ARG, "hrl_board_pack_many_pivot: NULL pointer");
+        pj.rm[l] = running_mean[l]; pj.rv[l] = running_var[l]; pj.pivot[l] = pivot_col[l];
+    }
     pj.first_block[0] = 0;
     for (int k = 0; k < n_jobs; k++) {
         const HrlPackJob &j = jobs[k];
@@ -405,9 +429,15 @@ extern "C" int hrl_board_pack_many(const HrlPackJob *jobs, int32_t n_jobs, void 
         if (blocks > 2 * kNumSM) blocks = 2 * kNumSM;
         pj.first_block[k + 1] = pj.first_block[k] + blocks;
     }
-    board_pack_kernel<<<pj.first_block[n_jobs], 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(pj);
+    const int pivot_blocks = layers ? layers * ((C * HW + 255) / 256) : 0;
+    board_pack_kernel<<<pj.first_block[n_jobs] + pivot_blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(pj);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
+}
+
+extern "C" int hrl_board_pack_many(const HrlPackJob *jobs, int32_t n_jobs, void *stream) {
+    HRL_REQUIRE(jobs && n_jobs >= 1, HRL_ERR_BAD_ARG, "hrl_board_pack_many: 1..%d jobs", HRL_MAX_BOARD_JOBS);
+    return hrl_board_pack_many_pivot(jobs, n_jobs, nullptr, nullptr, nullptr, 0, 0, 0, stream);
 }
 
 extern "C" int hrl_board_pack(const float *w, int32_t Cout, int32_t Cin, int32_t kh, int32_t kw, int32_t H, int32_t W, float *image_fwd,

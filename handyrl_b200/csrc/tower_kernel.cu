@@ -1,7 +1,8 @@
 // Small kernels between the fused tensor-core products of a conv -> BatchNorm -> ReLU tower over a tiny board
 // (handyrl_b200/tower.py; the architecture of the reference's SimpleConv2dModel, envs/tictactoe.py:52-69):
 //
-//   hrl_bn_finalize_fwd   column sums of a layer's raw output (written by hrl_gemm_fused, epilogue STATS) -> per-channel batch
+//   hrl_bn_finalize_fwd   column sums of a layer's output less a pivot (written by hrl_gemm_fused, epilogue STATS, pivot =
+//                         ep_mean = mean_col as it is on entry) -> per-channel batch
 //                         mean / biased variance -> running statistics (nn.BatchNorm2d semantics) and, per COLUMN of the
 //                         (samples x C*HW) activation matrix, the constants the next product's operand transform applies:
 //                         scale = gamma*rstd, shift = beta - mean*scale (plus mean and rstd for the backward)
@@ -27,7 +28,8 @@ __device__ __forceinline__ void block_sum2(double &s, double &q) {
     __syncthreads();
 }
 
-// one CTA per channel
+// one CTA per channel; the sums are of y - K with the pivot K = mean_col[c * HW] on entry (the caller keeps it equal over a
+// channel's columns), read before mean_col is overwritten
 __global__ void __launch_bounds__(256) bn_tower_finalize_fwd_kernel(const float *__restrict__ partials, int tiles, int C, int HW, double count,
                                                                     const float *__restrict__ gamma, const float *__restrict__ beta, float eps,
                                                                     float momentum, float *__restrict__ running_mean,
@@ -35,6 +37,7 @@ __global__ void __launch_bounds__(256) bn_tower_finalize_fwd_kernel(const float 
                                                                     float *__restrict__ mean_col, float *__restrict__ rstd_col,
                                                                     float *__restrict__ scale_col, float *__restrict__ shift_col) {
     const int c = blockIdx.x, N = C * HW;
+    const double K = (double)mean_col[c * HW];  // (block_sum2's barriers order this read before the stores below)
     double s = 0.0, q = 0.0;
     for (int i = threadIdx.x; i < tiles * HW; i += blockDim.x) {
         const int t = i / HW, h = i - t * HW;
@@ -42,8 +45,8 @@ __global__ void __launch_bounds__(256) bn_tower_finalize_fwd_kernel(const float 
         q += (double)partials[((long long)t * 2 + 1) * N + c * HW + h];
     }
     block_sum2(s, q);
-    const double m = s / count;
-    double var = q / count - m * m;              // biased: what F.batch_norm normalises with
+    const double d = s / count, m = K + d;
+    double var = q / count - d * d;              // biased: what F.batch_norm normalises with
     if (var < 0.0) var = 0.0;
     const float mf = (float)m, rs = (float)(1.0 / sqrt(var + (double)eps));
     const float sc = gamma[c] * rs, sh = beta[c] - mf * sc;

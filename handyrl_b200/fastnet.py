@@ -182,11 +182,10 @@ class BoardBatchNorm2d(nn.BatchNorm2d):
     (cuDNN's spatial BN kernels launch one CTA per channel: ~1 ms at N=16384, C=32)."""
 
     def forward(self, x):
-        if not (self.training and x.dim() == 4 and x.shape[2] * x.shape[3] <= MAX_CELLS and self.track_running_stats):
+        if not (self.training and x.dim() == 4 and x.shape[2] * x.shape[3] <= MAX_CELLS and self.track_running_stats
+                and self.momentum is not None):      # (momentum None: a cumulative average, left to nn.BatchNorm2d)
             return super().forward(x)
         N, C, H, W = x.shape
-        if self.momentum is None:
-            raise NotImplementedError('cumulative moving average BatchNorm is not rewritten')
         if x.is_cuda and x.dtype == torch.float32 and self.affine:
             # fused kernels (csrc/bn_kernel.cu): 3 coalesced passes forward, 3 backward
             from . import ops

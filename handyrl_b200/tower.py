@@ -133,16 +133,25 @@ class FusedBoardNet:
         if epilogue in ('stats', 'mask_stats'):
             g.col_partials = _ptr(self.cp)
         if ep is not None:
-            g.ep_y, g.ep_ldy = _ptr(ep['y']), ep['y'].stride(0)
+            if 'y' in ep:
+                g.ep_y, g.ep_ldy = _ptr(ep['y']), ep['y'].stride(0)
             g.ep_scale, g.ep_shift = _ptr(ep.get('scale')), _ptr(ep.get('shift'))
             g.ep_mean, g.ep_rstd = _ptr(ep.get('mean')), _ptr(ep.get('rstd'))
         check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
         _count(2 if (splits > 1 and not partial) else 1)
 
     def _pack_all(self, jobs):
-        """jobs: dicts of HrlPackJob fields with tensors for the pointers -- one launch for up to MAX_BOARD_JOBS convolutions."""
+        """jobs: dicts of HrlPackJob fields with tensors for the pointers -- one launch for up to MAX_BOARD_JOBS convolutions.
+        The same launches write each tower layer's BatchNorm statistics pivot into its `mean` (up to MAX_BOARD_JOBS layers per
+        launch; there are fewer tower layers than jobs): the running mean where |running mean| >> running std, else 0.  The
+        statistics epilogue sums y - pivot and hrl_bn_finalize_fwd adds the pivot back, so that fp32 sums of y and y^2 do not
+        cancel when |mean| >> std.  The running statistics are saved state: a step's arithmetic depends on nothing a
+        checkpoint or a rejected step leaves out."""
+        bns = [(blk[1], st) for blk, st in zip(self.model.tower, self.bn)]
+        pivots = lambda ts: C.cast((C.c_void_p * max(1, len(ts)))(*[t.data_ptr() for t in ts]), C.c_void_p)
         for i in range(0, len(jobs), MAX_BOARD_JOBS):
             chunk = jobs[i:i + MAX_BOARD_JOBS]
+            piv = bns[i:i + MAX_BOARD_JOBS]
             arr = (HrlPackJob * len(chunk))()
             for j, kw in zip(arr, chunk):
                 w = kw['w']
@@ -150,7 +159,9 @@ class FusedBoardNet:
                 j.image_fwd, j.fwd_rows, j.fwd_row0 = _ptr(kw.get('fwd')), kw.get('fwd_rows', 0), kw.get('fwd_row0', 0)
                 j.image_bwd, j.bwd_rows, j.bwd_k0 = _ptr(kw.get('bwd')), kw.get('bwd_rows', 0), kw.get('bwd_k0', 0)
                 j.bias, j.bias_cells = _ptr(kw.get('bias')), _ptr(kw.get('bias_cells'))
-            check(lib().hrl_board_pack_many(C.byref(arr), len(chunk), _stream_ptr()))
+            check(lib().hrl_board_pack_many_pivot(C.byref(arr), len(chunk), pivots([b.running_mean for b, _ in piv]),
+                                                  pivots([b.running_var for b, _ in piv]), pivots([st['mean'] for _, st in piv]),
+                                                  len(piv), self.width, self.cells, _stream_ptr()))
             _count()
 
     def _fold_all(self):
@@ -198,13 +209,13 @@ class FusedBoardNet:
             for sq_, row0 in heads:       # the squeeze convolutions side by side in ONE operand
                 jobs.append(dict(w=sq_.weight, fwd=self.Whf, fwd_rows=self.NH, fwd_row0=row0, bwd=self.Whb, bwd_rows=D, bwd_k0=row0,
                                  bias=sq_.bias, bias_cells=self.bh[row0:]))
-            self._pack_all(jobs)
+            self._pack_all(jobs)          # (and the BatchNorm statistics pivots)
             # stem: bias + ReLU in the epilogue
             self._gemm(dict(t=self.x2d), dict(t=self.W0f, packed=True), self.A0, K=self.K0, N=D, bias=self.b0, epilogue='relu')
             src = dict(t=self.A0)
             for l, blk in enumerate(m.tower):
                 bnm, st = blk[1], self.bn[l]
-                self._gemm(src, dict(t=self.Wf[l], packed=True), self.Y[l], K=D, N=D, epilogue='stats')
+                self._gemm(src, dict(t=self.Wf[l], packed=True), self.Y[l], K=D, N=D, epilogue='stats', ep=dict(mean=st['mean']))
                 check(lib().hrl_bn_finalize_fwd(_ptr(self.cp), self.tiles, self.width, self.cells, M_, _ptr(bnm.weight), _ptr(bnm.bias),
                                                 float(bnm.eps), float(bnm.momentum), _ptr(bnm.running_mean), _ptr(bnm.running_var),
                                                 _ptr(bnm.num_batches_tracked), _ptr(st['mean']), _ptr(st['rstd']), _ptr(st['scale']),

@@ -317,8 +317,9 @@ int hrl_gemm_tf32x3(const float *A, int64_t lda, int32_t a_kmajor, const float *
  *                       BatchNorm-apply + ReLU of the previous layer (x = its raw output, p = gamma*rstd, r = beta - mean*p),
  *                       or the BatchNorm backward dY = dZ*p + Y*q + r (x = dZ, y = Y).  f = the reduction index, or the
  *                       operand row when feature_is_row (transposed operands of the weight-gradient product).
- *   epilogues           RELU: C = max(acc + bias, 0).  STATS: C = acc and per-column sum / sum of squares of the tile
- *                       (BatchNorm batch statistics of this layer's output).  MASK_STATS: C = acc * (z > 0) with
+ *   epilogues           RELU: C = max(acc + bias, 0).  STATS: C = acc and per-column sum / sum of squares of C - ep_mean
+ *                       over the tile (BatchNorm batch statistics of this layer's output, shifted by a pivot near the
+ *                       mean so that they do not cancel; ep_mean NULL = no shift).  MASK_STATS: C = acc * (z > 0) with
  *                       z = y*scale + shift of the pre-activation y (ReLU backward) and per-column sums of C and
  *                       C * (y - mean) * rstd (the two batch sums of the BatchNorm backward).
  * Column sums land in col_partials[row_tile][2][N] (row_tile = ceil(M/128) tiles, summed by hrl_bn_finalize_*).
@@ -348,7 +349,8 @@ typedef struct HrlGemmArgs {
     const float *ep_y;           /* MASK_STATS: pre-activation tile (M x N)                            */
     int64_t ep_ldy;
     const float *ep_scale, *ep_shift;   /* per column; NULL = 1 / 0                                    */
-    const float *ep_mean, *ep_rstd;     /* per column; NULL = second sum is sum(C * y)                 */
+    const float *ep_mean, *ep_rstd;     /* per column; MASK_STATS: NULL = second sum is sum(C * y);
+                                           STATS: ep_mean = the pivot of the sums, ep_rstd unused     */
     float *col_partials;         /* [ceil(M/128)][2][N] floats, or NULL                                */
     /* Convolution over a board as an implicit product (replaces cuDNN's fp32 SIMT kernels for the stride-1 "same" / wrap-around
      * convolutions of the board nets: reference geister.py:18-56 ConvLSTM cells, hungry_geese.py:20-37 TorusConv2d).  Activations
@@ -390,7 +392,9 @@ int hrl_gemm_fused(const HrlGemmArgs *args, void *stream);
  * Glue of a fused conv -> BatchNorm -> ReLU tower over a tiny board (handyrl_b200/tower.py: the architecture of the
  * reference's SimpleConv2dModel, envs/tictactoe.py:52-69, with every layer ONE hrl_gemm_fused launch per direction).
  *   hrl_bn_finalize_fwd   col_partials [tiles][2][C*HW] (column sum / sum of squares from the STATS epilogue) -> batch
- *                         statistics of nn.BatchNorm2d in training mode (running stats with `momentum`, unbiased running
+ *                         statistics.  mean_col is read first: on entry it holds the pivot that product subtracted (its
+ *                         ep_mean, equal over each channel's columns; zeros for unshifted sums); then it receives the
+ *                         batch mean.  Statistics of nn.BatchNorm2d in training mode (running stats with `momentum`, unbiased running
  *                         variance, num_batches_tracked += 1) and per-COLUMN mean / rstd / scale = gamma*rstd /
  *                         shift = beta - mean*scale (each C*HW floats) for the next product's operand transform
  *   hrl_bn_finalize_bwd   col_partials (column sums of dZ and dZ*xhat from the MASK_STATS epilogue) -> dgamma, dbeta and
@@ -461,6 +465,13 @@ typedef struct HrlFoldJob {
     int32_t Cout, Cin, kh, kw, H, W;
 } HrlFoldJob;
 int hrl_board_pack_many(const HrlPackJob *jobs, int32_t n_jobs, void *stream);
+/* The same launch (0..HRL_MAX_BOARD_JOBS jobs) plus the pivots of the STATS epilogue's shifted BatchNorm sums for 0..HRL_MAX_BOARD_JOBS
+ * layers of C channels over HW cells (fused tower: the pivot is layer l's ep_mean and the mean_col hrl_bn_finalize_fwd reads):
+ * pivot_col[l][c*HW + h] = running_mean[l][c] where running_mean^2 > 1024 * running_var (|mean| / std > 32: unshifted fp32
+ * sums would start to lose the variance), else 0 (the sums stay those of the unshifted statistics, bit for bit).
+ * running_mean / running_var / pivot_col: host arrays of `layers` device pointers. */
+int hrl_board_pack_many_pivot(const HrlPackJob *jobs, int32_t n_jobs, const float *const *running_mean, const float *const *running_var,
+                              float *const *pivot_col, int32_t layers, int32_t C, int32_t HW, void *stream);
 int hrl_board_fold_many(const HrlFoldJob *jobs, int32_t n_jobs, void *stream);
 int hrl_board_fold(const float *ddense, int32_t splits, int64_t split_stride, float *dw, int32_t Cout, int32_t Cin, int32_t kh,
                    int32_t kw, int32_t H, int32_t W, void *stream);
