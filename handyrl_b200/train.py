@@ -437,6 +437,17 @@ def accum_slots(diagnostics, skip_nonfinite):
     return NUM_LOSS + (NUM_DIAG if diagnostics else 0) + (1 if skip_nonfinite else 0)
 
 
+# the loss pass's diagnostics sums: where they sit behind the loss sums, in the accumulator and in the gradient bucket's tail
+_LOSS_DIAG = slice(NUM_LOSS, NUM_LOSS + NUM_LOSS_DIAG)
+
+
+def _accum_layout(diagnostics, skip_nonfinite):
+    """(loss, diag, skipped) slices of an accumulator of accum_slots(diagnostics, skip_nonfinite) slots; `diag` is None
+    without diagnostics and `skipped` (one slot) None without the guard."""
+    n = NUM_LOSS + (NUM_DIAG if diagnostics else 0)
+    return slice(0, NUM_LOSS), slice(NUM_LOSS, n) if diagnostics else None, slice(n, n + 1) if skip_nonfinite else None
+
+
 def skipped_line(skipped, steps):
     """'skipped = 3 of 1200 steps: non-finite loss or gradient': the steps of an epoch the guard rejected."""
     return 'skipped = %d of %d steps: non-finite loss or gradient' % (skipped, steps)
@@ -583,22 +594,21 @@ class PendingModel:
     """The model of a finished epoch, still on its way to the host.  `resolve()` (called by Trainer.update() on the
     Learner's thread) waits for the side-stream copy only, prints the epoch's loss line, rebuilds the CPU model in
     eval mode and caches its pickled bytes on it (the Learner pickles the model for every worker request,
-    train.py:605-615).  With a moving average of the weights (`host_avg`), it also leaves the averaged state_dict, keyed
-    like the model's, in `ema_state`; with the optimiser state (`host_optim`, LearnerStep.end_epoch's layout), it leaves
-    that state in the OptimizerStateFormat dict in `optim_state`, scheduled at step count `steps`.  With validation passes
-    (`host_val`), it prints their lines after the loss line and leaves their sums in `validation` (what
-    LearnerStep.pop_validation() returns).  `host_losses` holds the learner's accumulator in the layout `diagnostics` and
+    train.py:605-615).  `host` maps the names of LearnerStep's hand-off entries to their pinned host copies.  With a moving
+    average of the weights ('avg'), it also leaves the averaged state_dict, keyed like the model's, in `ema_state`; with the
+    optimiser state ('optim', the optim_snap layout), it leaves that state in the OptimizerStateFormat dict in `optim_state`,
+    scheduled at step count `steps`.  With validation passes ('val'), it prints their lines after the loss line and leaves
+    their sums in `validation` (what LearnerStep.pop_validation() returns).  `host_losses` holds the learner's accumulator in
+    the layout `diagnostics` and
     `skip_nonfinite` give (accum_slots); with the guard, the number of the epoch's `batch_cnt` steps that were rejected is left
     in `skipped` and, when it is not zero, printed (skipped_line) after the loss and diagnostics lines.  The Trainer sets
     `replay_ratio` to the epoch's ReplayRatioLimiter.end_epoch() figures under train_args['replay_ratio'], and report() prints
     them (replay_ratio_line) after those lines and before the validation lines."""
 
-    def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host_avg=None, host_optim=None,
-                 steps=0, host_val=None, diagnostics=False, skip_nonfinite=False, batch_cnt=0):
+    def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host=None, steps=0, diagnostics=False,
+                 skip_nonfinite=False, batch_cnt=0):
         self.stepper, self.done, self.host_state, self.host_losses = stepper, done_event, host_state, host_losses
-        self.heads, self.template, self.host_avg = heads, template, host_avg
-        self.host_optim, self.steps = host_optim, steps
-        self.host_val = host_val
+        self.heads, self.template, self.host, self.steps = heads, template, host or {}, steps
         self.has_diagnostics, self.skip_nonfinite, self.batch_cnt = bool(diagnostics), bool(skip_nonfinite), batch_cnt
         self.ema_state = None
         self.optim_state = None
@@ -612,12 +622,11 @@ class PendingModel:
         if len(host) != accum_slots(self.has_diagnostics, self.skip_nonfinite):
             raise ValueError('PendingModel: %d accumulator slots, the layout has %d'
                              % (len(host), accum_slots(self.has_diagnostics, self.skip_nonfinite)))
-        sums = dict(zip(LOSS_KEYS, host[:NUM_LOSS]))
+        loss, diag, skipped = _accum_layout(self.has_diagnostics, self.skip_nonfinite)
+        sums = dict(zip(LOSS_KEYS, host[loss]))
         dcnt = sums['dcnt']
-        self.diagnostics = None
-        if self.has_diagnostics:        # the learner's diagnostics sums ride behind the loss sums
-            self.diagnostics = ops.summarize_diagnostics(host[NUM_LOSS:NUM_LOSS + NUM_DIAG])
-        self.skipped = int(host[-1]) if self.skip_nonfinite else 0
+        self.diagnostics = ops.summarize_diagnostics(host[diag]) if self.has_diagnostics else None
+        self.skipped = int(host[skipped][0]) if self.skip_nonfinite else 0
         if dcnt > 0:
             print(loss_line('loss', sums, self.heads))
             if self.diagnostics is not None:
@@ -626,8 +635,8 @@ class PendingModel:
             print(skipped_line(self.skipped, self.batch_cnt))
         if self.replay_ratio is not None:
             print(replay_ratio_line(self.replay_ratio))
-        if self.host_val is not None:
-            self.validation = self.stepper.validation_sums(self.host_val.tolist())
+        if 'val' in self.host:
+            self.validation = self.stepper.validation_sums(self.host['val'].tolist())
             for name, val in self.validation.items():
                 if val['dcnt'] > 0:
                     print(loss_line(name, val, self.heads))
@@ -636,18 +645,15 @@ class PendingModel:
     def resolve(self):
         self.done.synchronize()
         sums = self.report()
-        tpl = self.template
-        store = self.stepper.state
+        tpl, stepper = self.template, self.stepper
         keys = list(tpl.state_dict().keys())
-        state = store.state_dict_from(self.host_state, keys)
-        for k, b in store.loose:
-            state[k] = b.detach().cpu()
-        if self.host_avg is not None:           # loose buffers: the live model's
-            avg = store.state_dict_from(store.averaged_bytes(self.host_avg, self.host_state), keys)
-            self.ema_state = collections.OrderedDict((k, avg[k] if k in avg else state[k].clone()) for k in keys)
-        if self.host_optim is not None:
-            self.optim_state = self.stepper.optimizer_state_from(self.host_optim, self.steps)
-        tpl.load_state_dict(state)
+        state = stepper._state_dict_of(self.host_state)
+        if 'avg' in self.host:
+            avg = stepper._state_dict_of(stepper.state.averaged_bytes(self.host['avg'], self.host_state))
+            self.ema_state = collections.OrderedDict((k, avg[k]) for k in keys)
+        if 'optim' in self.host:
+            self.optim_state = stepper.optimizer_state_from(self.host['optim'], self.steps)
+        tpl.load_state_dict({k: state[k] for k in keys})
         tpl.eval()
         blob = pickle.dumps(tpl)
         model = pickle.loads(blob)                        # == copy.deepcopy(tpl), and leaves the bytes for the workers
@@ -661,6 +667,11 @@ def attach_pickle_cache(model, blob):
     What the workers unpickle is the plain nn.Module that `blob` holds."""
     object.__setattr__(model, '__reduce_ex__', lambda protocol, _b=blob: (pickle.loads, (_b,)))
     return model
+
+
+# LearnerStep._handoff: end_epoch fills the device buffer `snap` on the step stream by `copies`, (view of snap, live tensor)
+# pairs, runs `after()`, and carries snap to the start of PendingModel.host[name], pinned memory of `room` (or snap's) elements
+_Handoff = collections.namedtuple('_Handoff', 'name snap copies after room', defaults=(None, None))
 
 
 class LearnerStep:
@@ -712,6 +723,10 @@ class LearnerStep:
     PendingModel.skipped) goes up, and last_losses still holds the rejected step's sums.  `steps` and the host's batch counts
     keep counting batches drawn; a rejected batch adds nothing to dcnt.  One more launch per step.  Validation passes are not
     guarded.
+
+    A feature that adds device state registers it in __init__, where it allocates it: in `_mutable` (or `_zeroed`) when a
+    step or validation pass changes it, so that the capture's warm-up leaves it as it was, and in `_handoff` (a _Handoff)
+    when the epoch boundary carries it to the host; end_epoch, _snapshot and _restore have no per-feature code.
     """
 
     def __init__(self, model, args, example_batch, lr, device=None, process_group=None, use_graph=True,
@@ -731,7 +746,7 @@ class LearnerStep:
             diagnostics = bool(args.get('diagnostics', False))
         self.diagnostics = diagnostics
         n_sums = accum_slots(diagnostics, self.skip_nonfinite)             # accumulator: loss sums [+ diagnostics] [+ skips]
-        n_tail = NUM_LOSS + (NUM_LOSS_DIAG if diagnostics else 0)           # bucket tail: [+ the loss pass's diagnostics]
+        self.n_tail = _LOSS_DIAG.stop if diagnostics else NUM_LOSS         # bucket tail: [+ the loss pass's diagnostics]
         # the learner owns its precision contract (1e-5 of the reference's fp32 arithmetic): PyTorch's default lets
         # cuDNN convolutions run on TF32 tensor cores (10-bit mantissa).  train_args['allow_tf32'] = True opts out.
         if allow_tf32 is None:
@@ -768,22 +783,46 @@ class LearnerStep:
             peer_allreduce = self.world > 1 and os.environ.get('HRL_PEER_ALLREDUCE', '1') != '0'
         self.peer = ops.PeerAllReduce(self.pg, self.device) if (peer_allreduce and self.world > 1) else None
         self.state = StateStore(self.model, self.device)
-        self.opt = ops.FlatAdam(params, lr=lr, weight_decay=weight_decay, max_norm=max_norm, extra=n_tail,
+        self.opt = ops.FlatAdam(params, lr=lr, weight_decay=weight_decay, max_norm=max_norm, extra=self.n_tail,
                                 grad_alloc=self.peer.alloc if self.peer is not None else None,
                                 param_storage=self.state.flat_param)
         self.state.index_params(self.model)
         self.optim_format = OptimizerStateFormat(self.model.named_parameters(), betas=self.opt.betas, eps=self.opt.eps,
                                                  weight_decay=weight_decay, max_norm=max_norm)
         self.schedule_steps = 0          # the step count the current learning rate was scheduled at
-        self.state_snap = torch.empty_like(self.state.bytes)
-        self.avg_bytes = self.avg = self.avg_snap = None       # moving average of the fp32 state: a copy of bytes [0, i_off)
+        # what a step or a validation pass changes and the capture's warm-up must leave as it was: _snapshot clones `_mutable`,
+        # _restore copies the clones back into the same tensors (the graphs bake their pointers) and zeroes `_zeroed`.
+        # StateStore's bytes and loose buffers hold every parameter and buffer, i.e. the model's whole state_dict
+        self._mutable = [self.state.bytes] + [b for _, b in self.state.loose] + \
+            [self.opt.exp_avg, self.opt.exp_avg_sq, self.opt.step_count]
+        self._zeroed = []
+        snap = torch.empty_like(self.state.bytes)
+        self.acc_snap = torch.zeros(n_sums, dtype=torch.float64, device=self.device)       # filled by epoch_schedule
+        self._handoff = [_Handoff('state', snap, [(snap, self.state.bytes)]), _Handoff('losses', self.acc_snap, [])]
+        self.avg_bytes = self.avg = None       # moving average of the fp32 state: a copy of bytes [0, i_off)
         self.avg_seeded = False
         if self.weight_ema is not None:
             self.avg_bytes = self.state.bytes[:self.state.i_off].clone()
             self.avg = self.avg_bytes.view(torch.float32)
-            self.avg_snap = torch.empty_like(self.avg_bytes)
-        # validation sums [live (NUM_LOSS) | averaged (NUM_LOSS)], the epoch hand-off's copy, and the state saved around a pass
-        self.val_accum_all = self.val_accum = self.val_ema_accum = self.val_snap = self.val_saved = None
+            self._mutable.append(self.avg)
+            snap = torch.empty_like(self.avg_bytes)     # on the host an image of `bytes`, which averaged_bytes completes
+            self._handoff.append(_Handoff('avg', snap, [(snap, self.avg_bytes)], room=self.state.bytes.numel()))
+        self.copy_stream = torch.cuda.Stream(device=self.device)
+        self._handoff_slots = None
+        self._handoff_i = 0
+        self._last_done = None
+        self._staging = None
+        self._staging_i = 0
+        self._captured = False
+        self.launches_per_step = 0
+        self.ema = torch.full((1,), float(example_batch['action'].shape[0] * args.get('forward_steps', 1)) * self.world,
+                              dtype=torch.float32, device=self.device)
+        self.optim_snap = None           # optimiser state of the epoch hand-off (_optim_views)
+        if self.save_optimizer:
+            self.optim_snap = self._optim_image(self.device)
+            self._handoff.append(_Handoff('optim', self.optim_snap, self._optim_copies(self.optim_snap)))
+        # validation sums [live (NUM_LOSS) | averaged (NUM_LOSS)] and the state saved around a pass
+        self.val_accum_all = self.val_accum = self.val_ema_accum = self.val_saved = None
         self.val_buf = None
         self.val_graphs = {}
         self.launches_per_validation = 0
@@ -792,21 +831,10 @@ class LearnerStep:
             self.val_accum = self.val_accum_all[:NUM_LOSS]
             if self.avg is not None:
                 self.val_ema_accum = self.val_accum_all[NUM_LOSS:]
-            self.val_snap = torch.zeros_like(self.val_accum_all)
+            self._zeroed.append(self.val_accum_all)
+            snap = torch.zeros_like(self.val_accum_all)
+            self._handoff.append(_Handoff('val', snap, [(snap, self.val_accum_all)], after=self.val_accum_all.zero_))
             self.val_saved = torch.empty_like(self.state.bytes)
-        self.acc_snap = torch.zeros(n_sums, dtype=torch.float64, device=self.device)
-        self.copy_stream = torch.cuda.Stream(device=self.device)
-        self._handoff_slots = None
-        self._handoff_i = 0
-        self._staging = None
-        self._staging_i = 0
-        self.launches_per_step = 0
-        self.ema = torch.full((1,), float(example_batch['action'].shape[0] * args.get('forward_steps', 1)) * self.world,
-                              dtype=torch.float32, device=self.device)
-        # optimiser state of the epoch hand-off: [exp_avg | exp_avg_sq (n_pad fp32 each) | step_count (int64) | lr | ema (fp32)]
-        self.optim_snap = None
-        if self.save_optimizer:
-            self.optim_snap = torch.empty(8 * self.opt.n_pad + 16, dtype=torch.uint8, device=self.device)
 
         self.layout = BatchLayout(example_batch)
         self.dev_buffer = torch.zeros(self.layout.nbytes, dtype=torch.uint8, device=self.device)
@@ -828,20 +856,24 @@ class LearnerStep:
         self.loss_buf = None
         self.last_losses = torch.zeros(NUM_LOSS, device=self.device)
         self.accum = torch.zeros(n_sums, dtype=torch.float64, device=self.device)
-        self.loss_accum = self.accum[:NUM_LOSS]
+        self._mutable.append(self.accum)
+        loss, diag, skipped = _accum_layout(diagnostics, self.skip_nonfinite)
+        self.loss_accum = self.accum[loss]
         self.diag_accum = None
         if diagnostics:
-            self.diag_accum = self.accum[NUM_LOSS:NUM_LOSS + NUM_DIAG]
+            self.diag_accum = self.accum[diag]
             self.opt.diag = self.diag_accum[NUM_LOSS_DIAG:]        # the optimiser's entries: accumulated by its own kernel
         # guard against non-finite steps: the count of rejected steps is the accumulator's last slot; the buffers the forward
         # moves (StateStore bytes [f_off, nbytes)) are saved at the start of every step and put back when it is rejected
         self.skipped = self.guard_saved = None
         if self.skip_nonfinite:
-            self.skipped = self.accum[n_sums - 1:]
+            self.skipped = self.accum[skipped]
             self.opt.skip = torch.zeros(1, dtype=torch.int32, device=self.device)
             self.opt.guard_tail = NUM_LOSS
+            self._mutable.append(self.opt.skip)
             if self.state.nbytes > self.state.f_off:
                 self.guard_saved = torch.empty(self.state.nbytes - self.state.f_off, dtype=torch.uint8, device=self.device)
+                self._mutable.append(self.guard_saved)
         self.host_slots = torch.zeros((8, NUM_LOSS)).pin_memory()
         self._slot = 0
         self.graph = self.graph_fwd = self.graph_bwd = None
@@ -905,7 +937,7 @@ class LearnerStep:
                 torch.autograd.backward(heads, grads)
         self.opt.extra_slots[:NUM_LOSS].copy_(buf.losses)     # the loss sums ride the gradient bucket
         if self.diagnostics:
-            self.opt.extra_slots[NUM_LOSS:NUM_LOSS + NUM_LOSS_DIAG].copy_(buf.diagnostics[:NUM_LOSS_DIAG])
+            self.opt.extra_slots[_LOSS_DIAG].copy_(buf.diagnostics[:NUM_LOSS_DIAG])
         if self.peer is not None:
             reduced = self.peer(self.opt.n_pad, self.opt.partials)      # all-reduce + norm partials, one kernel
             self.opt.step_reduced(reduced)
@@ -918,13 +950,12 @@ class LearnerStep:
             tail = self.opt.extra_slots
             self.last_losses.copy_(tail[:NUM_LOSS])
         if self.skip_nonfinite:         # one launch: accumulate an accepted step, or count a rejected one and restore its buffers
-            n_tail = NUM_LOSS + (NUM_LOSS_DIAG if self.diagnostics else 0)
-            ops.step_commit(self.opt.skip, tail[:n_tail], self.accum, self.skipped,
+            ops.step_commit(self.opt.skip, tail[:self.n_tail], self.accum, self.skipped,
                             self._guarded_buffers() if self.guard_saved is not None else None, self.guard_saved)
         else:
             self.loss_accum.add_(self.last_losses)
             if self.diagnostics:
-                self.diag_accum[:NUM_LOSS_DIAG].add_(tail[NUM_LOSS:NUM_LOSS + NUM_LOSS_DIAG])
+                self.accum[_LOSS_DIAG].add_(tail[_LOSS_DIAG])
         if self.avg is not None:        # after the optimiser: step_count already counts this step
             ops.weight_ema_update(self.avg, self.state.bytes[:self.state.i_off].view(torch.float32), self.opt.step_count,
                                   self.weight_ema, self.avg_seeded, skip=self.opt.skip)
@@ -1016,37 +1047,21 @@ class LearnerStep:
             self.val_graphs[averaged] = g
 
     def _snapshot(self):
-        bufs = {k: v.clone() for k, v in self.model.state_dict().items()}
-        guard = None
-        if self.skip_nonfinite:         # (the skip count rides in accum)
-            guard = (self.opt.skip.clone(), self.guard_saved.clone() if self.guard_saved is not None else None)
-        return (bufs, self.opt.exp_avg.clone(), self.opt.exp_avg_sq.clone(), self.opt.step_count.clone(),
-                self.accum.clone(), self.avg.clone() if self.avg is not None else None, guard)
+        return [t.clone() for t in self._mutable]
 
-    def _restore(self, state):
-        if self.val_accum_all is not None:
-            self.val_accum_all.zero_()
-        bufs, m, v, sc, acc, avg, guard = state
-        with torch.no_grad():
-            for k, t in self.model.state_dict().items():
-                t.copy_(bufs[k])
-            self.opt.exp_avg.copy_(m)
-            self.opt.exp_avg_sq.copy_(v)
-            self.opt.step_count.copy_(sc)
-            self.accum.copy_(acc)
-            if avg is not None:
-                self.avg.copy_(avg)
-            if guard is not None:
-                self.opt.skip.copy_(guard[0])
-                if guard[1] is not None:
-                    self.guard_saved.copy_(guard[1])
+    def _restore(self, saved):
+        """Put back what _snapshot saved, into the same tensors, and zero the sums of the warm-up's validation passes."""
+        for t, s in zip(self._mutable, saved):
+            t.copy_(s)
+        for t in self._zeroed:
+            t.zero_()
 
     def new_packed(self):
         return PackedBatch(self.layout)
 
     def warm_up(self):
         """Run the warm-up steps and capture the graphs now (otherwise done lazily by the first step)."""
-        if not getattr(self, '_captured', False):
+        if not self._captured:
             self._capture()
 
     def step(self, packed):
@@ -1063,7 +1078,7 @@ class LearnerStep:
         self._enqueue(dev_bytes, None)
 
     def _enqueue(self, src_bytes, packed):
-        if not getattr(self, '_captured', False):
+        if not self._captured:
             self._capture()
         if packed is not None:
             # host batch: the H2D copy runs on the copy stream into one of two staging buffers, i.e. while the previous
@@ -1113,7 +1128,7 @@ class LearnerStep:
             raise RuntimeError('LearnerStep was built without validation (train_args["validation_rate"] / validation=True)')
         if averaged:
             self._require_average()
-        if not getattr(self, '_captured', False):
+        if not self._captured:
             self._capture()
         with torch.cuda.stream(self.stream):
             if self.use_graph:
@@ -1214,16 +1229,16 @@ class LearnerStep:
         and the buffers StateStore keeps outside its allocation are the live model's."""
         self._require_average()
         self.stream.synchronize()
-        host = self.state.bytes.cpu()
-        host[:self.state.i_off] = self.avg_bytes.cpu()
-        return self._state_dict_of(host)
+        host_avg = torch.empty_like(self.state.bytes, device='cpu')       # as end_epoch hands it over: an image of `bytes`
+        host_avg[:self.state.i_off] = self.avg_bytes.cpu()
+        return self._state_dict_of(self.state.averaged_bytes(host_avg, self.state.bytes.cpu()))
 
     def seed_weight_ema(self, state_dict):
         """Start the average from a saved one (a CPU state_dict keyed like the model's, e.g. a <epoch>.ema.pth file): its fp32
         entries replace the average, and every later step weighs the live weights with 1 - decay.  Call it before the first
         step (or warm_up), which fixes the captured launch."""
         self._require_average()
-        if getattr(self, '_captured', False):
+        if self._captured:
             raise RuntimeError('seed_weight_ema must come before the first step / warm_up()')
         store = self.state
         views = {'p': self.avg[:store.n_pad], 'f': self.avg[store.f_off // 4:]}
@@ -1242,10 +1257,19 @@ class LearnerStep:
         self.avg_seeded = True
 
     def _optim_views(self, buf):
-        """(exp_avg, exp_avg_sq, step_count, lr, ema) views of a byte buffer in the optim_snap layout."""
+        """(exp_avg, exp_avg_sq, step_count, lr, ema) views of a byte buffer in the optim_snap layout:
+        [exp_avg | exp_avg_sq (n_pad fp32 each) | step_count (int64) | lr | ema (fp32)]."""
         n4 = 4 * self.opt.n_pad
         return (buf[:n4].view(torch.float32), buf[n4:2 * n4].view(torch.float32), buf[2 * n4:2 * n4 + 8].view(torch.int64),
                 buf[2 * n4 + 8:2 * n4 + 12].view(torch.float32), buf[2 * n4 + 12:2 * n4 + 16].view(torch.float32))
+
+    def _optim_image(self, device):
+        return torch.empty(8 * self.opt.n_pad + 16, dtype=torch.uint8, device=device)
+
+    def _optim_copies(self, image):
+        """The (view of image, live tensor) copies that fill a buffer in the optim_snap layout."""
+        return list(zip(self._optim_views(image),
+                        (self.opt.exp_avg, self.opt.exp_avg_sq, self.opt.step_count, self.opt.lr, self.ema)))
 
     def optimizer_state_from(self, host_optim, steps):
         """The OptimizerStateFormat dict of a host copy of optim_snap, scheduled at step count `steps`."""
@@ -1256,15 +1280,17 @@ class LearnerStep:
         """Blocking copy of the optimiser state the next step uses, in the OptimizerStateFormat dict (what end_epoch hands
         over as PendingModel.optim_state)."""
         self.stream.synchronize()
-        return self.optim_format.to_dict(self.opt.exp_avg.cpu(), self.opt.exp_avg_sq.cpu(), int(self.opt.step_count.item()),
-                                         float(self.opt.lr.item()), float(self.ema.item()), self.schedule_steps)
+        image = self._optim_image('cpu')
+        for dst, src in self._optim_copies(image):
+            dst.copy_(src)
+        return self.optimizer_state_from(image, self.schedule_steps)
 
     def load_optimizer_state(self, d):
         """Resume from an OptimizerStateFormat dict (e.g. a <epoch>.optim.pth file): Adam's moments and step count, the
         learning rate and the data-count average.  Call it before the first step (or warm_up), which snapshots the state
         around the capture's warm-up steps.  A dict whose parameter names or shapes differ from the net's, or whose betas,
         eps, weight_decay or max_norm differ from this learner's, raises KeyError / ValueError and changes nothing."""
-        if getattr(self, '_captured', False):
+        if self._captured:
             raise RuntimeError('load_optimizer_state must come before the first step / warm_up()')
         m, v, step, lr, data_cnt_ema, steps = self.optim_format.unpack(d)
         with torch.no_grad():
@@ -1296,48 +1322,30 @@ class LearnerStep:
         state, when they are kept, snapshot and copied the same way; the optimiser state is taken after the schedule, i.e.
         as the next step uses it)."""
         if self._handoff_slots is None:
-            self._handoff_slots = [(torch.empty(self.state.bytes.numel(), dtype=torch.uint8).pin_memory(),
-                                    torch.zeros(self.acc_snap.numel(), dtype=torch.float64).pin_memory(),
-                                    torch.empty(self.state.bytes.numel(), dtype=torch.uint8).pin_memory()
-                                    if self.avg is not None else None,
-                                    torch.empty(self.optim_snap.numel(), dtype=torch.uint8).pin_memory()
-                                    if self.optim_snap is not None else None,
-                                    torch.zeros(self.val_snap.numel(), dtype=torch.float64).pin_memory()
-                                    if self.val_snap is not None else None) for _ in range(2)]
-        host_state, host_losses, host_avg, host_optim, host_val = self._handoff_slots[self._handoff_i % 2]
+            self._handoff_slots = [{e.name: torch.empty(e.room or e.snap.numel(), dtype=e.snap.dtype).pin_memory()
+                                    for e in self._handoff} for _ in range(2)]
+        host = self._handoff_slots[self._handoff_i % 2]
         self._handoff_i += 1
         with torch.cuda.stream(self.stream):
             self.epoch_schedule(batch_cnt, steps, default_lr)
-            if getattr(self, '_last_done', None) is not None:
+            if self._last_done is not None:
                 self.stream.wait_event(self._last_done)          # the previous snapshot has left the device buffer
-            self.state_snap.copy_(self.state.bytes)
-            if self.avg is not None:
-                self.avg_snap.copy_(self.avg_bytes)
-            if self.optim_snap is not None:
-                for dst, src in zip(self._optim_views(self.optim_snap),
-                                    (self.opt.exp_avg, self.opt.exp_avg_sq, self.opt.step_count, self.opt.lr, self.ema)):
+            for e in self._handoff:
+                for dst, src in e.copies:
                     dst.copy_(src)
-            if self.val_snap is not None:
-                self.val_snap.copy_(self.val_accum_all)
-                self.val_accum_all.zero_()
+                if e.after:
+                    e.after()
             ready = torch.cuda.Event()
             ready.record(self.stream)
         with torch.cuda.stream(self.copy_stream):
             self.copy_stream.wait_event(ready)
-            host_state.copy_(self.state_snap, non_blocking=True)
-            host_losses.copy_(self.acc_snap, non_blocking=True)
-            if self.avg is not None:
-                host_avg[:self.state.i_off].copy_(self.avg_snap, non_blocking=True)
-            if self.optim_snap is not None:
-                host_optim.copy_(self.optim_snap, non_blocking=True)
-            if self.val_snap is not None:
-                host_val.copy_(self.val_snap, non_blocking=True)
+            for e in self._handoff:
+                host[e.name][:e.snap.numel()].copy_(e.snap, non_blocking=True)
             done = torch.cuda.Event()
             done.record(self.copy_stream)
         self._last_done = done
-        return PendingModel(self, done, host_state, host_losses, heads, template, host_avg=host_avg, host_optim=host_optim,
-                            steps=int(steps), host_val=host_val, diagnostics=self.diagnostics,
-                            skip_nonfinite=self.skip_nonfinite, batch_cnt=batch_cnt)
+        return PendingModel(self, done, host['state'], host['losses'], heads, template, host=host, steps=int(steps),
+                            diagnostics=self.diagnostics, skip_nonfinite=self.skip_nonfinite, batch_cnt=batch_cnt)
 
 
 # --------------------------------------------------------------------------- batcher + trainer
