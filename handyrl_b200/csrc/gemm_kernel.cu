@@ -41,7 +41,6 @@ constexpr int kMaxN = 288;          // columns of one CTA tile (shared memory: 2
 constexpr int kChunkK = 32;         // reduction elements per shared-memory stage
 constexpr int kStages = 2;
 constexpr int kItemsA = kTileM * 8 / kGemmThreads;
-constexpr int kAcc = kMaxN / 4;     // accumulators per thread: a warpgroup holds 64 rows x kMaxN / 2 columns
 
 constexpr int kMaxSegments = 64;     // (dy, x) pairs of one segmented weight-gradient product
 
@@ -118,246 +117,183 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int PENDING>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
 
-// the last wait names every accumulator, so that no read of them is scheduled before it
-__device__ __forceinline__ void wgmma_wait_all(float (&d)[kAcc]) {
-    asm volatile("wgmma.wait_group.sync.aligned 0;"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 :
-                 : "memory");
+// the last wait: every accumulator passes through an empty asm after it, so that no read of them is scheduled before it
+template <int NACC>
+__device__ __forceinline__ void wgmma_wait_all(float (&d)[NACC]) {
+    wgmma_wait<0>();
+#pragma unroll
+    for (int i = 0; i < NACC; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
 
 // D[64 x N] += A[64 x 8] * B[N x 8]^T, both operands in shared memory (tf32, K-major).  The instruction shape is part of
-// the opcode: one specialisation per width; every one names all kAcc accumulators so that they stay in fixed registers.
+// the opcode: one specialisation per width, each naming exactly its N / 2 accumulators a thread.
 template <int N>
-__device__ __forceinline__ void wgmma_tf32(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc);
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t a_desc, uint64_t b_desc);
 template <>
-__device__ __forceinline__ void wgmma_tf32<8>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32 {%0, %1, %2, %3}, %72, %73, p, 1, 1;\n\t}"
+__device__ __forceinline__ void wgmma_tf32<8>(float (&d)[4], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n8k8.f32.tf32.tf32 {%0, %1, %2, %3}, %4, %5, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<16>(float (&d)[8], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<24>(float (&d)[12], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %14, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n24k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11}, %12, %13, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<40>(float (&d)[20], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %22, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n40k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, %20, %21, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<48>(float (&d)[24], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<56>(float (&d)[28], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %30, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n56k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27}, %28, %29, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<72>(float (&d)[36], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %38, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n72k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35}, %36, %37, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<80>(float (&d)[40], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n80k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<88>(float (&d)[44], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %46, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n88k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43}, %44, %45, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<96>(float (&d)[48], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %48, %49, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<104>(float (&d)[52], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %54, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n104k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51}, %52, %53, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<112>(float (&d)[56], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %58, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n112k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %56, %57, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<120>(float (&d)[60], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %62, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n120k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59}, %60, %61, p, 1, 1;\n\t}"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
+                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
+                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59])
+                 : "l"(a_desc), "l"(b_desc), "r"(1)
+                 : "memory");
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t a_desc, uint64_t b_desc) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
                    "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
                    "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
                    "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
                    "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
+                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
                  : "l"(a_desc), "l"(b_desc), "r"(1)
                  : "memory");
 }
 template <>
-__device__ __forceinline__ void wgmma_tf32<16>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<24>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n24k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<32>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<40>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n40k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<48>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<56>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n56k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<64>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<72>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n72k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<80>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n80k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<88>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n88k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<96>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<104>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n104k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<112>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n112k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<120>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n120k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<128>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<136>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n136k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67}, %72, %73, p, 1, 1;\n\t}"
-                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
-                   "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-                   "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]),
-                   "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-                   "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
-                   "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "l"(a_desc), "l"(b_desc), "r"(1)
-                 : "memory");
-}
-template <>
-__device__ __forceinline__ void wgmma_tf32<144>(float (&d)[kAcc], uint64_t a_desc, uint64_t b_desc) {
+__device__ __forceinline__ void wgmma_tf32<144>(float (&d)[72], uint64_t a_desc, uint64_t b_desc) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %74, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n144k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71}, %72, %73, p, 1, 1;\n\t}"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
@@ -370,37 +306,16 @@ __device__ __forceinline__ void wgmma_tf32<144>(float (&d)[kAcc], uint64_t a_des
                  : "memory");
 }
 
-// one stage of the 3xTF32 product for this warpgroup's quarter of the tile: small terms first, a_lo*b_hi + a_hi*b_lo + a_hi*b_hi
+// one stage of the 3xTF32 product for this warpgroup's quarter of the tile: small terms first, a_lo*b_hi + a_hi*b_lo + a_hi*b_hi.
+// The width is a compile-time constant of the kernel: with a runtime choice between widths ptxas cannot keep the
+// accumulators in fixed registers across the cases and serialises the chain with injected warpgroup.arrive (C7519).
 template <int N>
-__device__ __forceinline__ void mma_stage(float (&d)[kAcc], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
+__device__ __forceinline__ void mma_stage(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
 #pragma unroll
     for (int ks = 0; ks < kChunkK / 8; ks++) {
         wgmma_tf32<N>(d, wgmma_desc(a_lo + 32 * ks), wgmma_desc(b_hi + 32 * ks));
         wgmma_tf32<N>(d, wgmma_desc(a_hi + 32 * ks), wgmma_desc(b_lo + 32 * ks));
         wgmma_tf32<N>(d, wgmma_desc(a_hi + 32 * ks), wgmma_desc(b_hi + 32 * ks));
-    }
-}
-
-__device__ __forceinline__ void mma_stage_n(int n, float (&d)[kAcc], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo) {
-    switch (n) {
-    case 8: mma_stage<8>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 16: mma_stage<16>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 24: mma_stage<24>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 32: mma_stage<32>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 40: mma_stage<40>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 48: mma_stage<48>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 56: mma_stage<56>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 64: mma_stage<64>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 72: mma_stage<72>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 80: mma_stage<80>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 88: mma_stage<88>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 96: mma_stage<96>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 104: mma_stage<104>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 112: mma_stage<112>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 120: mma_stage<120>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 128: mma_stage<128>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 136: mma_stage<136>(d, a_hi, a_lo, b_hi, b_lo); break;
-    case 144: mma_stage<144>(d, a_hi, a_lo, b_hi, b_lo); break;
     }
 }
 
@@ -417,11 +332,11 @@ __device__ __forceinline__ void split_tf32(const float4 v, float4 &hi, float4 &l
 
 // ---- operand loaders.  Every thread owns a fixed set of "items" (one row x 4 consecutive reduction elements = one 16-byte
 // shared-memory slot per split half, K-major SWIZZLE_128B: a row's chunk = 128 bytes, slot j of row r at j ^ (r & 7)); their
-// coordinates are computed once, each chunk only advances the pointers.
+// coordinates follow from the thread index (the kernel derives them again in every chunk), each chunk advances the pointers.
 // (An operand stored [K][rows] is transposed by the loads -- 4 scalar loads per item, coalesced along the rows: wgmma takes
 //  tf32 operands K-major only.)
-// Item (B operand): 32-bit offsets and row0 + row in 22 bits of meta -- the host bounds N and b.ld below 2^22.
-// ItemA (A operand): 64-bit offsets (any ld) and the row inside the tile (< 128); the tile's first row is added by the caller.
+// Item (B operand): 32-bit offsets -- the host bounds b.ld below 2^22.  ItemA (A operand): 64-bit offsets (any ld).
+// The row is the row inside the tile (< 288); the tile's first row is added by the caller.
 template <typename Off>
 struct ItemT {             // three (B) or four (A) registers per item (a thread holds up to 5 B and 2 A items)
     Off off;               // first of the 4 elements in chunk 0, relative to the tile's first element
@@ -435,7 +350,7 @@ using Item = ItemT<int>;
 using ItemA = ItemT<long long>;
 
 template <bool KMAJOR, typename It = Item>
-__device__ __forceinline__ It make_item(int i, int n_items, long long ld, int rows_pad, int rows, int row0) {
+__device__ __forceinline__ It make_item(int i, int n_items, long long ld, int rows_pad, int rows) {
     It it;
     int row, j;
     if (KMAJOR) {           // 8 consecutive lanes = the 128 contiguous bytes of one row's chunk: one cache line per quarter
@@ -446,7 +361,7 @@ __device__ __forceinline__ It make_item(int i, int n_items, long long ld, int ro
         row = i - j * rows_pad;
     }
     const bool live = i < n_items && row < rows;
-    it.meta = (uint32_t)(4 * j) | ((live ? 1u : 0u) << 9) | ((uint32_t)(row0 + row) << 10);
+    it.meta = (uint32_t)(4 * j) | ((live ? 1u : 0u) << 9) | ((uint32_t)row << 10);
     it.slot = (uint32_t)row * 128u + (uint32_t)((j ^ (row & 7)) << 4);
     it.off = (decltype(it.off))(KMAJOR ? (long long)row * ld + 4 * j : (long long)(4 * j) * ld + row);
     if (i >= n_items) it.slot = 0xFFFFFFFFu;
@@ -541,13 +456,20 @@ __device__ __forceinline__ float4 transform_item(const GemmOperand &op, const It
 
 // A and B go global -> registers -> (transform, hi/lo split) -> shared memory; a packed B image arrives by one bulk copy a
 // stage.  Each thread owns kItemsA items of the A tile (coalesced: 8 consecutive lanes = the 128 bytes of one k-major row,
-// or consecutive rows of a transposed one) and ITEMS_B items of the B tile.
-template <bool A_K, bool B_K, int ITEMS_B, bool PACKED>
-__global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const GemmParams p, const int n_pad) {
+// or consecutive rows of a transposed one) and ITEMS_B items of the B tile.  NW = the MMA width of a warpgroup = half the
+// tile's padded column count n_pad (one instantiation per width the host dispatches).
+template <bool A_K, bool B_K, bool PACKED, int NW>
+__global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const GemmParams p) {
+    constexpr int n_pad = 2 * NW, nw = NW;
+    constexpr int ITEMS_B = PACKED ? 1 : (n_pad * 8 + kGemmThreads - 1) / kGemmThreads;
+    // B items loaded ahead of the stage barrier; the rest of the 5 items of the widest tiles are loaded after it, so that
+    // at most 3 B float4s (plus the A items) are in flight next to the 72 accumulators
+    constexpr int kItemsB1 = ITEMS_B < 3 ? ITEMS_B : 3;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);      // swizzle atoms need 1024-byte alignment
     __shared__ __align__(8) uint64_t bars[kStages];     // packed B: the stage's bulk copy has landed
     __shared__ float b_consts[2][kMaxN];     // per-row constants of a single-source B transform (no registers, no per-chunk loads)
+    __shared__ float a_consts[3][kTileM];    // the same for A (one or two sources): p, q, r of the tile's rows
     __shared__ short conv_off_s[kConvMaxTable];
     __shared__ int conv_src_s[2][kChunkK * 9];      // conv_mode 2: source pixel of (pixel of the chunk, tap), two chunks in flight
 
@@ -584,6 +506,16 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
             b_consts[1][i] = in ? __ldg(p.b.r + n0 + i) : 0.f;
         }
     }
+    // per-row constants of the A transform (the weight gradient's BatchNorm-backward operand)
+    const bool a_rows = p.a.p != nullptr && p.a.feature_is_row;
+    if (a_rows) {
+        for (int i = tid; i < kTileM; i += kGemmThreads) {
+            const bool in = i < rows_a;
+            a_consts[0][i] = in ? __ldg(p.a.p + m0 + i) : 1.f;
+            a_consts[1][i] = in && p.a.q ? __ldg(p.a.q + m0 + i) : 0.f;
+            a_consts[2][i] = in ? __ldg(p.a.r + m0 + i) : 0.f;
+        }
+    }
     __syncthreads();
 
     // ---- A items.  conv_mode 1: the row is a pixel, the chunk belongs to one kernel tap -> the source is the tap's neighbour
@@ -591,12 +523,19 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
     const long long a2 = p.a.ptr2 ? (p.a.ptr2 - p.a.ptr) : 0;
     const bool vec_a = A_K && (p.a.ld % 4 == 0) && ((reinterpret_cast<uintptr_t>(a_base) & 15) == 0) &&
                        (!p.a.ptr2 || (reinterpret_cast<uintptr_t>(p.a.ptr2) & 15) == 0);
-    ItemA ia[kItemsA];
-    int conv_pos[kItemsA];
+    // The items' coordinates are derived from the thread index again in every chunk (a few integer operations; `t` passes
+    // through an empty asm so that the compiler cannot hoist them out of the loop): held across the loop they would take
+    // 3-4 registers an item, and the instantiations with 5 B items and 72 accumulators would spill.
+    auto items_a = [&](int t, ItemA (&ia)[kItemsA]) {
 #pragma unroll
-    for (int u = 0; u < kItemsA; u++) {
-        ia[u] = make_item<A_K, ItemA>(tid + u * kGemmThreads, kTileM * 8, p.a.ld, kTileM, rows_a, 0);
-        conv_pos[u] = p.conv_mode == 1 ? (int)(((long long)m0 + ia[u].row()) % p.conv_hw) : 0;
+        for (int u = 0; u < kItemsA; u++) ia[u] = make_item<A_K, ItemA>(t + u * kGemmThreads, kTileM * 8, p.a.ld, kTileM, rows_a);
+    };
+    int conv_pos[kItemsA];
+    {
+        ItemA ia[kItemsA];
+        items_a(tid, ia);
+#pragma unroll
+        for (int u = 0; u < kItemsA; u++) conv_pos[u] = A_K && p.conv_mode == 1 ? (int)(((long long)m0 + ia[u].row()) % p.conv_hw) : 0;
     }
 
     // ---- B items
@@ -605,21 +544,22 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
     const long long b2 = p.b.ptr2 ? (p.b.ptr2 - p.b.ptr) : 0;
     const bool vec_b = B_K && (p.b.ld % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.b.ptr) & 15) == 0) &&
                        (!p.b.ptr2 || (reinterpret_cast<uintptr_t>(p.b.ptr2) & 15) == 0);
-    Item ib[ITEMS_B];
+    auto items_b = [&](int t, Item (&ib)[ITEMS_B]) {
 #pragma unroll
-    for (int u = 0; u < ITEMS_B; u++) {
-        ib[u] = make_item<B_K>(tid + u * kGemmThreads, n_pad * 8, p.b.ld, n_pad, n_here, n0);
-        if (!PACKED && !B_K && p.conv_mode == 2) {          // row n -> (tap, channel)
-            const int n = ib[u].row(), tap = n / p.conv_cin;
-            ib[u].off = (n - tap * p.conv_cin) | (tap << 16);
+        for (int u = 0; u < ITEMS_B; u++) {
+            ib[u] = make_item<B_K>(t + u * kGemmThreads, n_pad * 8, p.b.ld, n_pad, n_here);
+            if (!PACKED && !B_K && p.conv_mode == 2) {          // row n -> (tap, channel)
+                const int n = n0 + ib[u].row(), tap = n / p.conv_cin;
+                ib[u].off = (n - tap * p.conv_cin) | (tap << 16);
+            }
         }
-    }
+    };
 
     // ---- this warpgroup's quarter of the tile: rows 64 (wg & 1) ..., columns nw (wg >> 1) ...
-    const int wg = warp >> 2, nw = n_pad / 2;
-    float acc[kAcc];
+    const int wg = warp >> 2;
+    float acc[NW / 2];
 #pragma unroll
-    for (int i = 0; i < kAcc; i++) acc[i] = 0.f;
+    for (int i = 0; i < NW / 2; i++) acc[i] = 0.f;
 
     for (int c = c_begin; c < c_end; c++) {
         const int it = c - c_begin, s = it % kStages;
@@ -636,10 +576,59 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
             }
             asm volatile("bar.sync 1, %0;" ::"n"(kGemmThreads) : "memory");
         }
+        int t = tid;
+        asm volatile("" : "+r"(t));
+        ItemA ia[kItemsA];
+        Item ib[ITEMS_B];
+        items_a(t, ia);
+        items_b(t, ib);
         float4 va[kItemsA], vb[ITEMS_B];
+        // B items [u0, u1): global -> registers, transform
+        auto load_b = [&](int u0, int u1) {
+#pragma unroll
+            for (int u = u0; u < u1; u++)
+                vb[u] = (!B_K && p.conv_mode == 2) ? load_item_conv(ib[u], b_base, p.b.ld, k0, p, conv_src_s[it & 1])
+                                                   : load_item<B_K>(ib[u], Bg, p.b.ld, vec_b, adv_b, k_left);
+            if (b_rows) {
+#pragma unroll
+                for (int u = u0; u < u1; u++) {
+                    if (!ib[u].live()) continue;
+                    const float pc = b_consts[0][ib[u].row()], rc = b_consts[1][ib[u].row()];
+                    float4 v;
+                    v.x = fmaf(vb[u].x, pc, rc); v.y = fmaf(vb[u].y, pc, rc); v.z = fmaf(vb[u].z, pc, rc); v.w = fmaf(vb[u].w, pc, rc);
+                    if (p.b.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+                    if (k_left < kChunkK) {                  // the reduction tail stays exactly zero
+                        const int k = ib[u].k();
+                        if (k + 0 >= k_left) v.x = 0.f;
+                        if (k + 1 >= k_left) v.y = 0.f;
+                        if (k + 2 >= k_left) v.z = 0.f;
+                        if (k + 3 >= k_left) v.w = 0.f;
+                    }
+                    vb[u] = v;
+                }
+            } else if (p.b.p != nullptr) {
+#pragma unroll
+                for (int u = u0; u < u1; u++) {
+                    const float4 y = p.b.ptr2 ? load_item<B_K>(ib[u], Bg, p.b.ld, vec_b, adv_b + b2, k_left) : make_float4(0.f, 0.f, 0.f, 0.f);
+                    vb[u] = transform_item(p.b, ib[u], vb[u], y, k0, k_left, n0);
+                }
+            }
+        };
+        // B items [u0, u1): hi/lo split -> shared memory
+        auto store_b = [&](uint8_t *stp, int u0, int u1) {
+#pragma unroll
+            for (int u = u0; u < u1; u++) {
+                if (ib[u].slot != 0xFFFFFFFFu) {
+                    float4 h4, l4;
+                    split_tf32(vb[u], h4, l4);
+                    *reinterpret_cast<float4 *>(stp + ib[u].slot) = h4;
+                    *reinterpret_cast<float4 *>(stp + b_bytes + ib[u].slot) = l4;
+                }
+            }
+        };
         if ((p.debug & 3) != 2) {
             // all the loads first (one exposed latency per chunk, not one per item), then the transforms
-            if (p.conv_mode == 1) {
+            if (A_K && p.conv_mode == 1) {          // (the host requires a k-major A for convolutions)
                 const int tap = c / p.conv_cpt, ch0 = (c - tap * p.conv_cpt) * kChunkK;      // first channel of the chunk
 #pragma unroll
                 for (int u = 0; u < kItemsA; u++) {
@@ -651,7 +640,29 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
                 const long long adv_a = A_K ? (long long)k0 : (long long)k0 * p.a.ld;
 #pragma unroll
                 for (int u = 0; u < kItemsA; u++) va[u] = load_item<A_K>(ia[u], Ag, p.a.ld, vec_a, adv_a, k_left);
-                if (p.a.p != nullptr) {
+                if (a_rows) {
+#pragma unroll
+                    for (int u = 0; u < kItemsA; u++) {
+                        const float4 y = p.a.ptr2 ? load_item<A_K>(ia[u], Ag, p.a.ld, vec_a, adv_a + a2, k_left) : make_float4(0.f, 0.f, 0.f, 0.f);
+                        if (!ia[u].live()) continue;
+                        const int r = ia[u].row();
+                        const float pc = a_consts[0][r], qc = a_consts[1][r], rc = a_consts[2][r];
+                        float4 v;
+                        v.x = fmaf(va[u].x, pc, fmaf(y.x, qc, rc));
+                        v.y = fmaf(va[u].y, pc, fmaf(y.y, qc, rc));
+                        v.z = fmaf(va[u].z, pc, fmaf(y.z, qc, rc));
+                        v.w = fmaf(va[u].w, pc, fmaf(y.w, qc, rc));
+                        if (p.a.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
+                        if (k_left < kChunkK) {                  // the reduction tail stays exactly zero
+                            const int k = ia[u].k();
+                            if (k + 0 >= k_left) v.x = 0.f;
+                            if (k + 1 >= k_left) v.y = 0.f;
+                            if (k + 2 >= k_left) v.z = 0.f;
+                            if (k + 3 >= k_left) v.w = 0.f;
+                        }
+                        va[u] = v;
+                    }
+                } else if (p.a.p != nullptr) {
 #pragma unroll
                     for (int u = 0; u < kItemsA; u++) {
                         const float4 y = p.a.ptr2 ? load_item<A_K>(ia[u], Ag, p.a.ld, vec_a, adv_a + a2, k_left) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -659,36 +670,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
                     }
                 }
             }
-            if (!PACKED) {
-#pragma unroll
-                for (int u = 0; u < ITEMS_B; u++)
-                    vb[u] = (!B_K && p.conv_mode == 2) ? load_item_conv(ib[u], b_base, p.b.ld, k0, p, conv_src_s[it & 1])
-                                                       : load_item<B_K>(ib[u], Bg, p.b.ld, vec_b, adv_b, k_left);
-                if (b_rows) {
-#pragma unroll
-                    for (int u = 0; u < ITEMS_B; u++) {
-                        if (!ib[u].live()) continue;
-                        const float pc = b_consts[0][ib[u].row() - n0], rc = b_consts[1][ib[u].row() - n0];
-                        float4 v;
-                        v.x = fmaf(vb[u].x, pc, rc); v.y = fmaf(vb[u].y, pc, rc); v.z = fmaf(vb[u].z, pc, rc); v.w = fmaf(vb[u].w, pc, rc);
-                        if (p.b.relu) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f); }
-                        if (k_left < kChunkK) {                  // the reduction tail stays exactly zero
-                            const int k = ib[u].k();
-                            if (k + 0 >= k_left) v.x = 0.f;
-                            if (k + 1 >= k_left) v.y = 0.f;
-                            if (k + 2 >= k_left) v.z = 0.f;
-                            if (k + 3 >= k_left) v.w = 0.f;
-                        }
-                        vb[u] = v;
-                    }
-                } else if (p.b.p != nullptr) {
-#pragma unroll
-                    for (int u = 0; u < ITEMS_B; u++) {
-                        const float4 y = p.b.ptr2 ? load_item<B_K>(ib[u], Bg, p.b.ld, vec_b, adv_b + b2, k_left) : make_float4(0.f, 0.f, 0.f, 0.f);
-                        vb[u] = transform_item(p.b, ib[u], vb[u], y, k0, k_left, 0);
-                    }
-                }
-            }
+            if (!PACKED) load_b(0, kItemsB1);
         }
         // the stage is free once every warpgroup's products of chunk it - kStages have completed
         wgmma_wait<kStages - 1>();
@@ -703,6 +685,9 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
                          : "memory");
         }
         if ((p.debug & 3) != 2) {
+            asm volatile("" : "+r"(t));           // the slots again: cheaper than holding them across the barrier
+            items_a(t, ia);
+            items_b(t, ib);
 #pragma unroll
             for (int u = 0; u < kItemsA; u++) {
                 if (ia[u].slot != 0xFFFFFFFFu) {
@@ -713,15 +698,9 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
                 }
             }
             if (!PACKED) {
-#pragma unroll
-                for (int u = 0; u < ITEMS_B; u++) {
-                    if (ib[u].slot != 0xFFFFFFFFu) {
-                        float4 h4, l4;
-                        split_tf32(vb[u], h4, l4);
-                        *reinterpret_cast<float4 *>(stp + ib[u].slot) = h4;
-                        *reinterpret_cast<float4 *>(stp + b_bytes + ib[u].slot) = l4;
-                    }
-                }
+                store_b(stp, 0, kItemsB1);
+                load_b(kItemsB1, ITEMS_B);          // the second pass of the widest tiles (while the previous chunk's MMAs run)
+                store_b(stp, kItemsB1, ITEMS_B);
             }
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy stores -> visible to the tensor core
@@ -731,7 +710,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
             const uint32_t st = smem_base + s * stage_bytes;
             const uint32_t a_hi = st + 2 * b_bytes + (uint32_t)(wg & 1) * 64 * 128, b_hi = st + (uint32_t)(wg >> 1) * nw * 128;
             wgmma_fence();
-            mma_stage_n(nw, acc, a_hi, a_hi + a_bytes, b_hi, b_hi + b_bytes);
+            mma_stage<NW>(acc, a_hi, a_hi + a_bytes, b_hi, b_hi + b_bytes);
             wgmma_commit();
         }
     }
@@ -779,8 +758,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tf32x3_kernel(const Gemm
         const int r0 = (wg & 1) * 64 + (warp & 3) * 16 + (lane >> 2);
         const int cb = (wg >> 1) * nw + 2 * (lane & 3);
 #pragma unroll
-        for (int j = 0; j < kAcc / 4; j++) {
-            if (8 * j >= nw) break;
+        for (int j = 0; j < NW / 8; j++) {
             const int col = cb + 8 * j;
             float b0 = 0.f, b1 = 0.f;
             if (p.bias != nullptr) {
@@ -877,6 +855,24 @@ __global__ void sum_partials_kernel(const float *__restrict__ partials, int spli
         for (int k = 1; k < splits; k++) s += partials[(long long)k * stride + i];
         out[i] = s;
     }
+}
+
+template <bool A_K, bool B_K, bool PACKED, int NW>
+static int launch_gemm(const GemmParams &p, dim3 grid, size_t smem_bytes, cudaStream_t stream) {
+    HRL_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<A_K, B_K, PACKED, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    gemm_tf32x3_kernel<A_K, B_K, PACKED, NW><<<grid, kGemmThreads, smem_bytes, stream>>>(p);
+    return HRL_OK;
+}
+
+// the operand layouts of one MMA width (a packed B image is k-major)
+template <int NW>
+static int launch_gemm_width(const GemmParams &p, dim3 grid, size_t smem_bytes, cudaStream_t stream) {
+    if (p.b.packed) return p.a.kmajor ? launch_gemm<true, true, true, NW>(p, grid, smem_bytes, stream)
+                                      : launch_gemm<false, true, true, NW>(p, grid, smem_bytes, stream);
+    if (p.a.kmajor) return p.b.kmajor ? launch_gemm<true, true, false, NW>(p, grid, smem_bytes, stream)
+                                      : launch_gemm<true, false, false, NW>(p, grid, smem_bytes, stream);
+    return p.b.kmajor ? launch_gemm<false, true, false, NW>(p, grid, smem_bytes, stream)
+                      : launch_gemm<false, false, false, NW>(p, grid, smem_bytes, stream);
 }
 
 }  // namespace hrl
@@ -988,30 +984,28 @@ extern "C" int hrl_gemm_fused(const HrlGemmArgs *args, void *stream_) {
     const size_t ep_bytes = 1024 + ((size_t)kTileM * (n_pad + 4) + 2 * red_rows * (size_t)n_pad) * 4;      // epilogue tile + column-sum scratch
     if (smem_bytes < ep_bytes) smem_bytes = ep_bytes;
     const dim3 grid((unsigned)((M + kTileM - 1) / kTileM), (unsigned)n_tiles, (unsigned)splits);
-    const int items_b = (n_pad * 8 + kGemmThreads - 1) / kGemmThreads;
-#define HRL_GEMM_LAUNCH3(AK, BK, IB, PK)                                                                                   \
-    {                                                                                                                     \
-        HRL_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<AK, BK, IB, PK>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
-                                            (int)smem_bytes));                                                            \
-        gemm_tf32x3_kernel<AK, BK, IB, PK><<<grid, kGemmThreads, smem_bytes, stream>>>(p, n_pad);                          \
+    int st;
+    switch (n_pad / 2) {          // the MMA width of a warpgroup: n_pad is a multiple of 16 up to 256, then 288
+    case 8: st = launch_gemm_width<8>(p, grid, smem_bytes, stream); break;
+    case 16: st = launch_gemm_width<16>(p, grid, smem_bytes, stream); break;
+    case 24: st = launch_gemm_width<24>(p, grid, smem_bytes, stream); break;
+    case 32: st = launch_gemm_width<32>(p, grid, smem_bytes, stream); break;
+    case 40: st = launch_gemm_width<40>(p, grid, smem_bytes, stream); break;
+    case 48: st = launch_gemm_width<48>(p, grid, smem_bytes, stream); break;
+    case 56: st = launch_gemm_width<56>(p, grid, smem_bytes, stream); break;
+    case 64: st = launch_gemm_width<64>(p, grid, smem_bytes, stream); break;
+    case 72: st = launch_gemm_width<72>(p, grid, smem_bytes, stream); break;
+    case 80: st = launch_gemm_width<80>(p, grid, smem_bytes, stream); break;
+    case 88: st = launch_gemm_width<88>(p, grid, smem_bytes, stream); break;
+    case 96: st = launch_gemm_width<96>(p, grid, smem_bytes, stream); break;
+    case 104: st = launch_gemm_width<104>(p, grid, smem_bytes, stream); break;
+    case 112: st = launch_gemm_width<112>(p, grid, smem_bytes, stream); break;
+    case 120: st = launch_gemm_width<120>(p, grid, smem_bytes, stream); break;
+    case 128: st = launch_gemm_width<128>(p, grid, smem_bytes, stream); break;
+    case 144: st = launch_gemm_width<144>(p, grid, smem_bytes, stream); break;
+    default: HRL_REQUIRE(false, HRL_ERR_BAD_ARG, "hrl_gemm_fused: no kernel for a tile of %d padded columns", n_pad);
     }
-#define HRL_GEMM_LAUNCH2(AK, BK, IB) HRL_GEMM_LAUNCH3(AK, BK, IB, false)
-#define HRL_GEMM_LAUNCH(IB)                                                                    \
-    {                                                                                         \
-        if (p.a.kmajor && p.b.kmajor) HRL_GEMM_LAUNCH2(true, true, IB)                        \
-        else if (p.a.kmajor) HRL_GEMM_LAUNCH2(true, false, IB)                                \
-        else if (p.b.kmajor) HRL_GEMM_LAUNCH2(false, true, IB)                                \
-        else HRL_GEMM_LAUNCH2(false, false, IB)                                               \
-    }
-    if (p.b.packed) {
-        if (p.a.kmajor) HRL_GEMM_LAUNCH3(true, true, 1, true)
-        else HRL_GEMM_LAUNCH3(false, true, 1, true)
-    } else if (items_b <= 1) HRL_GEMM_LAUNCH(1)
-    else if (items_b <= 3) HRL_GEMM_LAUNCH(3)
-    else HRL_GEMM_LAUNCH(5)
-#undef HRL_GEMM_LAUNCH
-#undef HRL_GEMM_LAUNCH2
-#undef HRL_GEMM_LAUNCH3
+    if (st != HRL_OK) return st;
     HRL_CUDA_CHECK(cudaGetLastError());
     if (splits > 1 && g.C != nullptr) {       // C == NULL: the caller consumes the slice partials itself (hrl_board_fold)
         const long long n = (long long)M * N;
