@@ -143,3 +143,44 @@ def refresh(prio, prio_serial, dir_serial, live_slots, max_prio):
             prio[s] = max_prio
             prio_serial[s] = dir_serial[s]
     return prio, prio_serial
+
+
+# ---------------------------------------------------------------- priorities in the replay checkpoints (train_args['save_replay'])
+
+def image(slot_serial, priority, max_prio, resident_serials):
+    """The priorities a replay checkpoint stores, keyed by serial: of the per-slot state (PriorityState.prio_serial and prio
+    as host arrays), the slots whose serial belongs to a resident episode.  A slot that never held an episode (-1) or whose
+    episode has left the ring is dropped; a resident episode the sampler has not seen yet has no entry."""
+    slot_serial, priority = np.asarray(slot_serial, np.int64), np.asarray(priority, np.float32)
+    resident = np.asarray(resident_serials, np.int64)
+    keep = (slot_serial >= 0) & np.isin(slot_serial, resident[resident >= 0])
+    order = np.argsort(slot_serial[keep], kind='stable')
+    return {'serial': slot_serial[keep][order], 'priority': priority[keep][order], 'max_prio': float(max_prio)}
+
+
+def restore_entries(saved, saved_serials, positions, slots, serials):
+    """Where a checkpoint's priorities go in a restored ring.  saved: {'serial', 'priority'} (image()); saved_serials: the
+    serial each position of the checkpoint's episode list had (-1: held out); positions: for each episode resident now, oldest
+    first, its position in that list, or -1 for an episode that was not in it; slots, serials: the directory slot and the
+    serial each has now.  Returns (slots, serials, priorities) of the episodes that get their saved priority; the others keep
+    none and start at max_prio, as a new episode does.  A serial is unique in a ring and a position maps to one episode, so no
+    slot appears twice; repeated positions or serials raise ValueError."""
+    key = np.asarray(saved['serial'], np.int64)
+    prio = np.asarray(saved['priority'], np.float32)
+    saved_serials, positions = np.asarray(saved_serials, np.int64), np.asarray(positions, np.int64)
+    slots, serials = np.asarray(slots, np.int64), np.asarray(serials, np.int64)
+    if key.shape != prio.shape or positions.shape != slots.shape or slots.shape != serials.shape:
+        raise ValueError('restore_entries: array lengths differ')
+    if np.unique(key).size != key.size:
+        raise ValueError('restore_entries: a serial appears twice in the saved priorities')
+    known = positions >= 0
+    if positions[known].size and (positions[known].max() >= saved_serials.size or
+                                  np.unique(positions[known]).size != positions[known].size):
+        raise ValueError('restore_entries: positions outside the saved list or repeated')
+    old = np.full(positions.shape, -1, np.int64)
+    old[known] = saved_serials[positions[known]]
+    order = np.argsort(key, kind='stable')
+    at = np.searchsorted(key[order], old)
+    hit = (old >= 0) & (at < key.size)
+    hit[hit] = key[order][at[hit]] == old[hit]
+    return slots[hit], serials[hit], prio[order][at[hit]]

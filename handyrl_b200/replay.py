@@ -10,6 +10,7 @@ host path through batch.sample_window.
 Store layout = include/hrl_b200.h HrlGatherArgs: one row per episode step, columns per player slot.
 Nested observations are stored as the concatenation of their flattened leaves.
 """
+import collections
 import ctypes as C
 import hashlib
 import random
@@ -61,9 +62,13 @@ class DeviceReplay:
     deque to `maximum_episodes`, train.py:474-483); when either is exceeded the oldest episodes go.
     The episode directory (first row / length / outcome row, oldest first) is a numpy ring so that B windows
     are drawn with array operations instead of a Python loop per window.
+
+    track=True (train_args['save_replay']): `resident` holds, for every directory entry and in its order, the item the caller
+    staged with that episode (stage(fes, items); the GPU batcher passes the episode as it arrived), appended and evicted with
+    the directory under `lock`.  References only: nothing is copied and nothing is done per step.
     """
 
-    def __init__(self, capacity_steps, max_episodes, device='cuda', mirror=False):
+    def __init__(self, capacity_steps, max_episodes, device='cuda', mirror=False, track=False):
         self.device = torch.device(device)
         self.capacity = int(capacity_steps)
         self.max_episodes = int(max_episodes)
@@ -74,6 +79,7 @@ class DeviceReplay:
         self.ready = False
         self.next_outcome_row = 0
         self.lock = threading.Lock()       # guards the directory (feeder thread appends, learner thread samples)
+        self.resident = collections.deque() if track else None
         # every stored episode gets the next serial, so a directory slot that is reused is told apart from its old episode
         self._serial = np.full(self.max_episodes + 1, -1, np.int64)
         self.next_serial = 0
@@ -96,14 +102,24 @@ class DeviceReplay:
     def _popleft(self):
         self._head = (self._head + 1) % self._dir.shape[0]
         self._count -= 1
+        if self.resident is not None:
+            self.resident.popleft()
 
-    def _append(self, first_step, steps, row):
+    def _append(self, first_step, steps, row, item=None):
         slot = (self._head + self._count) % self._dir.shape[0]
         self._dir[slot] = (first_step, steps, row)
         self._serial[slot] = self.next_serial
         self.next_serial += 1
         self._count += 1
+        if self.resident is not None:
+            self.resident.append(item)
         return slot
+
+    def positions(self):
+        """(slots, serials) of the stored episodes, oldest first: the directory slot each sits in and the serial it was given
+        (int64 arrays; take them under self.lock when a feeder runs)."""
+        slots = (self._head + np.arange(self._count, dtype=np.int64)) % self._dir.shape[0]
+        return slots, self._serial[slots].copy()
 
     def snapshot(self, max_count):
         """(head slot, count) of the directory now, count capped at max_count (the sampler's view; take it under self.lock)."""
@@ -153,10 +169,10 @@ class DeviceReplay:
         """Upload several decoded episodes (stage + commit)."""
         return self.commit(self.stage(fes)) if fes else []
 
-    def stage(self, fes):
+    def stage(self, fes, items=None):
         """Host half of an upload: concatenate the episodes' step rows column by column into page-locked staging
         tensors.  Touches neither the ring nor the directory, so a feeder thread can do it without holding any lock
-        the learner needs."""
+        the learner needs.  `items` (one per episode, with track=True): what commit() puts in `resident` for each."""
         if not self.ready:
             self._allocate(fes[0])
         pin = self.device.type == 'cuda'
@@ -174,7 +190,9 @@ class DeviceReplay:
             'reward': host([fe.reward for fe in fes], np.float32), 'return': host([fe.ret for fe in fes], np.float32),
             'flags': host([fe.flags for fe in fes], np.uint8), 'turn': host([fe.turn for fe in fes], np.int32),
         }
-        return {'steps': [int(fe.steps) for fe in fes], 'cols': cols,
+        if items is not None and len(items) != len(fes):
+            raise ValueError('stage: %d items for %d episodes' % (len(items), len(fes)))
+        return {'steps': [int(fe.steps) for fe in fes], 'cols': cols, 'items': items,
                 'outcome': host([np.stack([fe.outcome for fe in fes])], np.float32)}
 
     def commit(self, staged):
@@ -185,7 +203,8 @@ class DeviceReplay:
         rows, appended = [], []
         with self.lock:
             src = 0
-            for n in staged['steps']:
+            items = staged.get('items') or [None] * len(staged['steps'])
+            for n, item in zip(staged['steps'], items):
                 if n > self.capacity:
                     raise ValueError('episode of %d steps exceeds the replay capacity of %d steps' % (n, self.capacity))
                 if self.write + n > self.capacity:          # episodes are stored contiguously: wrap
@@ -206,7 +225,7 @@ class DeviceReplay:
                 else:
                     segments.append([lo, src, n])
                 rows.append(row)
-                appended.append(self._append(lo, n, row))
+                appended.append(self._append(lo, n, row, item))
                 handles.append(EpisodeHandle(lo, n, row))
                 self.write = hi
                 src += n

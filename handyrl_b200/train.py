@@ -425,6 +425,170 @@ def replay_ratio_line(stats):
     return 'replay_ratio = %slimit:%g waited:%.2f' % (head, stats['limit'], stats['waited'])
 
 
+def save_replay(args):
+    """train_args['save_replay'] -> {'every': n, 'keep': k}: the replay is saved with every n-th numbered epoch and the run keeps
+    the newest k files it wrote (0: all), or None when the key is off (absent, None, False or 0).  True is n = 1; a positive
+    integer is n; {'every': n, 'keep': k} sets both (defaults 1 and 2).  Anything else raises ValueError, and so does the key
+    with gpu_replay: False (the saved set is what the GPU replay holds)."""
+    value = args.get('save_replay')
+    if value is None or value is False or (isinstance(value, numbers.Integral) and not isinstance(value, bool) and value == 0):
+        return None
+    spec = {'every': 1, 'keep': 2}
+    if isinstance(value, dict):
+        unknown = sorted(set(value) - set(spec), key=str)
+        if unknown:
+            raise ValueError("train_args['save_replay']: unknown key(s) %s (known: every, keep)" % unknown)
+        spec.update(value)
+    elif value is not True:
+        spec['every'] = value
+    for k, least in (('every', 1), ('keep', 0)):
+        v = spec[k]
+        if isinstance(v, bool) or not isinstance(v, numbers.Integral) or v < least:
+            raise ValueError("train_args['save_replay']: %s must be an integer >= %d; got %r" % (k, least, v))
+        spec[k] = int(v)
+    if not args.get('gpu_replay', True):
+        raise ValueError("train_args['save_replay'] needs the GPU replay (gpu_replay: True): it saves what that replay holds")
+    return spec
+
+
+_save_replay_spec = save_replay       # for the constructors whose `save_replay` argument shadows the parser
+
+REPLAY_FORMAT = 1
+
+
+def replay_file(snapshot, priority_state=None, limiter=None, steps=0, epoch=0):
+    """The dict of a models/<epoch>.replay.pth file (plain containers and tensors: it loads with torch.load alone):
+
+        {'format': 1,
+         'episodes': [episode, ...],    the episodes resident in the training and held-out rings, oldest first, as they arrived
+         'serials': int64 tensor,       the DeviceReplay serial of each, -1 for a held-out episode
+         'capacity_steps', 'maximum_episodes': int,
+         'sampler': {'rng', 'val_rng', 'sym_rng' (or None): numpy bit_generator.state dicts, 'prio_batches': int},
+         'priorities': None or {'serial': int64 tensor, 'priority': float32 tensor, 'max_prio': float}  (priority.image),
+         'limiter': None or ReplayRatioLimiter.snapshot(), 'steps': Trainer.steps, 'epoch': int}
+
+    snapshot: GpuBatcher.snapshot(); priority_state: LearnerStep.priority_state_dict() / PendingModel.priority_state."""
+    prio = None
+    if priority_state is not None:
+        img = priority.image(priority_state['slot_serial'].numpy(), priority_state['priority'].numpy(),
+                             priority_state['max_prio'], snapshot['serials'].numpy())
+        prio = {'serial': torch.from_numpy(img['serial']), 'priority': torch.from_numpy(img['priority']),
+                'max_prio': img['max_prio']}
+    return dict(snapshot, format=REPLAY_FORMAT, priorities=prio, limiter=limiter, steps=int(steps), epoch=int(epoch))
+
+
+def load_replay_file(path, leaf_shapes=None, actions=None):
+    """Read a replay file and check it: a known 'format', every entry present, one serial per episode, every episode a dict
+    with its step count and one of the two wire formats, the first episode decodable, and -- when given -- its observation
+    leaf shapes and action count equal to `leaf_shapes` (a list of tuples) and `actions`.  Raises ValueError naming the file."""
+    from .wire import episode_to_flat
+    try:
+        d = torch.load(path, map_location='cpu')
+    except Exception as e:
+        raise ValueError('%s: not a readable replay file (%s)' % (path, e))
+    if not isinstance(d, dict) or d.get('format') != REPLAY_FORMAT:
+        raise ValueError('%s: unknown replay file format %r (this version reads %d)'
+                         % (path, d.get('format') if isinstance(d, dict) else type(d).__name__, REPLAY_FORMAT))
+    missing = [k for k in ('episodes', 'serials', 'capacity_steps', 'maximum_episodes', 'sampler', 'priorities') if k not in d]
+    if missing:
+        raise ValueError('%s: no %s entry' % (path, ', '.join(missing)))
+    eps = d['episodes']
+    if not isinstance(eps, list) or len(d['serials']) != len(eps):
+        raise ValueError('%s: %d serials for %s episodes' % (path, len(d['serials']), len(eps) if isinstance(eps, list) else 'no'))
+    for i, ep in enumerate(eps):
+        if not isinstance(ep, dict) or not isinstance(ep.get('steps'), numbers.Integral) or ep['steps'] <= 0 \
+                or 'outcome' not in ep or not ('flat' in ep or ep.get('moment')):
+            raise ValueError('%s: episode %d is not an episode in either wire format' % (path, i))
+    if eps:
+        try:
+            fe = episode_to_flat(eps[0])
+            shapes, A = [tuple(l.shape[2:]) for l in tree_leaves(fe.obs)], int(fe.amask.shape[-1])
+        except Exception as e:
+            raise ValueError('%s: the episodes do not decode (%s: %s)' % (path, type(e).__name__, e))
+        if leaf_shapes is not None and shapes != [tuple(sh) for sh in leaf_shapes]:
+            raise ValueError('%s: observations of shape %s, expected %s' % (path, shapes, [tuple(sh) for sh in leaf_shapes]))
+        if actions is not None and A != int(actions):
+            raise ValueError('%s: %d actions, expected %d' % (path, A, int(actions)))
+    return d
+
+
+class ReplayCheckpoints:
+    """Writes models/<epoch>.replay.pth files off the caller's thread.  submit(epoch, obj) returns at once: one writer thread
+    (started by the first submit) torch.saves obj to a temporary name in the directory and renames it, so a file that exists
+    is complete.  While a write runs at most one submission waits: a newer one replaces it.  After each write the files this
+    object wrote beyond the newest `keep` are deleted (keep = 0: none); files it did not write are never touched.  close()
+    writes what still waits and joins the thread."""
+
+    def __init__(self, directory='models', keep=2):
+        self.directory, self.keep = directory, int(keep)
+        self.cond = threading.Condition()
+        self.queued = None
+        self.closed = False
+        self.thread = None
+        self.written = []           # paths this object wrote and has not deleted, oldest first
+        self.replaced = 0           # submissions a newer one overtook
+        self.last_error = None
+
+    def path(self, epoch):
+        return os.path.join(self.directory, '%s.replay.pth' % epoch)
+
+    def write(self, epoch, obj):
+        """Write one file now, on this thread; returns its path."""
+        os.makedirs(self.directory, exist_ok=True)
+        path = self.path(epoch)
+        tmp = path + '.tmp'
+        try:
+            torch.save(obj, tmp)
+            os.replace(tmp, path)
+        except BaseException:
+            if os.path.exists(tmp):
+                os.remove(tmp)
+            raise
+        if path in self.written:
+            self.written.remove(path)
+        self.written.append(path)
+        while self.keep and len(self.written) > self.keep:
+            old = self.written.pop(0)
+            if os.path.exists(old):
+                os.remove(old)
+        return path
+
+    def submit(self, epoch, obj):
+        with self.cond:
+            if self.closed:
+                raise RuntimeError('ReplayCheckpoints is closed')
+            if self.queued is not None:
+                self.replaced += 1
+            self.queued = (epoch, obj)
+            if self.thread is None:
+                self.thread = threading.Thread(target=self._run, daemon=True)
+                self.thread.start()
+            self.cond.notify_all()
+
+    def _run(self):
+        while True:
+            with self.cond:
+                while self.queued is None and not self.closed:
+                    self.cond.wait()
+                if self.queued is None:
+                    return
+                epoch, obj = self.queued
+                self.queued = None
+            try:
+                self.write(epoch, obj)
+            except Exception as e:          # a full disk must not end the run: the next epoch tries again
+                self.last_error = e
+                traceback.print_exc()
+
+    def close(self):
+        with self.cond:
+            self.closed = True
+            self.cond.notify_all()
+        if self.thread is not None:
+            self.thread.join()
+            self.thread = None
+
+
 def nonfinite_guard(args):
     """train_args['skip_nonfinite'] -> whether optimiser steps whose loss or gradient is not finite are rejected on the device
     (key absent, False or None: off)."""
@@ -603,7 +767,9 @@ class PendingModel:
     `skip_nonfinite` give (accum_slots); with the guard, the number of the epoch's `batch_cnt` steps that were rejected is left
     in `skipped` and, when it is not zero, printed (skipped_line) after the loss and diagnostics lines.  The Trainer sets
     `replay_ratio` to the epoch's ReplayRatioLimiter.end_epoch() figures under train_args['replay_ratio'], and report() prints
-    them (replay_ratio_line) after those lines and before the validation lines."""
+    them (replay_ratio_line) after those lines and before the validation lines.  Under train_args['save_replay'] the Trainer
+    sets `replay` to the GpuBatcher.snapshot() taken at the boundary, and with the priorities ('prio', the prio_snap layout)
+    resolve() leaves them in `priority_state` (what LearnerStep.priority_state_dict() returns)."""
 
     def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host=None, steps=0, diagnostics=False,
                  skip_nonfinite=False, batch_cnt=0):
@@ -615,6 +781,8 @@ class PendingModel:
         self.validation = None
         self.skipped = 0
         self.replay_ratio = None
+        self.replay = None
+        self.priority_state = None
 
     def report(self):
         """Read the epoch's sums from the host copy (already arrived) and print the epoch's lines; returns the loss sums."""
@@ -653,6 +821,8 @@ class PendingModel:
             self.ema_state = collections.OrderedDict((k, avg[k]) for k in keys)
         if 'optim' in self.host:
             self.optim_state = stepper.optimizer_state_from(self.host['optim'], self.steps)
+        if 'prio' in self.host:
+            self.priority_state = stepper.priority_state_from(self.host['prio'])
         tpl.load_state_dict({k: state[k] for k in keys})
         tpl.eval()
         blob = pickle.dumps(tpl)
@@ -724,6 +894,11 @@ class LearnerStep:
     keep counting batches drawn; a rejected batch adds nothing to dcnt.  One more launch per step.  Validation passes are not
     guarded.
 
+    save_replay (default: whether train_args['save_replay'] is set, off): with prioritized_replay, end_epoch also hands over the
+    per-slot priorities, their serials and max_prio (PendingModel.priority_state), by the same device-to-device snapshot and
+    side-stream copy.  priority_state_dict() reads them now; load_priority_state() writes saved ones.  The step is the same
+    with and without.
+
     A feature that adds device state registers it in __init__, where it allocates it: in `_mutable` (or `_zeroed`) when a
     step or validation pass changes it, so that the capture's warm-up leaves it as it was, and in `_handoff` (a _Handoff)
     when the epoch boundary carries it to the host; end_epoch, _snapshot and _restore have no per-feature code.
@@ -732,7 +907,8 @@ class LearnerStep:
     def __init__(self, model, args, example_batch, lr, device=None, process_group=None, use_graph=True,
                  max_norm=4.0, weight_decay=1e-5, time_loss_kernel=False, channels_last=True, cudnn_benchmark=True,
                  small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None,
-                 weight_ema=None, save_optimizer=None, validation=None, skip_nonfinite=None):
+                 weight_ema=None, save_optimizer=None, validation=None, skip_nonfinite=None, save_replay=None):
+        self.save_replay = bool(_save_replay_spec(args) is not None if save_replay is None else save_replay)
         self.weight_ema = weight_ema_decay(args.get('weight_ema') if weight_ema is None else weight_ema)
         rate = validation_rate(args)
         symmetry.config(args)           # malformed train_args['symmetry'] fails here; the gather applies it, not the step
@@ -846,6 +1022,10 @@ class LearnerStep:
         self.prio_state = None
         if self.priority is not None:
             self.prio_state = priority.PriorityState(self.priority, priority.ring_slots(args), B, self.device)
+        self.prio_snap = None            # priorities of the epoch hand-off (_prio_views)
+        if self.prio_state is not None and self.save_replay:
+            self.prio_snap = self._prio_image(self.device)
+            self._handoff.append(_Handoff('prio', self.prio_snap, self._prio_copies(self.prio_snap)))
         self.hidden0 = None
         if hasattr(self.model, 'init_hidden'):
             self.hidden0 = tree_map(lambda h: h.to(self.device), self.model.init_hidden([B, P]))
@@ -1301,6 +1481,61 @@ class LearnerStep:
             self.ema.fill_(data_cnt_ema)
         self.schedule_steps = steps
 
+    def _prio_views(self, buf):
+        """(prio_serial, prio, max_prio) views of a byte buffer in the prio_snap layout:
+        [prio_serial (ring int64) | prio (ring fp32) | max_prio (fp32)], padded to 8 bytes."""
+        r = self.prio_state.ring
+        return buf[:8 * r].view(torch.int64), buf[8 * r:12 * r].view(torch.float32), buf[12 * r:12 * r + 4].view(torch.float32)
+
+    def _prio_image(self, device):
+        return torch.empty((12 * self.prio_state.ring + 4 + 7) // 8 * 8, dtype=torch.uint8, device=device)
+
+    def _prio_copies(self, image):
+        ps = self.prio_state
+        return list(zip(self._prio_views(image), (ps.prio_serial, ps.prio, ps.max_prio)))
+
+    def _require_priorities(self):
+        if self.prio_state is None:
+            raise RuntimeError('LearnerStep was built without prioritised replay (train_args["prioritized_replay"])')
+
+    def priority_state_from(self, host_prio):
+        """{'slot_serial': int64 [ring], 'priority': float32 [ring], 'max_prio': float} of a host copy of prio_snap: per slot of
+        the replay directory, the serial of the episode the priority belongs to (-1: none yet) and the priority."""
+        serial, prio, mx = self._prio_views(host_prio)
+        return {'slot_serial': serial.clone(), 'priority': prio.clone(), 'max_prio': float(mx[0])}
+
+    def priority_state_dict(self):
+        """Blocking copy of the priorities as the next batch's sampler finds them (what end_epoch hands over as
+        PendingModel.priority_state under save_replay)."""
+        self._require_priorities()
+        self.stream.synchronize()
+        image = self._prio_image('cpu')
+        for dst, src in self._prio_copies(image):
+            dst.copy_(src)
+        return self.priority_state_from(image)
+
+    def load_priority_state(self, slots, serials, priorities, max_prio):
+        """Give the episodes in directory slots `slots`, which hold serials `serials`, the priorities `priorities`, and set
+        max_prio: ordinary indexed copies on the step stream, outside the captured step.  Every other slot is left alone, so
+        its episode starts at max_prio when the sampler first sees it.  The capture's warm-up steps run with serial -1 and
+        write no priority, so this may come before or after warm_up(); it must come before the first prioritised batch."""
+        self._require_priorities()
+        ps = self.prio_state
+        idx = torch.as_tensor(np.asarray(slots, np.int64))
+        ser = torch.as_tensor(np.asarray(serials, np.int64))
+        pri = torch.as_tensor(np.asarray(priorities, np.float32))
+        if not (idx.shape == ser.shape == pri.shape and idx.dim() == 1):
+            raise ValueError('load_priority_state: slots, serials and priorities must be 1-d and of one length')
+        if idx.numel() and (int(idx.min()) < 0 or int(idx.max()) >= ps.ring or idx.unique().numel() != idx.numel()):
+            raise ValueError('load_priority_state: slots outside [0, %d) or repeated' % ps.ring)
+        if not (np.isfinite(float(max_prio)) and float(max_prio) > 0 and bool(torch.isfinite(pri).all()) and bool((pri > 0).all())):
+            raise ValueError('load_priority_state: priorities and max_prio must be finite and positive')
+        with torch.cuda.stream(self.stream):
+            dev = idx.to(self.device)
+            ps.prio.index_copy_(0, dev, pri.to(self.device))
+            ps.prio_serial.index_copy_(0, dev, ser.to(self.device))
+            ps.max_prio.fill_(float(max_prio))
+
     def epoch_schedule(self, batch_cnt, steps, default_lr):
         """Device half of the epoch boundary, on the current stream: move the epoch's loss sums aside and apply the
         learning-rate schedule from the (all-reduced, hence global) data count.  Every rank of a sharded learner
@@ -1522,11 +1757,17 @@ class GpuBatcher:
     fill_validation() keeps the host sampler.
 
     With a `limiter` (a ReplayRatioLimiter, train_args['replay_ratio']), the feeder adds the steps of the episodes it committed
-    to the training ring after each commit; held-out episodes add nothing."""
+    to the training ring after each commit; held-out episodes add nothing.
+
+    With train_args['save_replay'] set (or track_resident=True), both rings keep the episodes they hold as they arrived
+    (DeviceReplay.resident, references only) and snapshot() returns them with the sampler's state; restore_sampler() puts that
+    state back.  `restore`: the dict of a replay file whose episodes are this batcher's backlog; the ring is then sized to hold
+    at least the file's capacity_steps where memory allows."""
 
     DESC_SLOTS = 4        # pinned descriptor buffers in rotation: bounds how far the host runs ahead of the GPU
 
-    def __init__(self, args, episodes, device, seed=None, forward=None, keep_validation=True, limiter=None):
+    def __init__(self, args, episodes, device, seed=None, forward=None, keep_validation=True, limiter=None,
+                 track_resident=None, restore=None):
         from .replay import DeviceReplay
         from .wire import episode_to_flat
         self.args = args
@@ -1552,6 +1793,8 @@ class GpuBatcher:
         self.fed = 0
         self._slots = None
         self._slot_i = 0
+        self.track_resident = bool(_save_replay_spec(args) is not None if track_resident is None else track_resident)
+        self._arrivals = 0                  # episodes the feeder has split so far: orders the two rings' episodes in a snapshot
 
         # tap first, then the backlog: nothing is missed; what the tap saw meanwhile is not enqueued twice, and the
         # backlog keeps its (recency) order ahead of it
@@ -1594,12 +1837,23 @@ class GpuBatcher:
             if est < args['maximum_episodes']:
                 print('handyrl_b200: the GPU replay holds about %d episodes (%d steps), fewer than maximum_episodes=%d'
                       % (est, cap, args['maximum_episodes']))
-        self.replay = DeviceReplay(cap, args['maximum_episodes'], device=device, mirror=self.priority is not None)
+        saved = int(restore['capacity_steps']) if restore is not None else 0
+        if saved > cap:                     # a restored backlog filled a ring of `saved` steps: hold all of it where memory allows
+            room = saved
+            if fe0 is not None and torch.device(device).type == 'cuda':
+                free, _ = torch.cuda.mem_get_info(device)
+                room = int(args.get('replay_memory_fraction', 0.5) * free / DeviceReplay.bytes_per_step(fe0))
+            if room < saved:
+                print('handyrl_b200: the GPU replay holds about %d episodes (%d steps), fewer than maximum_episodes=%d'
+                      % (int(max(cap, room) / max(mean_len, 1)), max(cap, room), args['maximum_episodes']))
+            cap = max(cap, min(saved, room))
+        self.replay = DeviceReplay(cap, args['maximum_episodes'], device=device, mirror=self.priority is not None,
+                                   track=self.track_resident)
         self.val_replay = None
         if self.validation is not None and keep_validation:
             r = self.validation
             self.val_replay = DeviceReplay(max(int(r * cap), 2 * max_len), max(1, int(round(r * args['maximum_episodes']))),
-                                           device=device)
+                                           device=device, track=self.track_resident)
         self.thread = threading.Thread(target=self._feed, daemon=True)
 
     def run(self):
@@ -1626,8 +1880,14 @@ class GpuBatcher:
                 held = [held_out(fe, self.validation) for fe in fes]
                 train = [fe for fe, h in zip(fes, held) if not h]
                 val = [fe for fe, h in zip(fes, held) if h] if self.val_replay is not None else []
-                staged = self.replay.stage(train) if train else None
-                val_staged = self.val_replay.stage(val) if val else None
+                items = val_items = ()      # without resident lists the rings are staged exactly as before
+                if self.track_resident:     # (arrival number, the episode as it arrived) rides with each directory entry
+                    tagged = list(zip(range(self._arrivals, self._arrivals + len(eps)), eps))
+                    self._arrivals += len(eps)
+                    items = ([it for it, h in zip(tagged, held) if not h],)
+                    val_items = ([it for it, h in zip(tagged, held) if h],)
+                staged = self.replay.stage(train, *items) if train else None
+                val_staged = self.val_replay.stage(val, *val_items) if val else None
                 with self.order_lock:
                     if self.last_gather is not None:   # device-side: never overwrite rows an enqueued gather reads
                         self.upload_stream.wait_event(self.last_gather)
@@ -1644,6 +1904,45 @@ class GpuBatcher:
             except Exception:
                 traceback.print_exc()
             self.fed += len(eps)
+
+    def snapshot(self):
+        """What a replay file stores of this batcher, as of one instant (taken under the lock that orders sampling and
+        uploads): {'episodes': the episodes resident in the training and held-out rings, oldest arrival first, as they arrived;
+        'serials': int64 tensor, the training ring's serial of each, -1 for a held-out one; 'capacity_steps';
+        'maximum_episodes'; 'sampler': {'rng', 'val_rng', 'sym_rng' (None without symmetry): bit_generator.state dicts,
+        'prio_batches': the Philox counter of the next prioritised batch}}.  References and small arrays only."""
+        if not self.track_resident:
+            raise RuntimeError("GpuBatcher keeps no resident lists (train_args['save_replay'] / track_resident=True)")
+        with self.order_lock:
+            with self.replay.lock:
+                items = list(self.replay.resident)
+                serials = self.replay.positions()[1]
+            val_items = []
+            if self.val_replay is not None:
+                with self.val_replay.lock:
+                    val_items = list(self.val_replay.resident)
+            sampler = {'rng': copy.deepcopy(self.rng.bit_generator.state),
+                       'val_rng': copy.deepcopy(self.val_rng.bit_generator.state),
+                       'sym_rng': copy.deepcopy(self.sym_rng.bit_generator.state) if self.sym_rng is not None else None,
+                       'prio_batches': int(self.prio_batches)}
+        if val_items:                       # two runs sorted by arrival: one stable merge
+            serials = np.concatenate([serials, np.full(len(val_items), -1, np.int64)])
+            items = items + val_items
+            order = np.argsort(np.fromiter((a for a, _ in items), np.int64, len(items)), kind='stable')
+            items, serials = [items[i] for i in order], serials[order]
+        return {'episodes': [ep for _, ep in items], 'serials': torch.from_numpy(np.ascontiguousarray(serials)),
+                'capacity_steps': int(self.replay.capacity), 'maximum_episodes': int(self.args['maximum_episodes']),
+                'sampler': sampler}
+
+    def restore_sampler(self, sampler):
+        """Put back the sampler state of a snapshot(): the generators of the training, validation and transform draws and the
+        prioritised sampler's batch counter.  A generator the snapshot lacks (symmetry was off) keeps its seed."""
+        with self.order_lock:
+            for name in ('rng', 'val_rng', 'sym_rng'):
+                gen, state = getattr(self, name), sampler.get(name)
+                if gen is not None and state is not None:
+                    gen.bit_generator.state = state
+            self.prio_batches = int(sampler['prio_batches'])
 
     def ready(self):
         """True once the whole backlog the trainer started with is resident (the reference samples from at least
@@ -1762,6 +2061,23 @@ class GpuBatcher:
             self.thread.join(timeout=5)
 
 
+def restore_priorities(stepper, batcher, d):
+    """Give the episodes of the replay file dict `d` that are resident in `batcher` (a GpuBatcher fed the very objects of
+    d['episodes']) their saved priorities in `stepper`, and set max_prio.  An episode is found by its object, since the
+    restored ring hands out new slots and serials.  Returns how many got one (0 when either side has no priorities)."""
+    if d['priorities'] is None or stepper.prio_state is None:
+        return 0
+    index = {id(ep): i for i, ep in enumerate(d['episodes'])}
+    with batcher.replay.lock:
+        items = list(batcher.replay.resident)
+        slots, serials = batcher.replay.positions()
+    positions = np.fromiter((index.get(id(ep), -1) for _, ep in items), np.int64, len(items))
+    saved = {k: np.asarray(d['priorities'][k]) for k in ('serial', 'priority')}
+    slots, serials, prio = priority.restore_entries(saved, np.asarray(d['serials']), positions, slots, serials)
+    stepper.load_priority_state(slots, serials, prio, d['priorities']['max_prio'])
+    return len(slots)
+
+
 class Trainer:
     """Drop-in for handyrl.train.Trainer (train.py:321-400): same constructor, attributes
     (`episodes`, `steps`), `run()` thread body and `update()` hand-off, same printed lines.
@@ -1801,18 +2117,27 @@ class Trainer:
     on the device with probability proportional to the recency law times a per-episode priority from the fused loss's
     advantages, and weighted to correct the bias (LearnerStep, GpuBatcher).  The printed lines keep their format; the loss
     line reports the weighted objective.  Validation batches use the host sampler and no weights.  Each rank keeps the
-    priorities of its own shard.  Priorities are not saved: after a restart every episode starts at max_prio.  Needs
-    gpu_replay.
+    priorities of its own shard.  Priorities are saved with the replay under save_replay; without it every episode starts at
+    max_prio after a restart.  Needs gpu_replay.
 
     train_args['replay_ratio'] = r > 0: before each batch (each chunk with several GPUs) the trainer thread waits until the
     samples trained since this Trainer started, that batch included, are at most r times the steps stored in the training
     replay since then (ReplayRatioLimiter; the backlog counts, held-out episodes and validation batches do not).  So that
     update() cannot deadlock the Learner, an epoch that has not taken a step yet when update() waits lets one step (chunk)
     through: each epoch exceeds the limit by at most that.  Each epoch prints 'replay_ratio = <ratio> limit:<r>
-    waited:<fraction>' after the loss, diagnostics and skipped lines; replay_ratio_stats() returns the counts."""
+    waited:<fraction>' after the loss, diagnostics and skipped lines; replay_ratio_stats() returns the counts.
+
+    train_args['save_replay'] = True, n or {'every': n, 'keep': k}: with every n-th numbered epoch, update() hands the episodes
+    resident in the GPU replay (training and held-out rings), the sampler's random state, the priorities and the limiter's
+    counts -- all as of the epoch boundary the checkpoint's weights belong to -- to a writer thread that writes
+    models/<epoch>.replay.pth (replay_file, ReplayCheckpoints; numbered like .ema.pth and .optim.pth) and keeps the newest k
+    files this run wrote.  A run restarted at restart_epoch with models/<restart_epoch>.replay.pth present starts with those
+    episodes in `episodes`, trains at once, and restores the sampler state and priorities before its first batch; it prints
+    'restored replay: <n> episodes (<m> held out), <s> steps, priorities: <yes|no>'.  Needs gpu_replay."""
 
     def __init__(self, args, model):
         ratio = replay_ratio(args)
+        self.save_replay = save_replay(args)
         self.weight_ema = weight_ema_decay(args.get('weight_ema'))
         self.validation = validation_rate(args)
         self.symmetry = symmetry.config(args)
@@ -1820,7 +2145,7 @@ class Trainer:
         self.validate_every = max(1, int(round(1.0 / self.validation))) if self.validation is not None else 0
         self.save_optimizer = bool(args.get('save_optimizer', False))
         self.checkpoint_files = None         # numbers the .ema.pth and .optim.pth files of one epoch alike
-        if self.weight_ema is not None or self.save_optimizer:
+        if self.weight_ema is not None or self.save_optimizer or self.save_replay is not None:
             self.checkpoint_files = AveragedCheckpoints(args.get('restart_epoch', 0))
         self.ema_files = self.checkpoint_files if self.weight_ema is not None else None
         self.optim_files = self.checkpoint_files if self.save_optimizer else None
@@ -1855,6 +2180,59 @@ class Trainer:
             if self.world > 1 and (not self.gpu_replay or args['batch_size'] % self.world != 0):
                 print('handyrl_b200: multi-GPU needs gpu_replay and batch_size %% num_gpus == 0; using one GPU')
                 self.world = 1
+        self.replay_files = None             # the writer of the .replay.pth files
+        self.restored = None                 # the replay file this run resumed from, until its sampler state is put back
+        self.restored_limiter = None         # the limiter counts that file held
+        if self.save_replay is not None:
+            self.replay_files = ReplayCheckpoints(self.checkpoint_files.directory, keep=self.save_replay['keep'])
+            if self.checkpoint_files.restart_epoch > 0:
+                self._restore_replay()
+
+    def _restore_replay(self):
+        """Start from models/<restart_epoch>.replay.pth: its episodes go into `episodes`, oldest first, before the Learner
+        appends any; the sampler state and the priorities follow once they are resident (_finish_restore)."""
+        path = self.checkpoint_files.seed_path('replay')
+        if path is None:
+            print('handyrl_b200: no %s, the replay starts empty'
+                  % self.checkpoint_files.path(self.checkpoint_files.restart_epoch, 'replay'))
+            return
+        d = load_replay_file(path)
+        if d['episodes'] and len(self.params) > 0:
+            self._check_fits_net(d['episodes'][0], path)
+        self.episodes.extend(d['episodes'])
+        self.restored = d
+        self.restored_limiter = d.get('limiter')
+        held = int((d['serials'] < 0).sum())
+        print('restored replay: %d episodes (%d held out), %d steps, priorities: %s'
+              % (len(d['episodes']), held, sum(ep['steps'] for ep in d['episodes']),
+                 'yes' if d['priorities'] is not None and self.priority is not None else 'no'))
+
+    def _check_fits_net(self, episode, path):
+        """A saved episode must be one this run's net can train on: the net takes its observation and answers with one
+        logit per saved action.  Raises ValueError naming the file."""
+        from .wire import episode_to_flat
+        fe = episode_to_flat(episode)
+        obs = tree_map(lambda a: torch.from_numpy(np.ascontiguousarray(a[0, :1], dtype=np.float32)).to(self.params[0].device), fe.obs)
+        was_training = self.model.training
+        self.model.eval()
+        try:
+            with torch.no_grad():
+                hidden = self.model.init_hidden([1]) if hasattr(self.model, 'init_hidden') else None
+                policy = self.model(obs, hidden)['policy']
+        except Exception as e:
+            raise ValueError('%s: the net does not take its observations of shape %s (%s: %s)'
+                             % (path, [tuple(l.shape[2:]) for l in tree_leaves(fe.obs)], type(e).__name__, e))
+        finally:
+            self.model.train(was_training)
+        if policy.shape[-1] != fe.amask.shape[-1]:
+            raise ValueError('%s: %d actions, the net has %d' % (path, fe.amask.shape[-1], policy.shape[-1]))
+
+    def _finish_restore(self):
+        """The restored backlog is resident: put back the sampler state and the priorities (rank 0's; helper ranks start
+        theirs afresh)."""
+        d, self.restored = self.restored, None
+        self.gpu_batcher.restore_sampler(d['sampler'])
+        restore_priorities(self.stepper, self.gpu_batcher, d)
 
     def update(self):
         """Called by the Learner (train.py:342-345, 533): ends the running epoch and returns (CPU model in eval
@@ -1879,6 +2257,11 @@ class Trainer:
             if self.optim_files is not None and item.optim_state is not None:
                 files['optim'] = item.optim_state
             self.checkpoint_files.save_epoch(files)
+            epoch = self.checkpoint_files.epoch
+            if self.replay_files is not None and item.replay is not None and epoch % self.save_replay['every'] == 0:
+                self.replay_files.submit(epoch, replay_file(
+                    item.replay, item.priority_state, self.limiter.snapshot() if self.limiter is not None else None,
+                    item.steps, epoch))
         # host mirrors of the schedule the device applied (train.py:382-384), for inspection / logging
         self.data_cnt_ema = self.data_cnt_ema * 0.8 + sums['dcnt'] / (1e-2 + item.batch_cnt) * 0.2
         self.lr = self.default_lr * self.data_cnt_ema / (1 + steps * 1e-5)
@@ -1891,7 +2274,10 @@ class Trainer:
         its replay_ratio line printed: ReplayRatioLimiter.end_epoch), or None before the first}."""
         if self.limiter is None:
             return None
-        return dict(self.limiter.snapshot(), epoch=self.replay_ratio_epoch)
+        stats = dict(self.limiter.snapshot(), epoch=self.replay_ratio_epoch)
+        if self.save_replay is not None:     # what the replay file this run resumed from recorded; not applied to the limiter
+            stats['restored'] = self.restored_limiter
+        return stats
 
     def _start_stepper(self):
         # the first batch is built on the host: it fixes every shape of the captured step
@@ -1926,7 +2312,7 @@ class Trainer:
         if self.gpu_replay:
             self.gpu_batcher = GpuBatcher(self.args, self.episodes, self.stepper.device,
                                           forward=self.fleet.send_episodes if self.fleet is not None else None,
-                                          limiter=self.limiter)
+                                          limiter=self.limiter, restore=self.restored)
             self.gpu_batcher.run()
         loss_buf = self.stepper.loss_buf
         self.heads = ['p'] + (['v'] if loss_buf.dvalue is not None else []) + \
@@ -1950,6 +2336,8 @@ class Trainer:
                     if self.stop_event.is_set():
                         return None
                     time.sleep(0.01)
+                if self.restored is not None:
+                    self._finish_restore()
             if self.limiter is not None and (self.fleet is None or batch_cnt % chunk == 0):
                 if not self.limiter.acquire(1 if self.fleet is None else chunk,
                                             lambda: self.stop_event.is_set() or self.update_flag):
@@ -1989,6 +2377,9 @@ class Trainer:
         pending.batch_cnt = batch_cnt
         if self.limiter is not None:
             pending.replay_ratio = self.limiter.end_epoch()
+        if self.replay_files is not None and self.gpu_batcher is not None:
+            # on this thread, between two batches: the sampler state is the one the boundary's weights and priorities go with
+            pending.replay = self.gpu_batcher.snapshot()
         return pending
 
     def _first_host_batch(self):
@@ -2026,6 +2417,8 @@ class Trainer:
         self.batcher.stop()
         if self.gpu_batcher is not None:
             self.gpu_batcher.stop()
+        if self.replay_files is not None:
+            self.replay_files.close()
         if self.stepper is not None:
             self.stepper.stream.synchronize()
         if self.fleet is not None:
