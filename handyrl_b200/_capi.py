@@ -72,7 +72,7 @@ class HrlGemmArgs(C.Structure):
                 ('ep_mean', C.c_void_p), ('ep_rstd', C.c_void_p), ('col_partials', C.c_void_p),
                 ('conv_off', C.c_void_p), ('conv_mode', C.c_int32), ('conv_hw', C.c_int32), ('conv_taps', C.c_int32),
                 ('conv_cin', C.c_int32), ('seg_a', C.c_void_p), ('seg_b', C.c_void_p), ('segments', C.c_int32),
-                ('conv_ones_row', C.c_int32)]
+                ('conv_ones_row', C.c_int32), ('bf16', C.c_int32)]
 
 
 MAX_BOARD_JOBS = 8
@@ -82,7 +82,7 @@ class HrlPackJob(C.Structure):
     _fields_ = [('w', C.c_void_p), ('Cout', C.c_int32), ('Cin', C.c_int32), ('kh', C.c_int32), ('kw', C.c_int32), ('H', C.c_int32),
                 ('W', C.c_int32), ('image_fwd', C.c_void_p), ('fwd_rows', C.c_int32), ('fwd_row0', C.c_int32),
                 ('image_bwd', C.c_void_p), ('bwd_rows', C.c_int32), ('bwd_k0', C.c_int32), ('bias', C.c_void_p),
-                ('bias_cells', C.c_void_p)]
+                ('bias_cells', C.c_void_p), ('bf16', C.c_int32)]
 
 
 class HrlFoldJob(C.Structure):
@@ -171,6 +171,7 @@ SYMBOLS = {
     'hrl_conv_geometry': (C.c_int, [C.c_int32] * 5 + [C.c_void_p]),
     'hrl_conv_pack_floats': (C.c_size_t, [C.c_int32] * 3),
     'hrl_conv_pack': (C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 3),
+    'hrl_conv_pack_bf16': (C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 3),
     'hrl_conv_wgrad_reduce2': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p]),
     'hrl_conv_wgrad_reduce': (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     'hrl_board_pack_many': (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p]),

@@ -8,7 +8,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 OUT = os.path.join(os.path.dirname(HERE), 'libhrl_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
-         '-Xcompiler', '-fPIC', '-shared', '--ptxas-options=-v']
+         '-Xcompiler', '-fPIC', '-shared', '--ptxas-options=-v',
+         '--threads', '0']          # the translation units compile in parallel (two of them are the GEMM's 102 instantiations each)
 
 
 def sources():

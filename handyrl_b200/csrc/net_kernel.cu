@@ -10,6 +10,7 @@
 //
 // All are single-pass, coalesced, fp32, one launch each (the eager PyTorch forms are 6-15 launches with temporaries;
 // a Geister learner step runs them ~3,000 times, which is what made that step launch-bound).
+#include <cuda_bf16.h>
 #include <math.h>
 
 #include <cstring>
@@ -48,6 +49,19 @@ __device__ __forceinline__ void pack_store(float *image, int n_pad, int row, int
     base[(long long)n_pad * 32] = v - hi;
 }
 
+// the same element in a bf16 image (HrlGemmArgs.bf16): image[chunk][row][64 bytes, slot (k % 32) / 8 ^ ((row >> 1) & 3)][k % 8]
+__device__ __forceinline__ void pack_store_bf16(float *image, int n_pad, int row, int k, float v) {
+    const long long chunk = k >> 5;
+    const int j = (k & 31) >> 3, e = k & 7;
+    __nv_bfloat16 *base = reinterpret_cast<__nv_bfloat16 *>(image) + chunk * ((long long)n_pad * 32) + (long long)row * 32;
+    base[((j ^ ((row >> 1) & 3)) << 3) + e] = __float2bfloat16_rn(v);
+}
+
+__device__ __forceinline__ void pack_store_any(float *image, int n_pad, int row, int k, float v, bool bf16) {
+    if (bf16) pack_store_bf16(image, n_pad, row, k, v);
+    else pack_store(image, n_pad, row, k, v);
+}
+
 __device__ __forceinline__ void board_pack_body(const HrlPackJob &j, int block, int nblocks) {
     const int HW = j.H * j.W, Cin = j.Cin, kh = j.kh, kw = j.kw, W = j.W;
     const int fwd_pad = hrl_padded_rows_dev(j.fwd_rows), bwd_pad = hrl_padded_rows_dev(j.bwd_rows);
@@ -57,8 +71,10 @@ __device__ __forceinline__ void board_pack_body(const HrlPackJob &j, int block, 
         const int o = row / HW, q = row - o * HW, i = col / HW, p = col - i * HW;
         const int a = p / W - q / W + kh / 2, b = p % W - q % W + kw / 2;
         const float v = (a >= 0 && a < kh && b >= 0 && b < kw) ? __ldg(j.w + ((long long)(o * Cin + i) * kh + a) * kw + b) : 0.f;
-        if (j.image_fwd) pack_store(j.image_fwd, fwd_pad, j.fwd_row0 + row, col, v);       // rows = output features, reduction = input features
-        if (j.image_bwd) pack_store(j.image_bwd, bwd_pad, col, j.bwd_k0 + row, v);          // rows = input features, reduction = output features
+        // rows = output features, reduction = input features
+        if (j.image_fwd) pack_store_any(j.image_fwd, fwd_pad, j.fwd_row0 + row, col, v, j.bf16);
+        // rows = input features, reduction = output features
+        if (j.image_bwd) pack_store_any(j.image_bwd, bwd_pad, col, j.bwd_k0 + row, v, j.bf16);
     }
     if (j.bias && j.bias_cells)          // the convolution's bias, one copy per cell (the product's per-column bias)
         for (int idx = block * blockDim.x + threadIdx.x; idx < j.Cout * HW; idx += nblocks * blockDim.x) j.bias_cells[idx] = __ldg(j.bias + idx / HW);
@@ -316,14 +332,14 @@ extern "C" size_t hrl_board_pack_floats(int64_t rows, int64_t K) {
 
 // ---- convolutions as implicit products (hrl_gemm_fused conv_mode 1 / 2) -----------------------------------------------
 __global__ void conv_pack_kernel(const float *__restrict__ w, int Cout, int Cin, int taps, float *__restrict__ image_fwd, int fwd_pad,
-                                 float *__restrict__ image_adj, int adj_pad) {
+                                 float *__restrict__ image_adj, int adj_pad, int bf16) {
     const int cin_p = (Cin + 31) / 32 * 32, cout_p = (Cout + 31) / 32 * 32;
     const long long n = (long long)Cout * Cin * taps;
     for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < n; idx += (long long)gridDim.x * blockDim.x) {
         const int t = (int)(idx % taps), ci = (int)((idx / taps) % Cin), co = (int)(idx / ((long long)taps * Cin));
         const float v = __ldg(w + idx);
-        if (image_fwd) pack_store(image_fwd, fwd_pad, co, t * cin_p + ci, v);
-        if (image_adj) pack_store(image_adj, adj_pad, ci, (taps - 1 - t) * cout_p + co, v);      // flipped kernel, channels swapped
+        if (image_fwd) pack_store_any(image_fwd, fwd_pad, co, t * cin_p + ci, v, bf16);
+        if (image_adj) pack_store_any(image_adj, adj_pad, ci, (taps - 1 - t) * cout_p + co, v, bf16);      // flipped kernel, channels swapped
     }
 }
 
@@ -374,15 +390,25 @@ extern "C" size_t hrl_conv_pack_floats(int32_t rows, int32_t channels, int32_t t
     return hrl_board_pack_floats(rows, (int64_t)taps * ((channels + 31) / 32 * 32));
 }
 
-extern "C" int hrl_conv_pack(const float *w, int32_t Cout, int32_t Cin, int32_t kh, int32_t kw, float *image_fwd, float *image_adj,
-                             void *stream) {
+static int conv_pack(const float *w, int32_t Cout, int32_t Cin, int32_t kh, int32_t kw, float *image_fwd, float *image_adj, int bf16,
+                     void *stream) {
     HRL_REQUIRE(w && (image_fwd || image_adj) && Cout > 0 && Cin > 0 && kh > 0 && kw > 0 && (!image_fwd || Cout <= 288) && (!image_adj || Cin <= 288),
                 HRL_ERR_BAD_ARG, "hrl_conv_pack: NULL pointer, bad shape or more than 288 operand rows");
     const long long n = (long long)Cout * Cin * kh * kw;
     conv_pack_kernel<<<grid_for(n), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(w, Cout, Cin, kh * kw, image_fwd, hrl_padded_rows_dev(Cout),
-                                                                                     image_adj, hrl_padded_rows_dev(Cin));
+                                                                                     image_adj, hrl_padded_rows_dev(Cin), bf16);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
+}
+
+extern "C" int hrl_conv_pack(const float *w, int32_t Cout, int32_t Cin, int32_t kh, int32_t kw, float *image_fwd, float *image_adj,
+                             void *stream) {
+    return conv_pack(w, Cout, Cin, kh, kw, image_fwd, image_adj, 0, stream);
+}
+
+extern "C" int hrl_conv_pack_bf16(const float *w, int32_t Cout, int32_t Cin, int32_t kh, int32_t kw, float *image_fwd, float *image_adj,
+                                  void *stream) {
+    return conv_pack(w, Cout, Cin, kh, kw, image_fwd, image_adj, 1, stream);
 }
 
 extern "C" int hrl_conv_wgrad_reduce2(const float *partials, int32_t splits, int32_t ncols, float *dw, float *db, int32_t Cout, int32_t Cin,

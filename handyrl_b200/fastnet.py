@@ -151,7 +151,7 @@ class BoardConv2d(nn.Conv2d):
                 from . import ops
                 if getattr(self, 'tensor_cores', True) and ops.conv_implicit_supported(x, self.weight):
                     # tensor cores: the convolution as an implicit product over (tap, channel), no dense matrix, no im2col
-                    return ops.conv_implicit(x, self.weight, self.bias, wrap)
+                    return ops.conv_implicit(x, self.weight, self.bias, wrap, bf16=_bf16(self))
                 if torch.is_grad_enabled() and not wrap:
                     return _ConvSame.apply(x, self.weight, self.bias)
             return super().forward(x)
@@ -162,7 +162,7 @@ class BoardConv2d(nn.Conv2d):
         if x.is_cuda and x.dtype == torch.float32 and getattr(self, 'tensor_cores', True):
             # tensor cores: dense matrix by one kernel, then forward / input-gradient / weight-gradient as wgmma products
             from . import ops
-            y = ops.board_conv(x, self.weight)
+            y = ops.board_conv(x, self.weight, bf16=_bf16(self))
             if self.bias is not None:
                 y = y + self.bias.view(1, Cout, 1, 1)
             return y
@@ -243,7 +243,7 @@ def _fused_torus_class(cls):
             from . import ops
             if (x.dim() == 4 and x.is_cuda and x.shape[2] * x.shape[3] <= MAX_CELLS and getattr(self.conv, 'tensor_cores', True)
                     and ops.conv_implicit_supported(x, self.conv.weight)):
-                h = ops.conv_implicit(x, self.conv.weight, self.conv.bias, True)      # the wrap lives in the neighbour table
+                h = ops.conv_implicit(x, self.conv.weight, self.conv.bias, True, bf16=_bf16(self.conv))      # the wrap lives in the neighbour table
                 return self.bn(h) if self.bn is not None else h
             return original(self, x)
         _TORUS_CLASSES[cls] = type('Fused' + cls.__name__, (cls,), {'forward': forward, '_hrl_original': cls})
@@ -265,16 +265,22 @@ def _fused_cell_class(cls):
     return _CELL_CLASSES[cls]
 
 
+def _bf16(conv):
+    return getattr(conv, 'tensor_cores', True) == 'bf16'
+
+
 def optimize_small_boards(model, tensor_cores=True):
     """Swap eligible modules to their board-aware subclasses, in place.  Returns how many were swapped.
     tensor_cores=False keeps the dense products on cuBLAS fp32 SIMT kernels (bit-for-bit fp32 summation; the tensor-core
-    3xTF32 products truncate their fp32 accumulator and are ~1e-5 relative per product, see DESIGN.md)."""
+    3xTF32 products truncate their fp32 accumulator and are ~1e-5 relative per product, see DESIGN.md).
+    tensor_cores='bf16' runs the same tensor-core products on bf16 operands (rounded after their fp32 transform, fp32
+    accumulation): faster, ~2^-8 relative per product."""
     n = 0
     for m in model.modules():
         if type(m) in _SWAPS:
             m.__class__ = _SWAPS[type(m)]
             if isinstance(m, BoardConv2d):
-                m.__dict__['tensor_cores'] = bool(tensor_cores)
+                m.__dict__['tensor_cores'] = 'bf16' if tensor_cores == 'bf16' else bool(tensor_cores)
             n += 1
         elif _is_conv_lstm_cell(m) and not hasattr(type(m), '_hrl_original'):
             m.__class__ = _fused_cell_class(type(m))

@@ -510,6 +510,32 @@ def gemm_tf32x3(a, b, bias=None, a_kmajor=True, b_kmajor=True, splits=1, out=Non
     return out
 
 
+def gemm_bf16(a, b, bias=None, a_kmajor=True, b_kmajor=True, splits=1, out=None, partials=None):
+    """C = A_op @ B_op^T on the tensor cores with bf16 operands (hrl_gemm_fused with HrlGemmArgs.bf16): both operands rounded to
+    the nearest bf16, products accumulated in fp32.  Layouts as gemm_tf32x3.  partials: a workspace of
+    hrl_gemm_workspace_floats floats that receives the K-slice partials instead of C (no sum, nothing returned)."""
+    assert a.is_cuda and b.is_cuda and a.dtype == torch.float32 and b.dtype == torch.float32
+    assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
+    M, K = (a.shape[0], a.shape[1]) if a_kmajor else (a.shape[1], a.shape[0])
+    N, Kb = (b.shape[0], b.shape[1]) if b_kmajor else (b.shape[1], b.shape[0])
+    assert K == Kb, (a.shape, b.shape, a_kmajor, b_kmajor)
+    g = _capi.HrlGemmArgs()
+    g.a.ptr, g.a.ld, g.a.kmajor = _ptr(a), a.stride(0), int(a_kmajor)
+    g.b.ptr, g.b.ld, g.b.kmajor = _ptr(b), b.stride(0), int(b_kmajor)
+    g.M, g.N, g.K, g.splits, g.bf16 = M, N, K, splits, 1
+    g.bias = _ptr(bias)
+    if partials is not None:
+        g.C, g.ldc, g.workspace = None, N, _ptr(partials)
+    else:
+        if out is None:
+            out = torch.empty((M, N), dtype=torch.float32, device=a.device)
+        ws = torch.empty(lib().hrl_gemm_workspace_floats(M, N, K, splits), dtype=torch.float32, device=a.device) if splits > 1 else None
+        g.C, g.ldc, g.workspace = _ptr(out), out.stride(0), _ptr(ws)
+    check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
+    _count(2 if (splits > 1 and partials is None) else 1)
+    return out
+
+
 class _LinearTC(torch.autograd.Function):
     """y = x @ w^T with all three products (forward, input gradient, weight gradient) on the tensor cores at fp32-class
     accuracy (hrl_gemm_tf32x3).  The weight gradient reduces over the rows of x (samples): both operands are read
@@ -572,10 +598,11 @@ class _BoardConv(torch.autograd.Function):
     forward   y = x2d @ dense(w)^T            (hrl_board_expand + hrl_gemm_tf32x3)
     backward  dx = dy2d @ dense(w)            (hrl_gemm_tf32x3, the dense matrix read as stored)
               dw = fold(sum_s dy2d_s^T x2d_s) (split-K hrl_gemm_tf32x3 leaving its slice partials, folded AND summed by
-                                               one hrl_board_fold launch: no dense gradient is ever materialised)"""
+                                               one hrl_board_fold launch: no dense gradient is ever materialised)
+    bf16: the same three products as hrl_gemm_fused on bf16 operands (gemm_bf16); the dense matrix and the fold stay fp32."""
 
     @staticmethod
-    def forward(ctx, x, weight):
+    def forward(ctx, x, weight, bf16=False):
         x = x.contiguous()
         weight = weight.contiguous()
         N, Cin, H, W = x.shape
@@ -583,9 +610,10 @@ class _BoardConv(torch.autograd.Function):
         dense = torch.empty((Cout * H * W, Cin * H * W), dtype=torch.float32, device=x.device)
         check(lib().hrl_board_expand(_ptr(weight), _ptr(dense), Cout, Cin, kh, kw, H, W, _stream_ptr()))
         _count()
-        y = gemm_tf32x3(x.view(N, Cin * H * W), dense)
+        y = (gemm_bf16 if bf16 else gemm_tf32x3)(x.view(N, Cin * H * W), dense)
         ctx.save_for_backward(x, dense)
         ctx.dims = (N, Cin, H, W, Cout, kh, kw)
+        ctx.bf16 = bf16
         return y.view(N, Cout, H, W)
 
     @staticmethod
@@ -595,32 +623,38 @@ class _BoardConv(torch.autograd.Function):
         dy2 = dy.contiguous().view(N, Cout * H * W)
         x2 = x.view(N, Cin * H * W)
         dx = dw = None
+        gemm = gemm_bf16 if ctx.bf16 else gemm_tf32x3
         if ctx.needs_input_grad[0]:
-            dx = gemm_tf32x3(dy2, dense, b_kmajor=False).view(N, Cin, H, W)
+            dx = gemm(dy2, dense, b_kmajor=False).view(N, Cin, H, W)
         if ctx.needs_input_grad[1]:
             rows, cols = Cout * H * W, Cin * H * W
             tiles = ((rows + 127) // 128) * ((cols + 287) // 288)
             splits = lib().hrl_gemm_effective_splits(N, max(1, min(N // 64, 132 // tiles)))
             dw = torch.empty((Cout, Cin, kh, kw), dtype=torch.float32, device=dy.device)
-            if splits > 1:
+            if splits > 1 and ctx.bf16:
+                ws = torch.empty(splits * rows * cols, dtype=torch.float32, device=dy.device)
+                gemm_bf16(dy2, x2, a_kmajor=False, b_kmajor=False, splits=splits, partials=ws)
+                _count(-1)
+            elif splits > 1:
                 ws = torch.empty(splits * rows * cols, dtype=torch.float32, device=dy.device)
                 check(lib().hrl_gemm_tf32x3(_ptr(dy2), dy2.stride(0), 0, _ptr(x2), x2.stride(0), 0, None, None, cols, rows, cols, N,
                                             splits, _ptr(ws), _stream_ptr()))
             else:
-                ws = gemm_tf32x3(dy2, x2, a_kmajor=False, b_kmajor=False).view(-1)
+                ws = gemm(dy2, x2, a_kmajor=False, b_kmajor=False).view(-1)
                 _count(-1)
             check(lib().hrl_board_fold(_ptr(ws), splits, rows * cols, _ptr(dw), Cout, Cin, kh, kw, H, W, _stream_ptr()))
             _count(2)
-        return dx, dw
+        return dx, dw, None
 
 
-def board_conv(x, weight):
-    return _BoardConv.apply(x, weight)
+def board_conv(x, weight, bf16=False):
+    """bf16: the products on bf16 operands (fastnet.optimize_small_boards(model, tensor_cores='bf16'))."""
+    return _BoardConv.apply(x, weight, bool(bf16))
 
 
 # ---- stride-1 "same" / wrap-around convolutions as implicit tensor-core products (hrl_gemm_fused conv_mode 1 / 2) -----------
 _CONV_TABLES = {}        # (H, W, kh, kw, wrap, device) -> int16 neighbour-offset table on the device
-_CONV_IMAGES = {}        # (weight ptr, shape) -> [forward image, adjoint image, generation they were packed in]
+_CONV_IMAGES = {}        # (weight ptr, shape, bf16) -> [forward image, adjoint image, generation they were packed in, weight ref]
 _CONV_GENERATION = [0]   # bumped whenever the parameters may have changed (fastnet.new_step)
 
 
@@ -639,21 +673,24 @@ def _conv_table(H, W, kh, kw, wrap, device):
     return t
 
 
-def _conv_images(w):
+def _conv_images(w, bf16=False):
     """The weight's packed forward / adjoint operand images, re-packed once per parameter generation.  (Keyed by address AND
-    identity: a freed model's weight address can be handed to another tensor of the same shape.)"""
+    identity: a freed model's weight address can be handed to another tensor of the same shape; and by precision: bf16 images
+    (hrl_conv_pack_bf16, a quarter of the size) for the bf16 products.)"""
     import weakref
     Cout, Cin, kh, kw = w.shape
-    key = (w.data_ptr(), tuple(w.shape))
+    key = (w.data_ptr(), tuple(w.shape), bool(bf16))
     ent = _CONV_IMAGES.get(key)
     if ent is None or ent[3]() is not w:
         if ent is None:
-            z = lambda rows, ch: torch.zeros(lib().hrl_conv_pack_floats(rows, ch, kh * kw), dtype=torch.float32, device=w.device)
+            z = lambda rows, ch: torch.zeros(lib().hrl_conv_pack_floats(rows, ch, kh * kw) // (4 if bf16 else 1), dtype=torch.float32,
+                                             device=w.device)
             ent = _CONV_IMAGES[key] = [z(Cout, Cin), z(Cin, Cout), None, None]
         ent[2], ent[3] = None, weakref.ref(w)
     gen = (_CONV_GENERATION[0], w._version)
     if ent[2] != gen:
-        check(lib().hrl_conv_pack(_ptr(w), Cout, Cin, kh, kw, _ptr(ent[0]), _ptr(ent[1]), _stream_ptr()))
+        pack = lib().hrl_conv_pack_bf16 if bf16 else lib().hrl_conv_pack
+        check(pack(_ptr(w), Cout, Cin, kh, kw, _ptr(ent[0]), _ptr(ent[1]), _stream_ptr()))
         _count()
         ent[2] = gen
     return ent[0], ent[1]
@@ -675,7 +712,7 @@ def _pixels(t):
     return t, t.permute(0, 2, 3, 1).reshape(-1, t.shape[1])
 
 
-def _conv_product(pix, image, rows, cin, taps, table, hw, bias=None):
+def _conv_product(pix, image, rows, cin, taps, table, hw, bias=None, bf16=False):
     """out[pixel][row] = sum over (tap, channel) of pix[neighbour(pixel, tap)][channel] * image[row][tap, channel]"""
     M = pix.shape[0]
     out = torch.empty((M, rows), dtype=torch.float32, device=pix.device)
@@ -685,6 +722,7 @@ def _conv_product(pix, image, rows, cin, taps, table, hw, bias=None):
     g.bias, g.C, g.ldc = _ptr(bias), _ptr(out), rows
     g.M, g.N, g.K, g.splits = M, rows, taps * ((cin + 31) // 32 * 32), 1
     g.conv_off, g.conv_mode, g.conv_hw, g.conv_taps, g.conv_cin = _ptr(table), 1, hw, taps, cin
+    g.bf16 = int(bf16)
     check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
     _count()
     return out
@@ -748,6 +786,7 @@ def _flush_weight_gradient(job):
         g.conv_off, g.conv_mode, g.conv_hw, g.conv_taps, g.conv_cin = _ptr(table), 2, hw, taps, Cin
         g.seg_a, g.seg_b = C.cast(seg_a, C.c_void_p), C.cast(seg_b, C.c_void_p)
         g.segments, g.conv_ones_row = n, int(ones)
+        g.bf16 = int(job['bf16'])
         check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
         for t, shape in ((w, w.shape), (b, None)):
             if t is not None and t.grad is None:
@@ -760,15 +799,15 @@ def _flush_weight_gradient(job):
 
 class _ConvImplicit(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, w, b, wrap):
+    def forward(ctx, x, w, b, wrap, bf16=False):
         N, Cin, H, W = x.shape
         Cout, _, kh, kw = w.shape
         table = _conv_table(H, W, kh, kw, wrap, x.device)
-        fwd, _ = _conv_images(w)
+        fwd, _ = _conv_images(w, bf16)
         xl, x2 = _pixels(x)
-        y2 = _conv_product(x2, fwd, Cout, Cin, kh * kw, table, H * W, bias=b)
+        y2 = _conv_product(x2, fwd, Cout, Cin, kh * kw, table, H * W, bias=b, bf16=bf16)
         ctx.save_for_backward(xl, w)
-        ctx.wrap, ctx.has_bias = wrap, b is not None
+        ctx.wrap, ctx.has_bias, ctx.bf16 = wrap, b is not None, bf16
         ctx.params = (w, b)             # the Parameter objects themselves (their .grad is what a deferred flush accumulates into)
         return y2.view(N, H, W, Cout).permute(0, 3, 1, 2)           # logical NCHW, channels-last in memory
 
@@ -783,14 +822,15 @@ class _ConvImplicit(torch.autograd.Function):
         dx = dw = db = None
         pw, pb = ctx.params
         if ctx.needs_input_grad[0]:
-            _, adj = _conv_images(pw)           # (the object forward saw: the image cache checks identity)
-            dx = _conv_product(dy2, adj, Cin, Cout, taps, table, H * W).view(N, H, W, Cin).permute(0, 3, 1, 2)
+            _, adj = _conv_images(pw, ctx.bf16)           # (the object forward saw: the image cache checks identity)
+            dx = _conv_product(dy2, adj, Cin, Cout, taps, table, H * W, bf16=ctx.bf16).view(N, H, W, Cin).permute(0, 3, 1, 2)
         if (ctx.needs_input_grad[1] and _DEFER['on'] and pw.is_leaf and (pb is None or (pb.is_leaf and ctx.needs_input_grad[2]))
                 and (pw.grad is None or pw.grad.is_contiguous())):
-            job = _DEFER['pending'].setdefault(pw.data_ptr(), {'w': pw, 'b': pb, 'pairs': [], 'geom': (table, H * W)})
+            job = _DEFER['pending'].setdefault((pw.data_ptr(), ctx.bf16),
+                                               {'w': pw, 'b': pb, 'pairs': [], 'geom': (table, H * W), 'bf16': ctx.bf16})
             if not job['pairs'] or job['pairs'][0][0].shape[0] == dy2.shape[0]:      # (pairs of one product cover the same pixels)
                 job['pairs'].append((dy2, xl.permute(0, 2, 3, 1).reshape(-1, Cin)))
-                return dx, None, None, None
+                return dx, None, None, None, None
         if ctx.needs_input_grad[1]:
             x2 = xl.permute(0, 2, 3, 1).reshape(-1, Cin)
             pixels, cols = x2.shape[0], taps * Cin
@@ -803,19 +843,21 @@ class _ConvImplicit(torch.autograd.Function):
             g.C, g.ldc = (None if s > 1 else _ptr(ws)), cols
             g.M, g.N, g.K, g.splits, g.workspace = Cout, cols, pixels, s, (_ptr(ws) if s > 1 else None)
             g.conv_off, g.conv_mode, g.conv_hw, g.conv_taps, g.conv_cin = _ptr(table), 2, H * W, taps, Cin
+            g.bf16 = int(ctx.bf16)
             check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
             dw = torch.empty_like(w, memory_format=torch.contiguous_format)
             check(lib().hrl_conv_wgrad_reduce(_ptr(ws), s, _ptr(dw), Cout, Cin, taps, _stream_ptr()))
             _count(2)
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = dy2.sum(0)
-        return dx, dw, db, None
+        return dx, dw, db, None, None
 
 
-def conv_implicit(x, w, b=None, wrap=False):
+def conv_implicit(x, w, b=None, wrap=False, bf16=False):
     """Stride-1 convolution with `same` zero padding (wrap=False) or wrap-around padding on both axes (wrap=True) of a board of at most
-    256 cells, forward / input gradient / weight gradient on the tensor cores at fp32-class accuracy (3xTF32)."""
-    return _ConvImplicit.apply(x, w, b, bool(wrap))
+    256 cells, forward / input gradient / weight gradient on the tensor cores at fp32-class accuracy (3xTF32), or with bf16=True on
+    bf16 operands (rounded to nearest even, fp32 accumulation; bias and bias gradient stay fp32)."""
+    return _ConvImplicit.apply(x, w, b, bool(wrap), bool(bf16))
 
 
 def _is_channels_last(t):

@@ -59,9 +59,12 @@ class FusedBoardNet:
     (CUDA-graph friendly).  The module keeps owning the parameters and BatchNorm buffers; this object only reads them and
     writes their gradients."""
 
-    def __init__(self, model, M, device):
+    def __init__(self, model, M, device, bf16=False):
         assert supports(model)
         self.model, self.M, self.device = model, int(M), device
+        # bf16: every product runs on bf16 operands (HrlGemmArgs.bf16, fp32 accumulation) with bf16 weight images; the heads,
+        # BatchNorm finalisation and fold kernels stay fp32
+        self.bf16 = bool(bf16)
         st = model.stem
         self.planes, self.width = st.in_channels, st.out_channels
         self.pmaps = model.p_squeeze.out_channels
@@ -78,9 +81,9 @@ class FusedBoardNet:
         self.tiles = (self.M + 127) // 128
         f = dict(dtype=torch.float32, device=device)
         M_, D = self.M, self.D
-        # weights as packed B-operand images (pre-split TF32 hi/lo, pre-swizzled, one bulk copy per stage): `f` for the
-        # forward product (rows = output features), `b` for the input-gradient product (rows = input features)
-        img = lambda rows, K: torch.zeros(lib().hrl_board_pack_floats(rows, K), **f)
+        # weights as packed B-operand images (pre-split TF32 hi/lo, or bf16 in a quarter of the bytes; pre-swizzled, one bulk copy
+        # per stage): `f` for the forward product (rows = output features), `b` for the input-gradient product (rows = input features)
+        img = lambda rows, K: torch.zeros(lib().hrl_board_pack_floats(rows, K) // (4 if self.bf16 else 1), **f)
         self.W0f = img(D, self.K0)
         self.Wf = [img(D, D) for _ in range(self.depth)]
         self.Wb = [img(D, D) for _ in range(self.depth)]
@@ -129,6 +132,7 @@ class FusedBoardNet:
         g.M, g.N, g.K = (self.M if M is None else M), N, K
         g.splits = splits
         g.epilogue = GEMM_EPILOGUES[epilogue]
+        g.bf16 = int(self.bf16)
         g.workspace = _ptr(ws) if splits > 1 else None
         if epilogue in ('stats', 'mask_stats'):
             g.col_partials = _ptr(self.cp)
@@ -159,6 +163,7 @@ class FusedBoardNet:
                 j.image_fwd, j.fwd_rows, j.fwd_row0 = _ptr(kw.get('fwd')), kw.get('fwd_rows', 0), kw.get('fwd_row0', 0)
                 j.image_bwd, j.bwd_rows, j.bwd_k0 = _ptr(kw.get('bwd')), kw.get('bwd_rows', 0), kw.get('bwd_k0', 0)
                 j.bias, j.bias_cells = _ptr(kw.get('bias')), _ptr(kw.get('bias_cells'))
+                j.bf16 = int(self.bf16)
             check(lib().hrl_board_pack_many_pivot(C.byref(arr), len(chunk), pivots([b.running_mean for b, _ in piv]),
                                                   pivots([b.running_var for b, _ in piv]), pivots([st['mean'] for _, st in piv]),
                                                   len(piv), self.width, self.cells, _stream_ptr()))

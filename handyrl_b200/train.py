@@ -844,8 +844,22 @@ def attach_pickle_cache(model, blob):
 _Handoff = collections.namedtuple('_Handoff', 'name snap copies after room', defaults=(None, None))
 
 
+def tensor_core_mode(value):
+    """train_args['tensor_cores'] -> the precision of the net's products on this library's kernels: True (the default: 3xTF32
+    tensor-core products, fp32-class accuracy), False (fp32 SIMT kernels) or 'bf16' (tensor-core products on bf16 operands,
+    rounded after their fp32 transform, fp32 accumulation).  Any other value reads as bool(value)."""
+    if isinstance(value, str) and value == 'bf16':
+        return 'bf16'
+    return bool(value)
+
+
 class LearnerStep:
     """One replay batch -> one optimiser step.
+
+    tensor_cores (default: train_args['tensor_cores'], True): the precision of the net's products, tensor_core_mode(); the
+    step runs the mode in `self.tensor_cores` (True, False or 'bf16').  'bf16' covers every product of the fused tower and of
+    the rewritten small-board convolutions, in the step and in validation passes alike; layers left on cuDNN / cuBLAS keep
+    following allow_tf32.
 
     step(packed):  ONE H2D copy of the packed pinned batch -> [CUDA graph: net forward ->
     fused loss fwd+bwd kernel -> net backward -> (all-reduce SUM) -> clip + Adam].
@@ -935,10 +949,10 @@ class LearnerStep:
         # implicit-GEMM kernels on the tiny boards of these games; NHWC + autotune is a pure layout choice
         # tiny boards: convolutions as one SGEMM, BatchNorm as fused reductions (fastnet.py); NCHW stays as is
         self.engine = None          # hand-scheduled fused forward/backward for recognised architectures (tower.py)
-        # train_args['tensor_cores'] = False: the small-board dense products stay on fp32 SIMT kernels (strict fp32 summation)
-        if tensor_cores is None:
-            tensor_cores = bool(args.get('tensor_cores', True))
-        self.tensor_cores = tensor_cores
+        # train_args['tensor_cores'] = False: the small-board dense products stay on fp32 SIMT kernels (strict fp32 summation);
+        # 'bf16': the same tensor-core products on bf16 operands (tensor_core_mode)
+        self.tensor_cores = tensor_core_mode(args.get('tensor_cores', True) if tensor_cores is None else tensor_cores)
+        tensor_cores = self.tensor_cores
         fused_tower = fused_tower and tensor_cores
         self.rewritten = fastnet.optimize_small_boards(self.model, tensor_cores=tensor_cores) if small_boards else 0
         if self.rewritten and channels_last:
@@ -1032,7 +1046,7 @@ class LearnerStep:
         from . import tower
         if fused_tower and small_boards and self.hidden0 is None and tower.supports(self.model) and \
                 torch.is_tensor(example_batch['observation']) and example_batch['observation'].shape[-2] * example_batch['observation'].shape[-1] <= 16:
-            self.engine = tower.FusedBoardNet(self.model, B * T * Pa, self.device)
+            self.engine = tower.FusedBoardNet(self.model, B * T * Pa, self.device, bf16=tensor_cores == 'bf16')
         self.loss_buf = None
         self.last_losses = torch.zeros(NUM_LOSS, device=self.device)
         self.accum = torch.zeros(n_sums, dtype=torch.float64, device=self.device)

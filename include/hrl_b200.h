@@ -370,6 +370,13 @@ typedef struct HrlGemmArgs {
     const float *const *seg_a;
     const float *const *seg_b;
     int32_t segments, conv_ones_row;
+    /* bf16 != 0: the product on bf16 operands (0 = 3xTF32, as hrl_gemm_tf32x3).  Each operand element goes through its
+     * transform in fp32 (fmaf, optional ReLU) and is then rounded to the nearest bf16, ties to even; the products of the
+     * rounded operands are exact in fp32 and accumulate in fp32 registers (wgmma .f32.bf16.bf16, k16).  Bias, epilogues,
+     * statistics sums, split-K partials and the ones row are fp32 as in the 3xTF32 form.  Relative error of an output
+     * ~2^-8 of sum_k |a||b| (each operand within 2^-9 relative), not the ~1e-6 of 3xTF32.  A packed B must then be a bf16
+     * image: hrl_board_pack_many / _pivot with HrlPackJob.bf16, or hrl_conv_pack_bf16. */
+    int32_t bf16;
 } HrlGemmArgs;
 
 #define HRL_CONV_OUTSIDE (-32768)
@@ -379,6 +386,10 @@ int hrl_conv_geometry(int32_t H, int32_t W, int32_t kh, int32_t kw, int32_t wrap
  * and adjoint (rows = Cin, reduction = flipped tap, Cout padded to 32).  Either may be NULL. */
 size_t hrl_conv_pack_floats(int32_t rows, int32_t channels, int32_t taps);
 int hrl_conv_pack(const float *w, int32_t Cout, int32_t Cin, int32_t kh, int32_t kw, float *image_fwd, float *image_adj, void *stream);
+/* The same images for HrlGemmArgs.bf16 products: bf16 weights (round to nearest even), [chunk][n_pad rows][64 bytes,
+ * SWIZZLE_64B: 16-byte slot j of row r at j ^ ((r >> 1) & 3)].  Each takes hrl_conv_pack_floats(...) / 4 floats. */
+int hrl_conv_pack_bf16(const float *w, int32_t Cout, int32_t Cin, int32_t kh, int32_t kw, float *image_fwd, float *image_adj,
+                       void *stream);
 /* dw[co][ci][a][b] = sum over slices of partials[s][co][(a*kw+b)*Cin + ci]  (fixed order) */
 int hrl_conv_wgrad_reduce(const float *partials, int32_t splits, float *dw, int32_t Cout, int32_t Cin, int32_t taps, void *stream);
 /* the same over partial rows of `ncols` floats (taps*Cin, or taps*Cin + 1 with the ones row: column taps*Cin -> db[co], may be NULL);
@@ -456,6 +467,9 @@ typedef struct HrlPackJob {
     int32_t bwd_rows, bwd_k0;
     const float *bias;
     float *bias_cells;
+    /* != 0: write the images of HrlGemmArgs.bf16 products instead -- bf16 weights (round to nearest even), [chunk][n_pad rows]
+     * [64 bytes, SWIZZLE_64B: 16-byte slot j of row r at j ^ ((r >> 1) & 3)], hrl_board_pack_floats(...) / 4 floats */
+    int32_t bf16;
 } HrlPackJob;
 typedef struct HrlFoldJob {
     const float *ddense;
