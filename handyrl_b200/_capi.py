@@ -87,7 +87,8 @@ class HrlPackJob(C.Structure):
 
 class HrlFoldJob(C.Structure):
     _fields_ = [('ddense', C.c_void_p), ('splits', C.c_int32), ('split_stride', C.c_int64), ('dw', C.c_void_p),
-                ('Cout', C.c_int32), ('Cin', C.c_int32), ('kh', C.c_int32), ('kw', C.c_int32), ('H', C.c_int32), ('W', C.c_int32)]
+                ('Cout', C.c_int32), ('Cin', C.c_int32), ('kh', C.c_int32), ('kw', C.c_int32), ('H', C.c_int32), ('W', C.c_int32),
+                ('accumulate', C.c_int32)]
 
 
 class HrlWindow(C.Structure):
@@ -144,6 +145,7 @@ SYMBOLS = {
     'hrl_weight_ema': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_int32, C.c_void_p]),
     'hrl_weight_ema_guarded': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_int32, C.c_void_p,
                                          C.c_void_p]),
+    'hrl_sum_rows': (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),
     'hrl_peer_allreduce_sumsq': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int64,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'hrl_bn_workspace_floats': (C.c_size_t, [C.c_int64, C.c_int32, C.c_int32, C.c_int32]),
@@ -160,9 +162,13 @@ SYMBOLS = {
     'hrl_bn_finalize_fwd': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_float] +
                             [C.c_void_p] * 8),
     'hrl_bn_finalize_bwd': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 9),
+    'hrl_bn_finalize_bwd_accumulate': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 8 +
+                                       [C.c_int32, C.c_void_p]),
     'hrl_heads_num_blocks': (C.c_int32, [C.c_int64]),
     'hrl_heads_fwd': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_int32] * 5 + [C.c_float] + [C.c_void_p] * 7),
     'hrl_heads_bwd': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_int32] * 5 + [C.c_float] + [C.c_void_p] * 16),
+    'hrl_heads_bwd_accumulate': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_int32] * 5 + [C.c_float] + [C.c_void_p] * 15 +
+                                 [C.c_int32, C.c_void_p]),
     'hrl_gemm_set_debug': (None, [C.c_int]),
     'hrl_gemm_padded_rows': (C.c_int32, [C.c_int64]),
     'hrl_board_pack_floats': (C.c_size_t, [C.c_int64, C.c_int64]),

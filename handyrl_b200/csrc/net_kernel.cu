@@ -183,7 +183,8 @@ __global__ void board_fold_kernel(const FoldJobs jobs) {
                 s += slab[(qy * W + qx) * cols + i * HW + py * W + px];
             }
         }
-        dw[((long long)(o * Cin + i) * kh + a) * kw + b] = s;
+        float *d = dw + ((long long)(o * Cin + i) * kh + a) * kw + b;
+        *d = J.accumulate ? *d + s : s;
     }
 }
 

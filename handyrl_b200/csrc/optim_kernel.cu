@@ -213,6 +213,15 @@ __global__ void __launch_bounds__(kOptThreads) step_commit_kernel(const int32_t 
         for (int64_t i = (n16 << 4) + threadIdx.x; i < nbytes; i += blockDim.x) state[i] = saved[i];
 }
 
+// the loss-pass sums of a gradient-accumulation step: out[j] = fp32(sum over rows i = 0..k-1, in order, of (double)rows[i*ld + j])
+__global__ void sum_rows_kernel(const float *__restrict__ rows, int k, int64_t ld, int n, float *__restrict__ out) {
+    for (int j = threadIdx.x; j < n; j += blockDim.x) {
+        double s = 0.0;
+        for (int i = 0; i < k; i++) s += (double)rows[(int64_t)i * ld + j];
+        out[j] = (float)s;
+    }
+}
+
 // moving average of the learner's state after the optimiser step: a <- fmaf(w, x - a, a),
 // w = 1 - decay once seeded, else max(1 - decay, 1 / t) with t = *step_p.  w == 1 (the first step)
 // stores x itself: fmaf(1, x - a, a) would round x - a.  Purely elementwise, so every element sees
@@ -374,4 +383,11 @@ extern "C" int hrl_weight_ema(float *avg, const float *state, int64_t n, const i
 extern "C" int hrl_weight_ema_guarded(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
                                       const int32_t *skip, void *stream) {
     return hrl::weight_ema<true>("hrl_weight_ema_guarded", avg, state, n, step, decay, seeded, skip, stream);
+}
+
+extern "C" int hrl_sum_rows(const float *rows, int32_t k, int64_t ld, int32_t n, float *out, void *stream) {
+    HRL_REQUIRE(rows && out && k >= 1 && n >= 1 && ld >= n, HRL_ERR_BAD_ARG, "hrl_sum_rows: NULL pointer or bad shape");
+    hrl::sum_rows_kernel<<<1, 128, 0, reinterpret_cast<cudaStream_t>(stream)>>>(rows, k, ld, n, out);
+    HRL_CUDA_CHECK(cudaGetLastError());
+    return HRL_OK;
 }

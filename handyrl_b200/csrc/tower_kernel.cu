@@ -7,7 +7,8 @@
 //                         (samples x C*HW) activation matrix, the constants the next product's operand transform applies:
 //                         scale = gamma*rstd, shift = beta - mean*scale (plus mean and rstd for the backward)
 //   hrl_bn_finalize_bwd   column sums of dZ and dZ*xhat (epilogue MASK_STATS) -> dgamma, dbeta and the per-column constants
-//                         of dY = dZ*p + Y*q + r (the BatchNorm backward as an operand transform)
+//                         of dY = dZ*p + Y*q + r (the BatchNorm backward as an operand transform); the _accumulate form adds
+//                         dgamma / dbeta to what they hold (micro-batches after the first of a gradient-accumulation step)
 //   hrl_heads_fwd / _bwd  the 1x1-conv "squeeze" outputs (already a product) -> LeakyReLU -> bias-free Linear policy /
 //                         tanh value / return heads, and their backward including the parameter gradients
 #include <math.h>
@@ -69,7 +70,7 @@ __global__ void __launch_bounds__(256) bn_tower_finalize_bwd_kernel(const float 
                                                                     const float *__restrict__ gamma, const float *__restrict__ mean_col,
                                                                     const float *__restrict__ rstd_col, float *__restrict__ dgamma,
                                                                     float *__restrict__ dbeta, float *__restrict__ p_col,
-                                                                    float *__restrict__ q_col, float *__restrict__ r_col) {
+                                                                    float *__restrict__ q_col, float *__restrict__ r_col, int accumulate) {
     const int c = blockIdx.x, N = C * HW;
     double s = 0.0, q = 0.0;
     for (int i = threadIdx.x; i < tiles * HW; i += blockDim.x) {
@@ -79,8 +80,8 @@ __global__ void __launch_bounds__(256) bn_tower_finalize_bwd_kernel(const float 
     }
     block_sum2(s, q);
     if (threadIdx.x == 0) {
-        dbeta[c] = (float)s;                      // sum dZ
-        if (dgamma) dgamma[c] = (float)q;         // sum dZ * xhat
+        dbeta[c] = accumulate ? dbeta[c] + (float)s : (float)s;                          // sum dZ
+        if (dgamma) dgamma[c] = accumulate ? dgamma[c] + (float)q : (float)q;            // sum dZ * xhat
     }
     if (gamma != nullptr) {
         const float mu = mean_col[c * HW], rs = rstd_col[c * HW];
@@ -205,7 +206,8 @@ __global__ void __launch_bounds__(128) heads_bwd_kernel(const float *__restrict_
     }
 }
 
-// out[i] = sum over blocks of partials[block][i] in a fixed order, scattered to up to 8 destination ranges
+// out[i] = sum over blocks of partials[block][i] in a fixed order, scattered to up to 8 destination ranges (accumulate: added to
+// what the ranges hold, the fp64 sum rounded to fp32 first)
 struct ScatterPlan {
     float *dst[8];
     int begin[8];       // first index of the range in the partial vector; range k covers [begin[k], begin[k+1])
@@ -213,14 +215,15 @@ struct ScatterPlan {
     int total;
 };
 
-__global__ void heads_fold_kernel(const float *__restrict__ partials, int blocks, ScatterPlan plan) {
+__global__ void heads_fold_kernel(const float *__restrict__ partials, int blocks, ScatterPlan plan, int accumulate) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= plan.total) return;
     double s = 0.0;
     for (int b = 0; b < blocks; b++) s += (double)partials[(long long)b * plan.total + i];
     int k = 0;
     while (k + 1 < plan.n && i >= plan.begin[k + 1]) k++;
-    plan.dst[k][i - plan.begin[k]] = (float)s;
+    float *d = plan.dst[k] + (i - plan.begin[k]);
+    *d = accumulate ? *d + (float)s : (float)s;
 }
 
 }  // namespace hrl
@@ -241,16 +244,24 @@ extern "C" int hrl_bn_finalize_fwd(const float *col_partials, int32_t tiles, int
     return HRL_OK;
 }
 
-extern "C" int hrl_bn_finalize_bwd(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows, const float *gamma,
-                                   const float *mean_col, const float *rstd_col, float *dgamma, float *dbeta, float *p_col, float *q_col,
-                                   float *r_col, void *stream) {
+extern "C" int hrl_bn_finalize_bwd_accumulate(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows,
+                                              const float *gamma, const float *mean_col, const float *rstd_col, float *dgamma, float *dbeta,
+                                              float *p_col, float *q_col, float *r_col, int32_t accumulate, void *stream) {
     HRL_REQUIRE(col_partials && dbeta && tiles > 0 && C > 0 && HW > 0 && rows > 0, HRL_ERR_BAD_ARG, "hrl_bn_finalize_bwd: NULL pointer or bad shape");
     HRL_REQUIRE(gamma == nullptr || (mean_col && rstd_col && dgamma && p_col && q_col && r_col), HRL_ERR_BAD_ARG,
                 "hrl_bn_finalize_bwd: with gamma, every BatchNorm output is required");
     bn_tower_finalize_bwd_kernel<<<C, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(col_partials, tiles, C, HW, (double)rows * HW, gamma,
-                                                                                       mean_col, rstd_col, dgamma, dbeta, p_col, q_col, r_col);
+                                                                                       mean_col, rstd_col, dgamma, dbeta, p_col, q_col, r_col,
+                                                                                       accumulate ? 1 : 0);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
+}
+
+extern "C" int hrl_bn_finalize_bwd(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows, const float *gamma,
+                                   const float *mean_col, const float *rstd_col, float *dgamma, float *dbeta, float *p_col, float *q_col,
+                                   float *r_col, void *stream) {
+    return hrl_bn_finalize_bwd_accumulate(col_partials, tiles, C, HW, rows, gamma, mean_col, rstd_col, dgamma, dbeta, p_col, q_col, r_col, 0,
+                                          stream);
 }
 
 static int heads_dims(int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps, int32_t A, HeadsDims &d) {
@@ -274,10 +285,11 @@ extern "C" int hrl_heads_fwd(const float *pre, int64_t ld, int64_t M, int32_t ce
     return HRL_OK;
 }
 
-extern "C" int hrl_heads_bwd(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps, int32_t A,
-                             float slope, const float *Wp, const float *Wv, const float *Wr, const float *value, const float *dpolicy,
-                             const float *dvalue, const float *dret, float *dpre, float *dWp, float *dWv, float *dWr, float *dbias_p,
-                             float *dbias_v, float *dbias_r, float *workspace, void *stream_) {
+extern "C" int hrl_heads_bwd_accumulate(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps,
+                                        int32_t A, float slope, const float *Wp, const float *Wv, const float *Wr, const float *value,
+                                        const float *dpolicy, const float *dvalue, const float *dret, float *dpre, float *dWp, float *dWv,
+                                        float *dWr, float *dbias_p, float *dbias_v, float *dbias_r, float *workspace, int32_t accumulate,
+                                        void *stream_) {
     HeadsDims d;
     if (int e = heads_dims(cells, pmaps, vmaps, rmaps, A, d)) return e;
     HRL_REQUIRE(pre && Wp && dpolicy && dpre && dWp && dbias_p && workspace && M > 0 && (!vmaps || (Wv && value && dvalue && dWv && dbias_v)) &&
@@ -301,7 +313,15 @@ extern "C" int hrl_heads_bwd(const float *pre, int64_t ld, int64_t M, int32_t ce
     if (rmaps) { plan.dst[k] = dbias_r; plan.begin[k++] = at; at += rmaps; }
     plan.n = k;
     plan.total = at;
-    heads_fold_kernel<<<(at + 127) / 128, 128, 0, stream>>>(workspace, blocks, plan);
+    heads_fold_kernel<<<(at + 127) / 128, 128, 0, stream>>>(workspace, blocks, plan, accumulate ? 1 : 0);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
+}
+
+extern "C" int hrl_heads_bwd(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps, int32_t A,
+                             float slope, const float *Wp, const float *Wv, const float *Wr, const float *value, const float *dpolicy,
+                             const float *dvalue, const float *dret, float *dpre, float *dWp, float *dWv, float *dWr, float *dbias_p,
+                             float *dbias_v, float *dbias_r, float *workspace, void *stream) {
+    return hrl_heads_bwd_accumulate(pre, ld, M, cells, pmaps, vmaps, rmaps, A, slope, Wp, Wv, Wr, value, dpolicy, dvalue, dret, dpre, dWp, dWv,
+                                    dWr, dbias_p, dbias_v, dbias_r, workspace, 0, stream);
 }

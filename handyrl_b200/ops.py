@@ -416,6 +416,19 @@ def weight_ema_update(avg, state_f32, step_count, decay, seeded, skip=None):
     _count()
 
 
+def sum_rows(rows, n, out):
+    """out[:n] = the sum of the rows of the (k, ld) float32 CUDA tensor `rows` over their first n columns, in row order in
+    float64 and rounded once (hrl_sum_rows: the loss-pass sums of a gradient-accumulation step into the bucket tail).  One
+    launch, bit-reproducible."""
+    for t, name in ((rows, 'rows'), (out, 'out')):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.stride(-1) == 1):
+            raise _capi.HrlError('handyrl_b200: %s must be a float32 CUDA tensor with unit column stride' % name)
+    if rows.dim() != 2 or not 1 <= n <= rows.shape[1] or out.numel() < n:
+        raise _capi.HrlError('handyrl_b200: sum_rows needs (k, ld) rows with ld >= n and n <= out.numel()')
+    check(lib().hrl_sum_rows(_ptr(rows), rows.shape[0], rows.stride(0), int(n), _ptr(out), _stream_ptr()))
+    _count()
+
+
 def step_commit(skip, tail, accum, skip_count, state=None, saved=None):
     """What follows a guarded optimiser step (hrl_step_commit, one launch reading the device flag `skip`): when the step was
     accepted, accum[:tail.numel()] += tail (float32 sums into the float64 accumulator, as ATen's add_ does); when it was

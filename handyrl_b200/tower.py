@@ -169,8 +169,9 @@ class FusedBoardNet:
                                                   len(piv), self.width, self.cells, _stream_ptr()))
             _count()
 
-    def _fold_all(self):
-        """Every weight-gradient product of the backward pass onto its convolution's taps, in one launch."""
+    def _fold_all(self, accumulate):
+        """Every weight-gradient product of the backward pass onto its convolution's taps, in one launch (added to the
+        gradients when `accumulate`)."""
         jobs, self.fold_jobs = self.fold_jobs, []
         for i in range(0, len(jobs), MAX_BOARD_JOBS):
             chunk = jobs[i:i + MAX_BOARD_JOBS]
@@ -178,6 +179,7 @@ class FusedBoardNet:
             for j, (src, splits, stride, grad) in zip(arr, chunk):
                 j.ddense, j.splits, j.split_stride, j.dw = _ptr(src), splits, stride, _ptr(grad)
                 (j.Cout, j.Cin, j.kh, j.kw), j.H, j.W = grad.shape, self.H, self.W
+                j.accumulate = int(accumulate)
             check(lib().hrl_board_fold_many(C.byref(arr), len(chunk), _stream_ptr()))
             _count()
 
@@ -238,8 +240,9 @@ class FusedBoardNet:
         return out
 
     # ------------------------------------------------------------------ backward
-    def backward(self, dpolicy, dvalue, dreturn=None):
-        """Gradients of every parameter from the output gradients, written into param.grad (which must exist)."""
+    def backward(self, dpolicy, dvalue, dreturn=None, accumulate=False):
+        """Gradients of every parameter from the output gradients, written into param.grad (which must exist), or added to
+        what param.grad holds when `accumulate` (the micro-batches after the first of a gradient-accumulation step)."""
         m = self.model
         M_, D, H, W = self.M, self.D, self.H, self.W
         L = self.depth
@@ -248,13 +251,14 @@ class FusedBoardNet:
             # (named: a temporary copy freed before the launch could be handed to the next .contiguous())
             dpolicy, dvalue = dpolicy.contiguous(), dvalue.contiguous()
             dreturn = dreturn.contiguous() if self.rmaps else None
-            check(lib().hrl_heads_bwd(_ptr(self.Hpre), self.ldh, M_, self.cells, self.pmaps, self.vmaps, self.rmaps, self.A, self.slope,
+            acc = int(accumulate)
+            check(lib().hrl_heads_bwd_accumulate(_ptr(self.Hpre), self.ldh, M_, self.cells, self.pmaps, self.vmaps, self.rmaps, self.A, self.slope,
                                       _ptr(m.p_out.weight), _ptr(m.v_out.weight), _ptr(m.r_out.weight) if self.rmaps else None,
                                       _ptr(self.value), _ptr(dpolicy), _ptr(dvalue),
                                       _ptr(dreturn), _ptr(self.dHpre),
                                       _ptr(g(m.p_out.weight)), _ptr(g(m.v_out.weight)), _ptr(g(m.r_out.weight)) if self.rmaps else None,
                                       _ptr(g(m.p_squeeze.bias)), _ptr(g(m.v_squeeze.bias)), _ptr(g(m.r_squeeze.bias)) if self.rmaps else None,
-                                      _ptr(self.heads_ws), _stream_ptr()))
+                                      _ptr(self.heads_ws), acc, _stream_ptr()))
             _count(2)
             top = self.bn[L - 1]
             a_top = dict(t=self.Y[L - 1], consts=(top['scale'], top['shift']), relu=True)          # A_L = relu(bn_L(Y_L))
@@ -268,9 +272,9 @@ class FusedBoardNet:
             for l in range(L - 1, -1, -1):
                 blk, st = m.tower[l], self.bn[l]
                 bnm = blk[1]
-                check(lib().hrl_bn_finalize_bwd(_ptr(self.cp), self.tiles, self.width, self.cells, M_, _ptr(bnm.weight), _ptr(st['mean']),
-                                                _ptr(st['rstd']), _ptr(g(bnm.weight)), _ptr(g(bnm.bias)), _ptr(st['p']), _ptr(st['q']),
-                                                _ptr(st['r']), _stream_ptr()))
+                check(lib().hrl_bn_finalize_bwd_accumulate(_ptr(self.cp), self.tiles, self.width, self.cells, M_, _ptr(bnm.weight),
+                                                           _ptr(st['mean']), _ptr(st['rstd']), _ptr(g(bnm.weight)), _ptr(g(bnm.bias)),
+                                                           _ptr(st['p']), _ptr(st['q']), _ptr(st['r']), acc, _stream_ptr()))
                 _count()
                 dy = dict(t=self.dZ[l], t2=self.Y[l], consts=(st['p'], st['q'], st['r']))            # dY_l from dZ_l on the fly
                 if l > 0:
@@ -286,8 +290,8 @@ class FusedBoardNet:
                 else:
                     self._gemm(dy, dict(t=self.Wb[0], packed=True), self.dZ0, K=D, N=D, epilogue='mask_stats', ep=dict(y=self.A0))
             # stem: bias gradient from the column sums of dZ0, weight gradient over the raw observations
-            check(lib().hrl_bn_finalize_bwd(_ptr(self.cp), self.tiles, self.width, self.cells, M_, None, None, None, None,
-                                            _ptr(g(m.stem.bias)), None, None, None, _stream_ptr()))
+            check(lib().hrl_bn_finalize_bwd_accumulate(_ptr(self.cp), self.tiles, self.width, self.cells, M_, None, None, None, None,
+                                                       _ptr(g(m.stem.bias)), None, None, None, acc, _stream_ptr()))
             _count()
             self._wgrad(dict(t=self.dZ0, kmajor=False), dict(t=self.x2d, kmajor=False), D, self.K0, ('stem', 0), [(g(m.stem.weight), 0)])
-            self._fold_all()
+            self._fold_all(accumulate)

@@ -337,6 +337,23 @@ def replay_ratio(args):
     return float(value)
 
 
+def gradient_accumulation(args):
+    """train_args['gradient_accumulation'] -> k, the number of micro-batches each batch is trained as (one optimiser step per
+    batch); 1 when accumulation is off (key absent, None, 0 or 1).  True, a negative value and anything that is not an integer
+    raise ValueError."""
+    return micro_batch_count(args.get('gradient_accumulation'))
+
+
+def micro_batch_count(value):
+    """The checks of gradient_accumulation() on a value: None or 0 -> 1, an integer k >= 1 -> k, anything else ValueError."""
+    if value is None:
+        return 1
+    if isinstance(value, bool) or not isinstance(value, numbers.Integral) or value < 0:
+        raise ValueError("train_args['gradient_accumulation'] must be an integer k >= 1 of micro-batches per batch, or 0 / None "
+                         "for none; got %r" % (value,))
+    return max(1, int(value))
+
+
 class ReplayRatioLimiter:
     """The Trainer's samples-per-insert limit (train_args['replay_ratio'] = r), counted on the host from numbers it already
     has: `trained`, the samples of the batches drawn (drew(): batch_size * forward_steps each, the global batch without
@@ -913,6 +930,16 @@ class LearnerStep:
     side-stream copy.  priority_state_dict() reads them now; load_priority_state() writes saved ones.  The step is the same
     with and without.
 
+    gradient_accumulation (default: train_args['gradient_accumulation'], off): an integer k >= 1 that divides the batch B.  The
+    step still consumes one batch of B windows and takes one optimiser step, but runs the net, the loss kernel and the
+    net's backward over the k micro-batches dev[i*B/k:(i+1)*B/k] in order, each adding its gradient into the bucket; then one
+    launch (ops.sum_rows) folds the micro-batches' loss (and diagnostics) sums, and the all-reduce, the optimiser and the rest
+    of the step run once.  The net is sized for B/k windows, so its activations (and the recurrent hidden state) take 1/k of
+    the memory.  The gradient is the full batch's up to fp32 summation order, except that BatchNorm normalises each
+    micro-batch with its own statistics and moves its running statistics once per micro-batch (k per step) -- the step k
+    ranks of B/k windows would take.  `micro_batches` is k; launches_per_step counts all k micro-batches.  With k > 1
+    validation passes run in the same k micro-batches, and time_loss_kernel is refused.
+
     A feature that adds device state registers it in __init__, where it allocates it: in `_mutable` (or `_zeroed`) when a
     step or validation pass changes it, so that the capture's warm-up leaves it as it was, and in `_handoff` (a _Handoff)
     when the epoch boundary carries it to the host; end_epoch, _snapshot and _restore have no per-feature code.
@@ -921,7 +948,14 @@ class LearnerStep:
     def __init__(self, model, args, example_batch, lr, device=None, process_group=None, use_graph=True,
                  max_norm=4.0, weight_decay=1e-5, time_loss_kernel=False, channels_last=True, cudnn_benchmark=True,
                  small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None,
-                 weight_ema=None, save_optimizer=None, validation=None, skip_nonfinite=None, save_replay=None):
+                 weight_ema=None, save_optimizer=None, validation=None, skip_nonfinite=None, save_replay=None,
+                 gradient_accumulation=None):
+        k = micro_batch_count(args.get('gradient_accumulation') if gradient_accumulation is None else gradient_accumulation)
+        if k > 1 and example_batch['action'].shape[0] % k:
+            raise ValueError('gradient_accumulation = %d does not divide the batch of %d windows' % (k, example_batch['action'].shape[0]))
+        if k > 1 and time_loss_kernel:
+            raise ValueError('time_loss_kernel times the loss kernel of a whole batch: it needs gradient_accumulation = 1')
+        self.micro_batches = k
         self.save_replay = bool(_save_replay_spec(args) is not None if save_replay is None else save_replay)
         self.weight_ema = weight_ema_decay(args.get('weight_ema') if weight_ema is None else weight_ema)
         rate = validation_rate(args)
@@ -1040,13 +1074,24 @@ class LearnerStep:
         if self.prio_state is not None and self.save_replay:
             self.prio_snap = self._prio_image(self.device)
             self._handoff.append(_Handoff('prio', self.prio_snap, self._prio_copies(self.prio_snap)))
+        Bm = B // k                      # windows per micro-batch: what the net and the loss kernel see at once
+        self._micro = None
+        if k > 1:
+            # micro-batch i: views of rows [i*Bm, (i+1)*Bm) of every (batch-major) tensor of the packed batch; its loss pass
+            # writes its sums to row i of loss_rows ([NUM_LOSS sums | NUM_DIAG diagnostics]) and its slice of the advantage tap
+            self.loss_rows = torch.zeros((k, NUM_LOSS + NUM_DIAG), dtype=torch.float32, device=self.device)
+            self.advantage = torch.zeros((B, T, P, 1), dtype=torch.float32, device=self.device) if self.prio_state is not None else None
+            self._micro = [tree_map(lambda t, i=i: t[i * Bm:(i + 1) * Bm], self.dev) for i in range(k)]
+            self._micro_weight = [self.prio_state.win_weight[i * Bm:(i + 1) * Bm] if self.prio_state is not None else None
+                                  for i in range(k)]
+            self._micro_bufs = None
         self.hidden0 = None
         if hasattr(self.model, 'init_hidden'):
-            self.hidden0 = tree_map(lambda h: h.to(self.device), self.model.init_hidden([B, P]))
+            self.hidden0 = tree_map(lambda h: h.to(self.device), self.model.init_hidden([Bm, P]))
         from . import tower
         if fused_tower and small_boards and self.hidden0 is None and tower.supports(self.model) and \
                 torch.is_tensor(example_batch['observation']) and example_batch['observation'].shape[-2] * example_batch['observation'].shape[-1] <= 16:
-            self.engine = tower.FusedBoardNet(self.model, B * T * Pa, self.device, bf16=tensor_cores == 'bf16')
+            self.engine = tower.FusedBoardNet(self.model, Bm * T * Pa, self.device, bf16=tensor_cores == 'bf16')
         self.loss_buf = None
         self.last_losses = torch.zeros(NUM_LOSS, device=self.device)
         self.accum = torch.zeros(n_sums, dtype=torch.float64, device=self.device)
@@ -1092,17 +1137,23 @@ class LearnerStep:
         return fastnet.BoardConv2d.dense_calls > before
 
     # -- the device work of one step, on the current stream (inputs already in self.dev)
-    def _part_forward(self):
+    def _begin_step(self):
         if self.guard_saved is not None:        # one device-to-device copy: what a rejected step puts back
             self.guard_saved.copy_(self._guarded_buffers())
         fastnet.new_step()          # adjoint-weight copies of the previous step are stale: the optimiser has run
         self.opt.zero_grad()
+
+    def _forward(self, dev):
+        """The net's raw outputs (B', T, Pa, ...) on the windows of `dev` (the batch, or one micro-batch of it)."""
         if self.engine is not None:
-            B, T, P, Pa, A = self.dims
-            flat = self.engine.forward(self.dev['observation'].flatten(0, 2))
-            self._outs = {k: v.unflatten(0, (B, T, Pa)) for k, v in flat.items()}
-        else:
-            self._outs = forward_raw(self.model, self.hidden0, self.dev, self.args, self.memory_format)
+            B, T, Pa = dev['action'].shape[:3]
+            flat = self.engine.forward(dev['observation'].flatten(0, 2))
+            return {k: v.unflatten(0, (B, T, Pa)) for k, v in flat.items()}
+        return forward_raw(self.model, self.hidden0, dev, self.args, self.memory_format)
+
+    def _part_forward(self):
+        self._begin_step()
+        self._outs = self._forward(self.dev)
         if self.loss_buf is None:
             B, T, P, Pa, A = self.dims
             self.loss_buf = ops.LossBuffers(B, T, P, Pa, A, 'value' in self._outs, 'return' in self._outs, self.device,
@@ -1114,11 +1165,12 @@ class LearnerStep:
                          buffers=self.loss_buf, diagnostics=self.diagnostics,
                          window_weight=self.prio_state.win_weight if self.prio_state is not None else None)
 
-    def _part_backward(self):
-        outs, buf = self._outs, self.loss_buf
+    def _net_backward(self, outs, buf, accumulate=False):
+        """The net's backward from the loss kernel's output gradients in `buf`, into the gradient bucket (added to it when
+        `accumulate`; the module path's autograd always adds)."""
         if self.engine is not None:
             self.engine.backward(buf.dpolicy.flatten(0, 2), buf.dvalue.flatten(0, 2),
-                                 buf.dreturn.flatten(0, 2) if buf.dreturn is not None else None)
+                                 buf.dreturn.flatten(0, 2) if buf.dreturn is not None else None, accumulate=accumulate)
         else:
             heads, grads = [outs['policy']], [buf.dpolicy]
             if 'value' in outs:
@@ -1129,9 +1181,52 @@ class LearnerStep:
                 grads.append(buf.dreturn)
             with ops.deferred_weight_gradients():       # shared (recurrent) convolution weights: one product per weight, at the end
                 torch.autograd.backward(heads, grads)
+
+    def _part_backward(self):
+        buf = self.loss_buf
+        self._net_backward(self._outs, buf)
         self.opt.extra_slots[:NUM_LOSS].copy_(buf.losses)     # the loss sums ride the gradient bucket
         if self.diagnostics:
             self.opt.extra_slots[_LOSS_DIAG].copy_(buf.diagnostics[:NUM_LOSS_DIAG])
+        self._finish_step()
+
+    def _accumulated_step(self):
+        """The device work of one step over micro_batches > 1 micro-batches (see the class docstring)."""
+        self._begin_step()          # (guard_saved is taken before micro-batch 0: a rejected step restores all k forwards)
+        for i, (dev, weight) in enumerate(zip(self._micro, self._micro_weight)):
+            outs = self._forward(dev)
+            if self._micro_bufs is None:
+                self._micro_bufs = self._micro_loss_buffers(outs)
+            self.loss_buf, buf = self._micro_bufs[0], self._micro_bufs[i]
+            ops.loss_fwd_bwd({k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, dev, self.args, buffers=buf,
+                             diagnostics=self.diagnostics, window_weight=weight)
+            self._net_backward(outs, buf, accumulate=i > 0)
+            del outs            # this micro-batch's activations and autograd graph go back to the pool before the next forward
+        ops.sum_rows(self.loss_rows, self.n_tail, self.opt.extra_slots)       # [loss sums | the loss pass's diagnostics]
+        self._finish_step()
+
+    def _micro_loss_buffers(self, outs):
+        """One LossBuffers per micro-batch: the output gradients and workspaces of B/k windows are shared (the micro-batches
+        run in order), the sums go to row i of loss_rows and the advantage tap to the micro-batch's slice of `advantage`."""
+        B, T, P, Pa, A = self.dims
+        Bm = B // self.micro_batches
+        base = ops.LossBuffers(Bm, T, P, Pa, A, 'value' in outs, 'return' in outs, self.device, diagnostics=self.diagnostics)
+        bufs = []
+        for i in range(self.micro_batches):
+            buf = copy.copy(base)
+            buf.losses = self.loss_rows[i, :NUM_LOSS]
+            if self.diagnostics:
+                buf.diagnostics = self.loss_rows[i, NUM_LOSS:]
+            if self.advantage is not None:
+                buf.advantage = self.advantage[i * Bm:(i + 1) * Bm]
+            bufs.append(buf)
+        return bufs
+
+    def _advantage_tap(self):
+        return self.loss_buf.advantage if self.micro_batches == 1 else self.advantage
+
+    def _finish_step(self):
+        """The step's tail, once per step: the (all-reduced) bucket -> the optimiser and what follows it."""
         if self.peer is not None:
             reduced = self.peer(self.opt.n_pad, self.opt.partials)      # all-reduce + norm partials, one kernel
             self.opt.step_reduced(reduced)
@@ -1154,7 +1249,7 @@ class LearnerStep:
             ops.weight_ema_update(self.avg, self.state.bytes[:self.state.i_off].view(torch.float32), self.opt.step_count,
                                   self.weight_ema, self.avg_seeded, skip=self.opt.skip)
         if self.prio_state is not None:     # after the optimiser: a rejected step stores no priority
-            ops.priority_update(self.prio_state, self.loss_buf.advantage, self.dev['turn_mask'], self.args.get('burn_in_steps', 0),
+            ops.priority_update(self.prio_state, self._advantage_tap(), self.dev['turn_mask'], self.args.get('burn_in_steps', 0),
                                 skip=self.opt.skip if self.skip_nonfinite else None)
 
     def _guarded_buffers(self):
@@ -1163,6 +1258,9 @@ class LearnerStep:
         return self.state.bytes[self.state.f_off:self.state.nbytes]
 
     def _device_step(self):
+        if self.micro_batches > 1:
+            self._accumulated_step()
+            return
         self._part_forward()
         self._part_loss()
         self._part_backward()
@@ -1175,17 +1273,16 @@ class LearnerStep:
             store.bytes[:store.i_off].copy_(self.avg_bytes)
         fastnet.new_step()          # the weights differ from those the cached convolution images were packed from
         B, T, P, Pa, A = self.dims
-        with torch.no_grad():
-            if self.engine is not None:
-                flat = self.engine.forward(self.dev['observation'].flatten(0, 2))
-                outs = {k: v.unflatten(0, (B, T, Pa)) for k, v in flat.items()}
-            else:
-                outs = forward_raw(self.model, self.hidden0, self.dev, self.args, self.memory_format)
-        if self.val_buf is None:
-            self.val_buf = ops.LossBuffers(B, T, P, Pa, A, 'value' in outs, 'return' in outs, self.device, grads=False)
-        sums = ops.loss_fwd({k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, self.dev, self.args,
-                            buffers=self.val_buf)
-        (self.val_ema_accum if averaged else self.val_accum).add_(sums)
+        for dev in (self._micro or [self.dev]):         # the same micro-batches as the step
+            with torch.no_grad():
+                outs = self._forward(dev)
+            if self.val_buf is None:
+                self.val_buf = ops.LossBuffers(B // self.micro_batches, T, P, Pa, A, 'value' in outs, 'return' in outs, self.device,
+                                               grads=False)
+            sums = ops.loss_fwd({k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, dev, self.args,
+                                buffers=self.val_buf)
+            (self.val_ema_accum if averaged else self.val_accum).add_(sums)
+            del outs
         store.bytes.copy_(self.val_saved)
 
     def _validation_forms(self):
@@ -2147,10 +2244,20 @@ class Trainer:
     models/<epoch>.replay.pth (replay_file, ReplayCheckpoints; numbered like .ema.pth and .optim.pth) and keeps the newest k
     files this run wrote.  A run restarted at restart_epoch with models/<restart_epoch>.replay.pth present starts with those
     episodes in `episodes`, trains at once, and restores the sampler state and priorities before its first batch; it prints
-    'restored replay: <n> episodes (<m> held out), <s> steps, priorities: <yes|no>'.  Needs gpu_replay."""
+    'restored replay: <n> episodes (<m> held out), <s> steps, priorities: <yes|no>'.  Needs gpu_replay.
+
+    train_args['gradient_accumulation'] = k: each batch of batch_size windows is trained as k micro-batches of batch_size / k
+    with one optimiser step (LearnerStep), so the net's activations take 1/k of the memory.  k must divide batch_size
+    (ValueError otherwise); with several GPUs each rank runs k micro-batches of its batch_size / num_gpus windows, and when
+    batch_size % (num_gpus * k) != 0 the trainer prints one line and uses one GPU.  Steps, the learning-rate law and the
+    printed lines are unchanged; BatchNorm normalises each micro-batch with its own statistics."""
 
     def __init__(self, args, model):
         ratio = replay_ratio(args)
+        self.micro_batches = gradient_accumulation(args)
+        if args['batch_size'] % self.micro_batches:
+            raise ValueError("train_args['gradient_accumulation'] = %d does not divide batch_size = %d"
+                             % (self.micro_batches, args['batch_size']))
         self.save_replay = save_replay(args)
         self.weight_ema = weight_ema_decay(args.get('weight_ema'))
         self.validation = validation_rate(args)
@@ -2193,6 +2300,11 @@ class Trainer:
             self.world = max(1, min(int(want), torch.cuda.device_count()) if want else torch.cuda.device_count())
             if self.world > 1 and (not self.gpu_replay or args['batch_size'] % self.world != 0):
                 print('handyrl_b200: multi-GPU needs gpu_replay and batch_size %% num_gpus == 0; using one GPU')
+                self.world = 1
+            elif self.world > 1 and args['batch_size'] % (self.world * self.micro_batches) != 0:
+                print('handyrl_b200: multi-GPU with gradient_accumulation needs batch_size %% (num_gpus * gradient_accumulation) == 0 '
+                      '(num_gpus %d, gradient_accumulation %d, batch_size %d); using one GPU'
+                      % (self.world, self.micro_batches, args['batch_size']))
                 self.world = 1
         self.replay_files = None             # the writer of the .replay.pth files
         self.restored = None                 # the replay file this run resumed from, until its sampler state is put back

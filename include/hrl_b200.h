@@ -270,6 +270,14 @@ int hrl_weight_ema_guarded(float *avg, const float *state, int64_t n, const int6
                            const int32_t *skip, void *stream);
 
 /*
+ * Gradient accumulation (opt-in; a batch trained as k micro-batches with one optimiser step): the fused loss pass of
+ * micro-batch i leaves its sums in row i of a (k, ld) buffer, and one launch folds them into the bucket tail:
+ *     out[j] = (float) sum_{i = 0..k-1} (double) rows[i*ld + j]      for j < n,
+ * in that fixed order (bit-reproducible), rounded once.  out may not overlap rows.
+ */
+int hrl_sum_rows(const float *rows, int32_t k, int64_t ld, int32_t n, float *out, void *stream);
+
+/*
  * Multi-GPU form of the same step: one-shot all-reduce (SUM) of the flat gradient bucket over NVLink peer
  * memory, fused with the sum-of-squares partials hrl_clip_adam_step consumes (replaces NCCL all-reduce +
  * hrl_grad_sumsq).  Every rank reads every rank's bucket directly (P2P loads through NVSwitch), adds them in
@@ -414,6 +422,11 @@ int hrl_gemm_fused(const HrlGemmArgs *args, void *stream);
  *                         -> policy = . Wp^T (A x pmaps*cells), value = tanh(. Wv^T), return = . Wr^T; the backward
  *                         writes dpre and the gradients of Wp / Wv / Wr and of the squeeze biases (fixed-order sums;
  *                         workspace: hrl_heads_num_blocks(M) * (A*pin + vin + rin + maps) floats).
+ *   hrl_bn_finalize_bwd_accumulate / hrl_heads_bwd_accumulate: the same, except that with accumulate != 0 the parameter
+ *                         gradients (dgamma, dbeta; dWp, dWv, dWr and the squeeze-bias gradients) are ADDED to what those
+ *                         buffers hold (each fp32 result rounded first), for the micro-batches after the first of a
+ *                         gradient-accumulation step.  dpre and p_col / q_col / r_col are written as before.  accumulate == 0
+ *                         is the plain form bit for bit.
  */
 int hrl_bn_finalize_fwd(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows, const float *gamma,
                         const float *beta, float eps, float momentum, float *running_mean, float *running_var,
@@ -421,6 +434,9 @@ int hrl_bn_finalize_fwd(const float *col_partials, int32_t tiles, int32_t C, int
 int hrl_bn_finalize_bwd(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows, const float *gamma,
                         const float *mean_col, const float *rstd_col, float *dgamma, float *dbeta, float *p_col, float *q_col,
                         float *r_col, void *stream);
+int hrl_bn_finalize_bwd_accumulate(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows, const float *gamma,
+                                   const float *mean_col, const float *rstd_col, float *dgamma, float *dbeta, float *p_col, float *q_col,
+                                   float *r_col, int32_t accumulate, void *stream);
 int32_t hrl_heads_num_blocks(int64_t M);
 int hrl_heads_fwd(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps, int32_t A,
                   float slope, const float *Wp, const float *Wv, const float *Wr, float *policy, float *value, float *ret, void *stream);
@@ -428,6 +444,11 @@ int hrl_heads_bwd(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_
                   float slope, const float *Wp, const float *Wv, const float *Wr, const float *value, const float *dpolicy,
                   const float *dvalue, const float *dret, float *dpre, float *dWp, float *dWv, float *dWr, float *dbias_p,
                   float *dbias_v, float *dbias_r, float *workspace, void *stream);
+int hrl_heads_bwd_accumulate(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps,
+                             int32_t A, float slope, const float *Wp, const float *Wv, const float *Wr, const float *value,
+                             const float *dpolicy, const float *dvalue, const float *dret, float *dpre, float *dWp, float *dWv,
+                             float *dWr, float *dbias_p, float *dbias_v, float *dbias_r, float *workspace, int32_t accumulate,
+                             void *stream);
 
 /*
  * Weight of a stride-1 "same" convolution (Cout,Cin,kh,kw; odd kernel, zero padding) <-> the dense matrix
@@ -477,6 +498,9 @@ typedef struct HrlFoldJob {
     int64_t split_stride;
     float *dw;
     int32_t Cout, Cin, kh, kw, H, W;
+    /* != 0: add the folded gradient to dw (its fp32 sum over the slices and taps rounded first) instead of storing it --
+     * micro-batches after the first of a gradient-accumulation step.  0 (what hrl_board_fold passes) stores. */
+    int32_t accumulate;
 } HrlFoldJob;
 int hrl_board_pack_many(const HrlPackJob *jobs, int32_t n_jobs, void *stream);
 /* The same launch (0..HRL_MAX_BOARD_JOBS jobs) plus the pivots of the STATS epilogue's shifted BatchNorm sums for 0..HRL_MAX_BOARD_JOBS
