@@ -15,6 +15,7 @@ Same public names as handyrl/train.py for the path
 """
 import collections
 import copy
+import functools
 import numbers
 import os
 import pickle
@@ -930,15 +931,16 @@ class LearnerStep:
     side-stream copy.  priority_state_dict() reads them now; load_priority_state() writes saved ones.  The step is the same
     with and without.
 
-    gradient_accumulation (default: train_args['gradient_accumulation'], off): an integer k >= 1 that divides the batch B.  The
-    step still consumes one batch of B windows and takes one optimiser step, but runs the net, the loss kernel and the
-    net's backward over the k micro-batches dev[i*B/k:(i+1)*B/k] in order, each adding its gradient into the bucket; then one
-    launch (ops.sum_rows) folds the micro-batches' loss (and diagnostics) sums, and the all-reduce, the optimiser and the rest
-    of the step run once.  The net is sized for B/k windows, so its activations (and the recurrent hidden state) take 1/k of
-    the memory.  The gradient is the full batch's up to fp32 summation order, except that BatchNorm normalises each
+    gradient_accumulation (default: train_args['gradient_accumulation'], 1): an integer k >= 1 that divides the batch B.  Every
+    step consumes one batch of B windows and takes one optimiser step, running the net, the loss kernel and the net's
+    backward over the k micro-batches dev[i*B/k:(i+1)*B/k] (`_micro`) in order, each adding its gradient into the bucket;
+    the micro-batches' loss (and diagnostics) sums are then folded into the bucket tail (one device copy at k = 1, one
+    ops.sum_rows launch otherwise), and the all-reduce, the optimiser and the rest of the step run once.  k = 1 is the whole
+    batch as one micro-batch.  The net is sized for B/k windows, so its activations (and the recurrent hidden state) take
+    1/k of the memory.  The gradient is the full batch's up to fp32 summation order, except that BatchNorm normalises each
     micro-batch with its own statistics and moves its running statistics once per micro-batch (k per step) -- the step k
-    ranks of B/k windows would take.  `micro_batches` is k; launches_per_step counts all k micro-batches.  With k > 1
-    validation passes run in the same k micro-batches, and time_loss_kernel is refused.
+    ranks of B/k windows would take.  `micro_batches` is k; launches_per_step counts all k micro-batches.  Validation
+    passes run in the same micro-batches; time_loss_kernel needs k = 1.
 
     A feature that adds device state registers it in __init__, where it allocates it: in `_mutable` (or `_zeroed`) when a
     step or validation pass changes it, so that the capture's warm-up leaves it as it was, and in `_handoff` (a _Handoff)
@@ -999,6 +1001,7 @@ class LearnerStep:
         self.model.train()
         self.time_loss_kernel = time_loss_kernel
         self.kernel_events = []
+        self._timed_loss = None          # time_loss_kernel: the loss kernel launched between the two step graphs
         self.pg = process_group
         self.world = torch.distributed.get_world_size(process_group) if process_group is not None else 1
         params = [p for p in self.model.parameters()]
@@ -1075,16 +1078,14 @@ class LearnerStep:
             self.prio_snap = self._prio_image(self.device)
             self._handoff.append(_Handoff('prio', self.prio_snap, self._prio_copies(self.prio_snap)))
         Bm = B // k                      # windows per micro-batch: what the net and the loss kernel see at once
-        self._micro = None
-        if k > 1:
-            # micro-batch i: views of rows [i*Bm, (i+1)*Bm) of every (batch-major) tensor of the packed batch; its loss pass
-            # writes its sums to row i of loss_rows ([NUM_LOSS sums | NUM_DIAG diagnostics]) and its slice of the advantage tap
-            self.loss_rows = torch.zeros((k, NUM_LOSS + NUM_DIAG), dtype=torch.float32, device=self.device)
-            self.advantage = torch.zeros((B, T, P, 1), dtype=torch.float32, device=self.device) if self.prio_state is not None else None
-            self._micro = [tree_map(lambda t, i=i: t[i * Bm:(i + 1) * Bm], self.dev) for i in range(k)]
-            self._micro_weight = [self.prio_state.win_weight[i * Bm:(i + 1) * Bm] if self.prio_state is not None else None
-                                  for i in range(k)]
-            self._micro_bufs = None
+        # micro-batch i: views of rows [i*Bm, (i+1)*Bm) of every (batch-major) tensor of the packed batch and of the window
+        # weights (k = 1: the whole batch); its loss pass writes its sums to row i of loss_rows ([NUM_LOSS sums | NUM_DIAG
+        # diagnostics]) and its rows of the advantage tap (_build_loss_buffers)
+        self._micro = [tree_map(lambda t, i=i: t[i * Bm:(i + 1) * Bm], self.dev) for i in range(k)]
+        self._win_weight = [self.prio_state.win_weight[i * Bm:(i + 1) * Bm] if self.prio_state is not None else None
+                            for i in range(k)]
+        self.loss_rows = torch.zeros((k, NUM_LOSS + NUM_DIAG), dtype=torch.float32, device=self.device)
+        self.advantage = torch.zeros((B, T, P, 1), dtype=torch.float32, device=self.device) if self.prio_state is not None else None
         self.hidden0 = None
         if hasattr(self.model, 'init_hidden'):
             self.hidden0 = tree_map(lambda h: h.to(self.device), self.model.init_hidden([Bm, P]))
@@ -1092,7 +1093,7 @@ class LearnerStep:
         if fused_tower and small_boards and self.hidden0 is None and tower.supports(self.model) and \
                 torch.is_tensor(example_batch['observation']) and example_batch['observation'].shape[-2] * example_batch['observation'].shape[-1] <= 16:
             self.engine = tower.FusedBoardNet(self.model, Bm * T * Pa, self.device, bf16=tensor_cores == 'bf16')
-        self.loss_buf = None
+        self.loss_buf = self._loss_bufs = None      # built by the first forward (_build_loss_buffers)
         self.last_losses = torch.zeros(NUM_LOSS, device=self.device)
         self.accum = torch.zeros(n_sums, dtype=torch.float64, device=self.device)
         self._mutable.append(self.accum)
@@ -1151,19 +1152,27 @@ class LearnerStep:
             return {k: v.unflatten(0, (B, T, Pa)) for k, v in flat.items()}
         return forward_raw(self.model, self.hidden0, dev, self.args, self.memory_format)
 
-    def _part_forward(self):
-        self._begin_step()
-        self._outs = self._forward(self.dev)
-        if self.loss_buf is None:
-            B, T, P, Pa, A = self.dims
-            self.loss_buf = ops.LossBuffers(B, T, P, Pa, A, 'value' in self._outs, 'return' in self._outs, self.device,
-                                            advantage=self.prio_state is not None)
-
-    def _part_loss(self):
-        outs = self._outs
-        ops.loss_fwd_bwd({k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, self.dev, self.args,
-                         buffers=self.loss_buf, diagnostics=self.diagnostics,
-                         window_weight=self.prio_state.win_weight if self.prio_state is not None else None)
+    def _build_loss_buffers(self, outs):
+        """The loss passes' buffers, built on the first forward because the heads come from the net's outputs.  One
+        LossBuffers per micro-batch: all share the output gradients and workspaces of B/k windows (the micro-batches run in
+        order), and micro-batch i's sums go to row i of loss_rows and its advantage tap to its rows of `advantage`.
+        loss_buf is micro-batch 0's; val_buf takes the validation passes' forward-only outputs."""
+        B, T, P, Pa, A = self.dims
+        Bm = B // self.micro_batches
+        heads = ('value' in outs, 'return' in outs)
+        base = ops.LossBuffers(Bm, T, P, Pa, A, *heads, self.device, diagnostics=self.diagnostics)
+        self._loss_bufs = []
+        for i in range(self.micro_batches):
+            buf = copy.copy(base)
+            buf.losses = self.loss_rows[i, :NUM_LOSS]
+            if self.diagnostics:
+                buf.diagnostics = self.loss_rows[i, NUM_LOSS:]
+            if self.advantage is not None:
+                buf.advantage = self.advantage[i * Bm:(i + 1) * Bm]
+            self._loss_bufs.append(buf)
+        self.loss_buf = self._loss_bufs[0]
+        if self.validation:
+            self.val_buf = ops.LossBuffers(Bm, T, P, Pa, A, *heads, self.device, grads=False)
 
     def _net_backward(self, outs, buf, accumulate=False):
         """The net's backward from the loss kernel's output gradients in `buf`, into the gradient bucket (added to it when
@@ -1182,48 +1191,31 @@ class LearnerStep:
             with ops.deferred_weight_gradients():       # shared (recurrent) convolution weights: one product per weight, at the end
                 torch.autograd.backward(heads, grads)
 
-    def _part_backward(self):
-        buf = self.loss_buf
-        self._net_backward(self._outs, buf)
-        self.opt.extra_slots[:NUM_LOSS].copy_(buf.losses)     # the loss sums ride the gradient bucket
-        if self.diagnostics:
-            self.opt.extra_slots[_LOSS_DIAG].copy_(buf.diagnostics[:NUM_LOSS_DIAG])
-        self._finish_step()
-
-    def _accumulated_step(self):
-        """The device work of one step over micro_batches > 1 micro-batches (see the class docstring)."""
+    def _step_parts(self):
+        """The device work of one step, on the current stream (inputs already in self.dev): begin, then for each micro-batch
+        in order net forward -> fused loss kernel -> net backward into the bucket, then the loss-pass sums into the bucket
+        tail and _finish_step.  A generator that pauses once, yielding the last micro-batch's loss kernel launch (a
+        callable) for the caller to run: _device_step runs it in place, time_loss_kernel between two graphs."""
         self._begin_step()          # (guard_saved is taken before micro-batch 0: a rejected step restores all k forwards)
-        for i, (dev, weight) in enumerate(zip(self._micro, self._micro_weight)):
+        for i, (dev, weight) in enumerate(zip(self._micro, self._win_weight)):
             outs = self._forward(dev)
-            if self._micro_bufs is None:
-                self._micro_bufs = self._micro_loss_buffers(outs)
-            self.loss_buf, buf = self._micro_bufs[0], self._micro_bufs[i]
-            ops.loss_fwd_bwd({k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, dev, self.args, buffers=buf,
-                             diagnostics=self.diagnostics, window_weight=weight)
+            if self.loss_buf is None:
+                self._build_loss_buffers(outs)
+            buf = self._loss_bufs[i]
+            loss = functools.partial(ops.loss_fwd_bwd, {k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, dev,
+                                     self.args, buffers=buf, diagnostics=self.diagnostics, window_weight=weight)
+            if i == len(self._micro) - 1:
+                yield loss
+            else:
+                loss()
             self._net_backward(outs, buf, accumulate=i > 0)
-            del outs            # this micro-batch's activations and autograd graph go back to the pool before the next forward
-        ops.sum_rows(self.loss_rows, self.n_tail, self.opt.extra_slots)       # [loss sums | the loss pass's diagnostics]
+            del outs, loss      # this micro-batch's activations and autograd graph go back to the pool before the next forward
+        # the loss sums [+ the loss pass's diagnostics] ride the gradient bucket: one row is copied, k rows are summed
+        if self.micro_batches == 1:
+            self.opt.extra_slots[:self.n_tail].copy_(self.loss_rows[0, :self.n_tail])
+        else:
+            ops.sum_rows(self.loss_rows, self.n_tail, self.opt.extra_slots)
         self._finish_step()
-
-    def _micro_loss_buffers(self, outs):
-        """One LossBuffers per micro-batch: the output gradients and workspaces of B/k windows are shared (the micro-batches
-        run in order), the sums go to row i of loss_rows and the advantage tap to the micro-batch's slice of `advantage`."""
-        B, T, P, Pa, A = self.dims
-        Bm = B // self.micro_batches
-        base = ops.LossBuffers(Bm, T, P, Pa, A, 'value' in outs, 'return' in outs, self.device, diagnostics=self.diagnostics)
-        bufs = []
-        for i in range(self.micro_batches):
-            buf = copy.copy(base)
-            buf.losses = self.loss_rows[i, :NUM_LOSS]
-            if self.diagnostics:
-                buf.diagnostics = self.loss_rows[i, NUM_LOSS:]
-            if self.advantage is not None:
-                buf.advantage = self.advantage[i * Bm:(i + 1) * Bm]
-            bufs.append(buf)
-        return bufs
-
-    def _advantage_tap(self):
-        return self.loss_buf.advantage if self.micro_batches == 1 else self.advantage
 
     def _finish_step(self):
         """The step's tail, once per step: the (all-reduced) bucket -> the optimiser and what follows it."""
@@ -1249,7 +1241,7 @@ class LearnerStep:
             ops.weight_ema_update(self.avg, self.state.bytes[:self.state.i_off].view(torch.float32), self.opt.step_count,
                                   self.weight_ema, self.avg_seeded, skip=self.opt.skip)
         if self.prio_state is not None:     # after the optimiser: a rejected step stores no priority
-            ops.priority_update(self.prio_state, self._advantage_tap(), self.dev['turn_mask'], self.args.get('burn_in_steps', 0),
+            ops.priority_update(self.prio_state, self.advantage, self.dev['turn_mask'], self.args.get('burn_in_steps', 0),
                                 skip=self.opt.skip if self.skip_nonfinite else None)
 
     def _guarded_buffers(self):
@@ -1258,12 +1250,8 @@ class LearnerStep:
         return self.state.bytes[self.state.f_off:self.state.nbytes]
 
     def _device_step(self):
-        if self.micro_batches > 1:
-            self._accumulated_step()
-            return
-        self._part_forward()
-        self._part_loss()
-        self._part_backward()
+        for loss in self._step_parts():
+            loss()
 
     def _device_validate(self, averaged):
         """The device work of one validation pass, on the current stream (inputs already in self.dev)."""
@@ -1272,13 +1260,11 @@ class LearnerStep:
         if averaged:
             store.bytes[:store.i_off].copy_(self.avg_bytes)
         fastnet.new_step()          # the weights differ from those the cached convolution images were packed from
-        B, T, P, Pa, A = self.dims
-        for dev in (self._micro or [self.dev]):         # the same micro-batches as the step
+        for dev in self._micro:         # the same micro-batches as the step
             with torch.no_grad():
                 outs = self._forward(dev)
-            if self.val_buf is None:
-                self.val_buf = ops.LossBuffers(B // self.micro_batches, T, P, Pa, A, 'value' in outs, 'return' in outs, self.device,
-                                               grads=False)
+            if self.loss_buf is None:
+                self._build_loss_buffers(outs)
             sums = ops.loss_fwd({k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, dev, self.args,
                                 buffers=self.val_buf)
             (self.val_ema_accum if averaged else self.val_accum).add_(sums)
@@ -1313,14 +1299,15 @@ class LearnerStep:
                 self._capture_validation(self.graph.pool())
                 self._restore(state)
             elif self.use_graph:
-                # the loss kernel is launched between two graphs so that CUDA events can bracket it
+                # the (last micro-batch's) loss kernel is launched between two graphs so that CUDA events can bracket it
+                parts = self._step_parts()
                 self.graph_fwd = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(self.graph_fwd, stream=self.stream):
-                    self._part_forward()
-                self._part_loss()
+                    self._timed_loss = next(parts)
+                self._timed_loss()
                 self.graph_bwd = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(self.graph_bwd, pool=self.graph_fwd.pool(), stream=self.stream):
-                    self._part_backward()
+                    next(parts, None)
                 self._capture_validation(self.graph_fwd.pool())
                 self._restore(state)
             self.stream.synchronize()
@@ -1404,7 +1391,7 @@ class LearnerStep:
                 self.graph_fwd.replay()
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record(self.stream)
-                self._part_loss()
+                self._timed_loss()
                 e1.record(self.stream)
                 self.kernel_events.append((e0, e1))
                 self.graph_bwd.replay()
@@ -1493,7 +1480,7 @@ class LearnerStep:
         self.stream.synchronize()
         self.graph = self.graph_fwd = self.graph_bwd = None
         self.val_graphs = {}
-        self._outs = None
+        self._timed_loss = None
         self._captured = False
         import gc
         gc.collect()
