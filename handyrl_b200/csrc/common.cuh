@@ -53,4 +53,12 @@ __device__ __forceinline__ double warp_sum_d(double v) {
 __device__ __forceinline__ float ld_stream(const float *p) { return __ldcs(p); }
 __device__ __forceinline__ void st_stream(float *p, float v) { __stcs(p, v); }
 
+// asynchronous 16-byte global -> shared copies (cp.async.cg: L2 only), one commit group per call of cp_async_commit
+__device__ __forceinline__ void cp_async16(uint32_t dst, const float *src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
 }  // namespace hrl

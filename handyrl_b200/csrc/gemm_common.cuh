@@ -11,9 +11,10 @@
 // [chunk][n_pad rows][64 bytes] (one bulk copy per stage), and a chunk is 2 wgmma m64nNk16 .f32.bf16.bf16 per warpgroup into the
 // same fp32 accumulators; the epilogues are shared.  A product of two bf16 values is exact in fp32, so the result is the
 // fp32-accumulated product of the rounded operands.
+// A unit that defines neither (csrc/gemm_tower_kernel.cu) gets the shared pieces only: operand layout, wgmma helpers.
 #pragma once
-#if !defined(HRL_GEMM_KERNEL) || !defined(HRL_GEMM_BF16)
-#error "define HRL_GEMM_KERNEL and HRL_GEMM_BF16 before including gemm_common.cuh"
+#if defined(HRL_GEMM_KERNEL) != defined(HRL_GEMM_BF16)
+#error "define both HRL_GEMM_KERNEL and HRL_GEMM_BF16 before including gemm_common.cuh, or neither"
 #endif
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -646,6 +647,7 @@ __device__ __forceinline__ float4 transform_item(const GemmOperand &op, const It
     return v;
 }
 
+#ifdef HRL_GEMM_KERNEL
 // A and B go global -> registers -> (transform, hi/lo split) -> shared memory; a packed B image arrives by one bulk copy a
 // stage.  Each thread owns kItemsA items of the A tile (coalesced: 8 consecutive lanes = the 128 bytes of one k-major row,
 // or consecutive rows of a transposed one) and ITEMS_B items of the B tile.  NW = the MMA width of a warpgroup = half the
@@ -1052,6 +1054,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) HRL_GEMM_KERNEL(const GemmPar
         }
     }
 }
+#endif  // HRL_GEMM_KERNEL
 
 // the bf16 entry points (csrc/gemm_bf16_kernel.cu): launches gemm_bf16_kernel of MMA width nw for p's operand layouts
 int launch_gemm_bf16(const GemmParams &p, int nw, dim3 grid, size_t smem_bytes, cudaStream_t stream);

@@ -32,6 +32,7 @@
 #define HRL_GEMM_KERNEL gemm_tf32x3_kernel     // the kernel template gemm_common.cuh defines, and its operand precision
 #define HRL_GEMM_BF16 false
 #include "gemm_common.cuh"
+#include "gemm_tower.cuh"
 #include "gemm_wgrad.cuh"
 
 // profiling / test hook (include/hrl_b200.h): 1 = no MMAs, 2 = no operand loads
@@ -179,8 +180,11 @@ extern "C" int hrl_gemm_fused(const HrlGemmArgs *args, void *stream_) {
     if (smem_bytes < ep_bytes) smem_bytes = ep_bytes;
     const dim3 grid((unsigned)((M + kTileM - 1) / kTileM), (unsigned)n_tiles, (unsigned)splits);
     int st;
-    // weight gradients (both operands stored [K][rows]) run on the mma.sync kernel that reads them untransposed
-    if (gemm_wgrad_applies(g)) st = launch_gemm_wgrad(g, p.chunks_per_split, splits, p.C, p.ldc, p.c_split_stride, p.debug, stream);
+    // the tower's forward and input gradients (K-major A, a packed 288-column weight image) run on the kernel that stages A
+    // raw, several chunks ahead; weight gradients (both operands stored [K][rows]) on the mma.sync kernel that reads them
+    // untransposed
+    if (gemm_tower_applies(g)) st = launch_gemm_tower(p, stream);
+    else if (gemm_wgrad_applies(g)) st = launch_gemm_wgrad(g, p.chunks_per_split, splits, p.C, p.ldc, p.c_split_stride, p.debug, stream);
     else if (g.bf16) st = launch_gemm_bf16(p, n_pad / 2, grid, smem_bytes, stream);
     else switch (n_pad / 2) {          // the MMA width of a warpgroup: n_pad is a multiple of 16 up to 256, then 288
     case 8: st = launch_gemm_width<8>(p, grid, smem_bytes, stream); break;

@@ -75,13 +75,6 @@ __device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], 
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-__device__ __forceinline__ void cp_async16(uint32_t dst, const float *src) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-
 // per-row constants of this thread's 6 rows of an operand (rows 16 i + 2 g + e of the warp's 48, i < 3, e < 2): p, q, r
 // as the transform uses them.  Rows past the operand get zeros (their outputs are not stored).
 template <int KIND, bool IS_A>
