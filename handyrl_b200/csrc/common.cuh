@@ -49,6 +49,12 @@ __device__ __forceinline__ double warp_sum_d(double v) {
     return v;
 }
 
+// the 3xTF32 split: hi = v with the 13 low mantissa bits cleared (exactly a TF32 number), lo = v - hi (exact)
+__device__ __forceinline__ void split_tf32(float v, float &hi, float &lo) {
+    hi = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
+    lo = v - hi;
+}
+
 // streaming global accesses: data touched exactly once should not displace L1 lines
 __device__ __forceinline__ float ld_stream(const float *p) { return __ldcs(p); }
 __device__ __forceinline__ void st_stream(float *p, float v) { __stcs(p, v); }

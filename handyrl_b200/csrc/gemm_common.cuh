@@ -1,9 +1,11 @@
 // Shared body of the tensor-core GEMM (csrc/gemm_kernel.cu: 3xTF32, the default; csrc/gemm_bf16_kernel.cu: bf16 operands).
-// The including translation unit names the kernel template and its operand precision:
+// The including translation unit names the kernel template, its operand precision and its launcher:
 //     #define HRL_GEMM_KERNEL gemm_tf32x3_kernel / gemm_bf16_kernel      template <A_K, B_K, PACKED, NW>
 //     #define HRL_GEMM_BF16   false / true                               the constexpr BF16 inside the body
-// so that each unit instantiates only its own precision, and the 3xTF32 kernels are the same __global__ function as before the
-// bf16 form existed (a __device__ body behind a wrapper kernel changes their register allocation).
+//     #define HRL_GEMM_LAUNCH launch_gemm_tf32x3 / launch_gemm_bf16      the MMA-width dispatch over its instantiations
+// so that each unit instantiates only its own precision (17 widths x 6 operand layouts) from one kernel text and one width
+// table, and the 3xTF32 kernels are the same __global__ function as before the bf16 form existed (a __device__ body behind a
+// wrapper kernel changes their register allocation).
 //
 // bf16 form (HrlGemmArgs.bf16): operands are staged as in the 3xTF32 form -- global -> registers -> fp32 transform (fmaf,
 // optional ReLU) -- then rounded to nearest even bf16 (__float2bfloat16_rn) and stored once, K-major SWIZZLE_64B (a
@@ -11,10 +13,10 @@
 // [chunk][n_pad rows][64 bytes] (one bulk copy per stage), and a chunk is 2 wgmma m64nNk16 .f32.bf16.bf16 per warpgroup into the
 // same fp32 accumulators; the epilogues are shared.  A product of two bf16 values is exact in fp32, so the result is the
 // fp32-accumulated product of the rounded operands.
-// A unit that defines neither (csrc/gemm_tower_kernel.cu) gets the shared pieces only: operand layout, wgmma helpers.
+// A unit that defines none (csrc/gemm_tower_kernel.cu) gets the shared pieces only: operand layout, wgmma helpers, epilogue.
 #pragma once
-#if defined(HRL_GEMM_KERNEL) != defined(HRL_GEMM_BF16)
-#error "define both HRL_GEMM_KERNEL and HRL_GEMM_BF16 before including gemm_common.cuh, or neither"
+#if defined(HRL_GEMM_KERNEL) != defined(HRL_GEMM_BF16) || defined(HRL_GEMM_KERNEL) != defined(HRL_GEMM_LAUNCH)
+#error "define all of HRL_GEMM_KERNEL, HRL_GEMM_BF16 and HRL_GEMM_LAUNCH before including gemm_common.cuh, or none"
 #endif
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -510,14 +512,10 @@ __device__ __forceinline__ uint2 pack_bf16x4(const float4 v) {
 }
 
 __device__ __forceinline__ void split_tf32(const float4 v, float4 &hi, float4 &lo) {
-    hi.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-    hi.y = __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-    hi.z = __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-    hi.w = __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-    lo.x = v.x - hi.x;
-    lo.y = v.y - hi.y;
-    lo.z = v.z - hi.z;
-    lo.w = v.w - hi.w;
+    split_tf32(v.x, hi.x, lo.x);
+    split_tf32(v.y, hi.y, lo.y);
+    split_tf32(v.z, hi.z, lo.z);
+    split_tf32(v.w, hi.w, lo.w);
 }
 
 // ---- operand loaders.  Every thread owns a fixed set of "items" (one row x 4 consecutive reduction elements = one 16-byte
@@ -647,6 +645,145 @@ __device__ __forceinline__ float4 transform_item(const GemmOperand &op, const It
     return v;
 }
 
+// ---- epilogue of the wgmma kernels (the general one below and gemm_tower_kernel): the accumulators of warpgroup wg cover
+// rows 64 (wg & 1) ... and columns NW (wg >> 1) ... of the tile at (m0, n0); registers -> shared-memory tile (padded rows) ->
+// coalesced global stores into K slice `split`'s output.
+template <int NW>
+__device__ __forceinline__ void gemm_epilogue(const GemmParams &p, float (&acc)[NW / 2], uint8_t *smem, int m0, int rows_a, int n0,
+                                              int n_here, int split) {
+    constexpr int n_pad = 2 * NW, nw = NW;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
+    // (a thread holds 2 columns of 2 rows per 8-column group: storing from registers would scatter every warp instruction)
+    //   HRL_GEMM_EP_RELU        C = max(acc, 0)
+    //   HRL_GEMM_EP_STATS       C = acc, plus per-column sum and sum of squares of acc - mean over the tile's rows (mean = the
+    //                           pivot ep_mean, or 0: shifted sums keep the variance when |mean| >> std)
+    //   HRL_GEMM_EP_MASK_STATS  C = acc * (z > 0) with z = y*scale+shift of the pre-activation tile y (the ReLU
+    //                           backward), plus per-column sums of C and of C * xhat, xhat = (y - mean) * rstd
+    //                           (the two batch sums the BatchNorm backward needs)
+    float *Cg = p.C + (long long)split * p.c_split_stride;
+    const int ldt = n_pad + 4;                           // row stride = 16 (mod 128) bytes: conflict-free 16-byte stores
+    float *tile = reinterpret_cast<float *>(smem);       // the stages are free once the last MMAs have completed
+    const int ep = p.epilogue;
+    // copy-out mapping: a thread owns ONE group of 4 columns (its constants and column sums live in 16 registers) and the
+    // rows my_r, my_r + rpp, ...; consecutive threads = consecutive 16 bytes of a row, then of the next row
+    const bool vec_c = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(Cg) & 15) == 0) && (n0 % 4 == 0) && (n_here % 4 == 0);
+    const int cols4 = n_here >> 2;
+    // rows per pass; capped by the column-sum scratch the host sized for the widest tile (a narrower last tile would take more)
+    const int rpp = vec_c ? min(kGemmThreads / cols4, kGemmThreads / max(1, (n_pad - 12) / 4)) : 1;
+    const int my_r = vec_c ? tid / cols4 : 0, my_c4 = tid - my_r * cols4;
+    const bool mine = vec_c && my_r < rpp;
+    const bool masked = ep == HRL_GEMM_EP_MASK_STATS;
+    const bool vec_y = masked && (p.ep_ldy % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.ep_y) & 15) == 0);
+    constexpr int kAhead = 4;                              // rows of the pre-activation tile in flight per thread
+    float4 yq[kAhead];
+    auto load_y = [&](int r) -> float4 {
+        const float *yp = p.ep_y + (long long)(m0 + r) * p.ep_ldy + n0 + 4 * my_c4;
+        if (vec_y) return __ldg(reinterpret_cast<const float4 *>(yp));
+        return make_float4(__ldg(yp), __ldg(yp + 1), __ldg(yp + 2), __ldg(yp + 3));
+    };
+    if (masked && mine) {
+#pragma unroll
+        for (int u = 0; u < kAhead; u++) {
+            const int r = my_r + u * rpp;
+            yq[u] = r < rows_a ? load_y(r) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+    }
+    __syncthreads();                                     // every warpgroup is done with the stages
+    {
+        // accumulator fragment of m64nN: register 4 j + i holds row 16 (warp % 4) + lane / 4 + 8 (i / 2), column 8 j + 2 (lane % 4) + i % 2
+        const int r0 = (wg & 1) * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int cb = (wg >> 1) * nw + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < NW / 8; j++) {
+            const int col = cb + 8 * j;
+            float b0 = 0.f, b1 = 0.f;
+            if (p.bias != nullptr) {
+                if (col < n_here) b0 = __ldg(p.bias + n0 + col);
+                if (col + 1 < n_here) b1 = __ldg(p.bias + n0 + col + 1);
+            }
+            *reinterpret_cast<float2 *>(tile + r0 * ldt + col) = make_float2(acc[4 * j] + b0, acc[4 * j + 1] + b1);
+            *reinterpret_cast<float2 *>(tile + (r0 + 8) * ldt + col) = make_float2(acc[4 * j + 2] + b0, acc[4 * j + 3] + b1);
+        }
+    }
+    __syncthreads();
+    {
+        const bool stats = (ep == HRL_GEMM_EP_STATS || masked) && p.col_partials != nullptr;
+        float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
+        if (mine) {
+            float k_sc[4] = {1.f, 1.f, 1.f, 1.f}, k_sh[4] = {0.f, 0.f, 0.f, 0.f}, k_mu[4] = {0.f, 0.f, 0.f, 0.f}, k_rs[4] = {1.f, 1.f, 1.f, 1.f};
+            if (masked || ep == HRL_GEMM_EP_STATS) {
+#pragma unroll
+                for (int e = 0; e < 4; e++) {
+                    const int col = n0 + 4 * my_c4 + e;
+                    if (p.ep_scale) k_sc[e] = __ldg(p.ep_scale + col);
+                    if (p.ep_shift) k_sh[e] = __ldg(p.ep_shift + col);
+                    if (p.ep_mean) k_mu[e] = __ldg(p.ep_mean + col);
+                    if (p.ep_rstd) k_rs[e] = __ldg(p.ep_rstd + col);
+                }
+            }
+            for (int r0 = my_r; r0 < rows_a; r0 += kAhead * rpp) {
+#pragma unroll
+                for (int u = 0; u < kAhead; u++) {
+                    const int r = r0 + u * rpp;
+                    if (r >= rows_a) break;
+                    float4 v = reinterpret_cast<const float4 *>(tile + r * ldt)[my_c4];
+                    if (ep == HRL_GEMM_EP_RELU) {
+                        v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+                    } else if (ep == HRL_GEMM_EP_STATS) {
+                        const float d[4] = {v.x - k_mu[0], v.y - k_mu[1], v.z - k_mu[2], v.w - k_mu[3]};
+#pragma unroll
+                        for (int e = 0; e < 4; e++) {
+                            s1[e] += d[e];
+                            s2[e] = fmaf(d[e], d[e], s2[e]);
+                        }
+                    } else if (masked) {
+                        const float4 y = yq[u];
+                        const int rn = r + kAhead * rpp;
+                        if (rn < rows_a) yq[u] = load_y(rn);              // the row this slot serves next
+                        const float yv[4] = {y.x, y.y, y.z, y.w};
+                        float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                        for (int e = 0; e < 4; e++) {
+                            const float z = fmaf(yv[e], k_sc[e], k_sh[e]);
+                            const float d = z > 0.f ? vv[e] : 0.f;
+                            const float xh = (yv[e] - k_mu[e]) * k_rs[e];
+                            vv[e] = d;
+                            s1[e] += d;
+                            s2[e] = fmaf(d, xh, s2[e]);
+                        }
+                        v = make_float4(vv[0], vv[1], vv[2], vv[3]);
+                    }
+                    reinterpret_cast<float4 *>(Cg + (long long)(m0 + r) * p.ldc + n0)[my_c4] = v;
+                }
+            }
+        } else if (!vec_c) {
+            for (int r = warp; r < rows_a; r += kGemmThreads / 32) {
+                const float *src = tile + r * ldt;
+                float *dst = Cg + (long long)(m0 + r) * p.ldc + n0;
+                for (int c1 = lane; c1 < n_here; c1 += 32) dst[c1] = (ep == HRL_GEMM_EP_RELU) ? fmaxf(src[c1], 0.f) : src[c1];
+            }
+        }
+        if (stats) {       // (the statistics epilogues require vec_c: checked by the host)
+            // per-thread column sums -> shared memory (behind the tile) -> fixed-order sum over the row passes -> global partials
+            float *red = tile + kTileM * ldt;                 // [rpp][2][n_pad]
+            if (mine) {
+#pragma unroll
+                for (int e = 0; e < 4; e++) {
+                    red[(my_r * 2 + 0) * n_pad + 4 * my_c4 + e] = s1[e];
+                    red[(my_r * 2 + 1) * n_pad + 4 * my_c4 + e] = s2[e];
+                }
+            }
+            __syncthreads();
+            for (int i = tid; i < 2 * n_here; i += kGemmThreads) {
+                const int which = i / n_here, col = i - which * n_here;
+                float acc = 0.f;
+                for (int w = 0; w < rpp; w++) acc += red[(w * 2 + which) * n_pad + col];
+                p.col_partials[((long long)blockIdx.x * 2 + which) * p.N + n0 + col] = acc;
+            }
+        }
+    }
+}
+
 #ifdef HRL_GEMM_KERNEL
 // A and B go global -> registers -> (transform, hi/lo split) -> shared memory; a packed B image arrives by one bulk copy a
 // stage.  Each thread owns kItemsA items of the A tile (coalesced: 8 consecutive lanes = the 128 bytes of one k-major row,
@@ -668,7 +805,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) HRL_GEMM_KERNEL(const GemmPar
     __shared__ short conv_off_s[kConvMaxTable];
     __shared__ int conv_src_s[2][kChunkK * 9];      // conv_mode 2: source pixel of (pixel of the chunk, tap), two chunks in flight
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, warp = tid >> 5;
     const int m0 = blockIdx.x * kTileM;
     const int n0 = blockIdx.y * kMaxN;
     const int split = blockIdx.z;
@@ -923,140 +1060,54 @@ __global__ void __launch_bounds__(kGemmThreads, 1) HRL_GEMM_KERNEL(const GemmPar
     }
     wgmma_wait_all(acc);
 
-    // ---- epilogue: registers -> shared-memory tile (padded rows) -> coalesced global stores.
-    // (a thread holds 2 columns of 2 rows per 8-column group: storing from registers would scatter every warp instruction)
-    //   HRL_GEMM_EP_RELU        C = max(acc, 0)
-    //   HRL_GEMM_EP_STATS       C = acc, plus per-column sum and sum of squares of acc - mean over the tile's rows (mean = the
-    //                           pivot ep_mean, or 0: shifted sums keep the variance when |mean| >> std)
-    //   HRL_GEMM_EP_MASK_STATS  C = acc * (z > 0) with z = y*scale+shift of the pre-activation tile y (the ReLU
-    //                           backward), plus per-column sums of C and of C * xhat, xhat = (y - mean) * rstd
-    //                           (the two batch sums the BatchNorm backward needs)
-    float *Cg = p.C + (long long)split * p.c_split_stride;
-    const int ldt = n_pad + 4;                           // row stride = 16 (mod 128) bytes: conflict-free 16-byte stores
-    float *tile = reinterpret_cast<float *>(smem);       // the stages are free once the last MMAs have completed
-    const int ep = p.epilogue;
-    // copy-out mapping: a thread owns ONE group of 4 columns (its constants and column sums live in 16 registers) and the
-    // rows my_r, my_r + rpp, ...; consecutive threads = consecutive 16 bytes of a row, then of the next row
-    const bool vec_c = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(Cg) & 15) == 0) && (n0 % 4 == 0) && (n_here % 4 == 0);
-    const int cols4 = n_here >> 2;
-    // rows per pass; capped by the column-sum scratch the host sized for the widest tile (a narrower last tile would take more)
-    const int rpp = vec_c ? min(kGemmThreads / cols4, kGemmThreads / max(1, (n_pad - 12) / 4)) : 1;
-    const int my_r = vec_c ? tid / cols4 : 0, my_c4 = tid - my_r * cols4;
-    const bool mine = vec_c && my_r < rpp;
-    const bool masked = ep == HRL_GEMM_EP_MASK_STATS;
-    const bool vec_y = masked && (p.ep_ldy % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.ep_y) & 15) == 0);
-    constexpr int kAhead = 4;                              // rows of the pre-activation tile in flight per thread
-    float4 yq[kAhead];
-    auto load_y = [&](int r) -> float4 {
-        const float *yp = p.ep_y + (long long)(m0 + r) * p.ep_ldy + n0 + 4 * my_c4;
-        if (vec_y) return __ldg(reinterpret_cast<const float4 *>(yp));
-        return make_float4(__ldg(yp), __ldg(yp + 1), __ldg(yp + 2), __ldg(yp + 3));
-    };
-    if (masked && mine) {
-#pragma unroll
-        for (int u = 0; u < kAhead; u++) {
-            const int r = my_r + u * rpp;
-            yq[u] = r < rows_a ? load_y(r) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-    }
-    __syncthreads();                                     // every warpgroup is done with the stages
-    {
-        // accumulator fragment of m64nN: register 4 j + i holds row 16 (warp % 4) + lane / 4 + 8 (i / 2), column 8 j + 2 (lane % 4) + i % 2
-        const int r0 = (wg & 1) * 64 + (warp & 3) * 16 + (lane >> 2);
-        const int cb = (wg >> 1) * nw + 2 * (lane & 3);
-#pragma unroll
-        for (int j = 0; j < NW / 8; j++) {
-            const int col = cb + 8 * j;
-            float b0 = 0.f, b1 = 0.f;
-            if (p.bias != nullptr) {
-                if (col < n_here) b0 = __ldg(p.bias + n0 + col);
-                if (col + 1 < n_here) b1 = __ldg(p.bias + n0 + col + 1);
-            }
-            *reinterpret_cast<float2 *>(tile + r0 * ldt + col) = make_float2(acc[4 * j] + b0, acc[4 * j + 1] + b1);
-            *reinterpret_cast<float2 *>(tile + (r0 + 8) * ldt + col) = make_float2(acc[4 * j + 2] + b0, acc[4 * j + 3] + b1);
-        }
-    }
-    __syncthreads();
-    {
-        const bool stats = (ep == HRL_GEMM_EP_STATS || masked) && p.col_partials != nullptr;
-        float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-        if (mine) {
-            float k_sc[4] = {1.f, 1.f, 1.f, 1.f}, k_sh[4] = {0.f, 0.f, 0.f, 0.f}, k_mu[4] = {0.f, 0.f, 0.f, 0.f}, k_rs[4] = {1.f, 1.f, 1.f, 1.f};
-            if (masked || ep == HRL_GEMM_EP_STATS) {
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    const int col = n0 + 4 * my_c4 + e;
-                    if (p.ep_scale) k_sc[e] = __ldg(p.ep_scale + col);
-                    if (p.ep_shift) k_sh[e] = __ldg(p.ep_shift + col);
-                    if (p.ep_mean) k_mu[e] = __ldg(p.ep_mean + col);
-                    if (p.ep_rstd) k_rs[e] = __ldg(p.ep_rstd + col);
-                }
-            }
-            for (int r0 = my_r; r0 < rows_a; r0 += kAhead * rpp) {
-#pragma unroll
-                for (int u = 0; u < kAhead; u++) {
-                    const int r = r0 + u * rpp;
-                    if (r >= rows_a) break;
-                    float4 v = reinterpret_cast<const float4 *>(tile + r * ldt)[my_c4];
-                    if (ep == HRL_GEMM_EP_RELU) {
-                        v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
-                    } else if (ep == HRL_GEMM_EP_STATS) {
-                        const float d[4] = {v.x - k_mu[0], v.y - k_mu[1], v.z - k_mu[2], v.w - k_mu[3]};
-#pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            s1[e] += d[e];
-                            s2[e] = fmaf(d[e], d[e], s2[e]);
-                        }
-                    } else if (masked) {
-                        const float4 y = yq[u];
-                        const int rn = r + kAhead * rpp;
-                        if (rn < rows_a) yq[u] = load_y(rn);              // the row this slot serves next
-                        const float yv[4] = {y.x, y.y, y.z, y.w};
-                        float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            const float z = fmaf(yv[e], k_sc[e], k_sh[e]);
-                            const float d = z > 0.f ? vv[e] : 0.f;
-                            const float xh = (yv[e] - k_mu[e]) * k_rs[e];
-                            vv[e] = d;
-                            s1[e] += d;
-                            s2[e] = fmaf(d, xh, s2[e]);
-                        }
-                        v = make_float4(vv[0], vv[1], vv[2], vv[3]);
-                    }
-                    reinterpret_cast<float4 *>(Cg + (long long)(m0 + r) * p.ldc + n0)[my_c4] = v;
-                }
-            }
-        } else if (!vec_c) {
-            for (int r = warp; r < rows_a; r += kGemmThreads / 32) {
-                const float *src = tile + r * ldt;
-                float *dst = Cg + (long long)(m0 + r) * p.ldc + n0;
-                for (int c1 = lane; c1 < n_here; c1 += 32) dst[c1] = (ep == HRL_GEMM_EP_RELU) ? fmaxf(src[c1], 0.f) : src[c1];
-            }
-        }
-        if (stats) {       // (the statistics epilogues require vec_c: checked by the host)
-            // per-thread column sums -> shared memory (behind the tile) -> fixed-order sum over the row passes -> global partials
-            float *red = tile + kTileM * ldt;                 // [rpp][2][n_pad]
-            if (mine) {
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    red[(my_r * 2 + 0) * n_pad + 4 * my_c4 + e] = s1[e];
-                    red[(my_r * 2 + 1) * n_pad + 4 * my_c4 + e] = s2[e];
-                }
-            }
-            __syncthreads();
-            for (int i = tid; i < 2 * n_here; i += kGemmThreads) {
-                const int which = i / n_here, col = i - which * n_here;
-                float acc = 0.f;
-                for (int w = 0; w < rpp; w++) acc += red[(w * 2 + which) * n_pad + col];
-                p.col_partials[((long long)blockIdx.x * 2 + which) * p.N + n0 + col] = acc;
-            }
-        }
+    gemm_epilogue<NW>(p, acc, smem, m0, rows_a, n0, n_here, split);
+}
+
+template <bool A_K, bool B_K, bool PACKED, int NW>
+static int launch_gemm(const GemmParams &p, dim3 grid, size_t smem_bytes, cudaStream_t stream) {
+    HRL_CUDA_CHECK(cudaFuncSetAttribute(HRL_GEMM_KERNEL<A_K, B_K, PACKED, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
+    HRL_GEMM_KERNEL<A_K, B_K, PACKED, NW><<<grid, kGemmThreads, smem_bytes, stream>>>(p);
+    return HRL_OK;
+}
+
+// the operand layouts of one MMA width (a packed B image is k-major)
+template <int NW>
+static int launch_gemm_width(const GemmParams &p, dim3 grid, size_t smem_bytes, cudaStream_t stream) {
+    if (p.b.packed) return p.a.kmajor ? launch_gemm<true, true, true, NW>(p, grid, smem_bytes, stream)
+                                      : launch_gemm<false, true, true, NW>(p, grid, smem_bytes, stream);
+    if (p.a.kmajor) return p.b.kmajor ? launch_gemm<true, true, false, NW>(p, grid, smem_bytes, stream)
+                                      : launch_gemm<true, false, false, NW>(p, grid, smem_bytes, stream);
+    return p.b.kmajor ? launch_gemm<false, true, false, NW>(p, grid, smem_bytes, stream)
+                      : launch_gemm<false, false, false, NW>(p, grid, smem_bytes, stream);
+}
+
+int HRL_GEMM_LAUNCH(const GemmParams &p, int nw, dim3 grid, size_t smem_bytes, cudaStream_t stream) {
+    switch (nw) {                 // the MMA width of a warpgroup: half of n_pad, a multiple of 16 up to 256, then 288
+    case 8: return launch_gemm_width<8>(p, grid, smem_bytes, stream);
+    case 16: return launch_gemm_width<16>(p, grid, smem_bytes, stream);
+    case 24: return launch_gemm_width<24>(p, grid, smem_bytes, stream);
+    case 32: return launch_gemm_width<32>(p, grid, smem_bytes, stream);
+    case 40: return launch_gemm_width<40>(p, grid, smem_bytes, stream);
+    case 48: return launch_gemm_width<48>(p, grid, smem_bytes, stream);
+    case 56: return launch_gemm_width<56>(p, grid, smem_bytes, stream);
+    case 64: return launch_gemm_width<64>(p, grid, smem_bytes, stream);
+    case 72: return launch_gemm_width<72>(p, grid, smem_bytes, stream);
+    case 80: return launch_gemm_width<80>(p, grid, smem_bytes, stream);
+    case 88: return launch_gemm_width<88>(p, grid, smem_bytes, stream);
+    case 96: return launch_gemm_width<96>(p, grid, smem_bytes, stream);
+    case 104: return launch_gemm_width<104>(p, grid, smem_bytes, stream);
+    case 112: return launch_gemm_width<112>(p, grid, smem_bytes, stream);
+    case 120: return launch_gemm_width<120>(p, grid, smem_bytes, stream);
+    case 128: return launch_gemm_width<128>(p, grid, smem_bytes, stream);
+    case 144: return launch_gemm_width<144>(p, grid, smem_bytes, stream);
+    default: HRL_REQUIRE(false, HRL_ERR_BAD_ARG, "hrl_gemm_fused: no kernel for an MMA width of %d columns", nw);
     }
 }
 #endif  // HRL_GEMM_KERNEL
 
-// the bf16 entry points (csrc/gemm_bf16_kernel.cu): launches gemm_bf16_kernel of MMA width nw for p's operand layouts
+// the entry points of the two precisions (csrc/gemm_kernel.cu, csrc/gemm_bf16_kernel.cu): launch the kernel of MMA width nw
+// for p's operand layouts
+int launch_gemm_tf32x3(const GemmParams &p, int nw, dim3 grid, size_t smem_bytes, cudaStream_t stream);
 int launch_gemm_bf16(const GemmParams &p, int nw, dim3 grid, size_t smem_bytes, cudaStream_t stream);
 
 }  // namespace hrl

@@ -29,8 +29,9 @@
 #include <stdint.h>
 #include <string.h>
 
-#define HRL_GEMM_KERNEL gemm_tf32x3_kernel     // the kernel template gemm_common.cuh defines, and its operand precision
+#define HRL_GEMM_KERNEL gemm_tf32x3_kernel     // the kernel template gemm_common.cuh defines, its operand precision and launcher
 #define HRL_GEMM_BF16 false
+#define HRL_GEMM_LAUNCH launch_gemm_tf32x3
 #include "gemm_common.cuh"
 #include "gemm_tower.cuh"
 #include "gemm_wgrad.cuh"
@@ -48,24 +49,6 @@ __global__ void sum_partials_kernel(const float *__restrict__ partials, int spli
         for (int k = 1; k < splits; k++) s += partials[(long long)k * stride + i];
         out[i] = s;
     }
-}
-
-template <bool A_K, bool B_K, bool PACKED, int NW>
-static int launch_gemm(const GemmParams &p, dim3 grid, size_t smem_bytes, cudaStream_t stream) {
-    HRL_CUDA_CHECK(cudaFuncSetAttribute(gemm_tf32x3_kernel<A_K, B_K, PACKED, NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-    gemm_tf32x3_kernel<A_K, B_K, PACKED, NW><<<grid, kGemmThreads, smem_bytes, stream>>>(p);
-    return HRL_OK;
-}
-
-// the operand layouts of one MMA width (a packed B image is k-major)
-template <int NW>
-static int launch_gemm_width(const GemmParams &p, dim3 grid, size_t smem_bytes, cudaStream_t stream) {
-    if (p.b.packed) return p.a.kmajor ? launch_gemm<true, true, true, NW>(p, grid, smem_bytes, stream)
-                                      : launch_gemm<false, true, true, NW>(p, grid, smem_bytes, stream);
-    if (p.a.kmajor) return p.b.kmajor ? launch_gemm<true, true, false, NW>(p, grid, smem_bytes, stream)
-                                      : launch_gemm<true, false, false, NW>(p, grid, smem_bytes, stream);
-    return p.b.kmajor ? launch_gemm<false, true, false, NW>(p, grid, smem_bytes, stream)
-                      : launch_gemm<false, false, false, NW>(p, grid, smem_bytes, stream);
 }
 
 }  // namespace hrl
@@ -186,26 +169,7 @@ extern "C" int hrl_gemm_fused(const HrlGemmArgs *args, void *stream_) {
     if (gemm_tower_applies(g)) st = launch_gemm_tower(p, stream);
     else if (gemm_wgrad_applies(g)) st = launch_gemm_wgrad(g, p.chunks_per_split, splits, p.C, p.ldc, p.c_split_stride, p.debug, stream);
     else if (g.bf16) st = launch_gemm_bf16(p, n_pad / 2, grid, smem_bytes, stream);
-    else switch (n_pad / 2) {          // the MMA width of a warpgroup: n_pad is a multiple of 16 up to 256, then 288
-    case 8: st = launch_gemm_width<8>(p, grid, smem_bytes, stream); break;
-    case 16: st = launch_gemm_width<16>(p, grid, smem_bytes, stream); break;
-    case 24: st = launch_gemm_width<24>(p, grid, smem_bytes, stream); break;
-    case 32: st = launch_gemm_width<32>(p, grid, smem_bytes, stream); break;
-    case 40: st = launch_gemm_width<40>(p, grid, smem_bytes, stream); break;
-    case 48: st = launch_gemm_width<48>(p, grid, smem_bytes, stream); break;
-    case 56: st = launch_gemm_width<56>(p, grid, smem_bytes, stream); break;
-    case 64: st = launch_gemm_width<64>(p, grid, smem_bytes, stream); break;
-    case 72: st = launch_gemm_width<72>(p, grid, smem_bytes, stream); break;
-    case 80: st = launch_gemm_width<80>(p, grid, smem_bytes, stream); break;
-    case 88: st = launch_gemm_width<88>(p, grid, smem_bytes, stream); break;
-    case 96: st = launch_gemm_width<96>(p, grid, smem_bytes, stream); break;
-    case 104: st = launch_gemm_width<104>(p, grid, smem_bytes, stream); break;
-    case 112: st = launch_gemm_width<112>(p, grid, smem_bytes, stream); break;
-    case 120: st = launch_gemm_width<120>(p, grid, smem_bytes, stream); break;
-    case 128: st = launch_gemm_width<128>(p, grid, smem_bytes, stream); break;
-    case 144: st = launch_gemm_width<144>(p, grid, smem_bytes, stream); break;
-    default: HRL_REQUIRE(false, HRL_ERR_BAD_ARG, "hrl_gemm_fused: no kernel for a tile of %d padded columns", n_pad);
-    }
+    else st = launch_gemm_tf32x3(p, n_pad / 2, grid, smem_bytes, stream);
     if (st != HRL_OK) return st;
     HRL_CUDA_CHECK(cudaGetLastError());
     if (splits > 1 && g.C != nullptr) {       // C == NULL: the caller consumes the slice partials itself (hrl_board_fold)

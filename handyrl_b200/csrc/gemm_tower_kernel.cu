@@ -6,7 +6,7 @@
 // hi / lo, store both halves swizzled, two CTA barriers, then the MMAs.  Only one chunk of A is in flight, and at the
 // tower's shape there is one 128-row tile per SM, so the global-load latency is exposed in every chunk.  Here:
 //   * tile and warps as in the wgmma kernel: 128 rows x 288 columns, 4 warpgroups, warpgroup wg owns rows 64 (wg & 1) ...
-//     and columns 144 (wg >> 1) ..., 72 fp32 accumulators a thread; the epilogue is a copy of the wgmma kernel's;
+//     and columns 144 (wg >> 1) ..., 72 fp32 accumulators a thread; the epilogue is the wgmma kernel's (gemm_epilogue);
 //   * A staging: every 32-element chunk is copied raw by 16-byte cp.async into shared rows padded to 36 floats, several
 //     chunks ahead (3 stages for one source; 2 for two sources, the input gradient's dZ and Y).  A fragment load of
 //     (row 16 w + g, k t) hits bank (4 g + t) mod 32: 32 distinct banks.  Copies stay inside the operand (rows < M, 16-byte
@@ -54,7 +54,7 @@ static_assert(1024 + ((size_t)kTileM * (2 * kNW + 4) + 2 * 7 * 2 * kNW) * 4 <= R
 static_assert(Ring<2>::smem + 3 * kMaxConstK * 4 + 64 <= 232448, "shared memory of one block");
 
 // D[64 x 144] += A[64 x 8] * B[144 x 8]^T: A from registers (the .tf32 fragment: rows g, g + 8, k t, t + 4), B in shared memory
-__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[72], const uint32_t (&a)[4], uint64_t b_desc) {
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[72], const float (&a)[4], uint64_t b_desc) {
     asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %77, 0;\n\t"
                  "wgmma.mma_async.sync.aligned.m64n144k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71}, {%72, %73, %74, %75}, %76, p, 1, 1;\n\t}"
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]),
@@ -63,148 +63,9 @@ __device__ __forceinline__ void wgmma_tf32_rs(float (&d)[72], const uint32_t (&a
                    "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
                    "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]),
                    "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(1)
+                 : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])),
+                   "l"(b_desc), "r"(1)
                  : "memory");
-}
-
-// ---- the epilogue of the wgmma kernel (gemm_common.cuh), copied: the accumulators of warpgroup wg cover rows 64 (wg & 1) ...
-// and columns 144 (wg >> 1) ... of the tile; registers -> shared-memory tile (padded rows) -> coalesced global stores, the
-// same copy-out mapping and the same fixed-order column sums.  (Moved into one __device__ __forceinline__ helper that both
-// kernels call, it changes the register allocation of
-// dozens of the wgmma kernel's instantiations, the flagship's among them.)
-__device__ __forceinline__ void epilogue(const GemmParams &p, float (&acc)[kNW / 2], uint8_t *smem, int m0, int rows_a) {
-    constexpr int NW = kNW, n_pad = 2 * NW, nw = NW;
-    const int n0 = 0, n_here = p.N, split = 0;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wg = warp >> 2;
-    // (a thread holds 2 columns of 2 rows per 8-column group: storing from registers would scatter every warp instruction)
-    //   HRL_GEMM_EP_RELU        C = max(acc, 0)
-    //   HRL_GEMM_EP_STATS       C = acc, plus per-column sum and sum of squares of acc - mean over the tile's rows (mean = the
-    //                           pivot ep_mean, or 0: shifted sums keep the variance when |mean| >> std)
-    //   HRL_GEMM_EP_MASK_STATS  C = acc * (z > 0) with z = y*scale+shift of the pre-activation tile y (the ReLU
-    //                           backward), plus per-column sums of C and of C * xhat, xhat = (y - mean) * rstd
-    //                           (the two batch sums the BatchNorm backward needs)
-    float *Cg = p.C + (long long)split * p.c_split_stride;
-    const int ldt = n_pad + 4;                           // row stride = 16 (mod 128) bytes: conflict-free 16-byte stores
-    float *tile = reinterpret_cast<float *>(smem);       // the stages are free once the last MMAs have completed
-    const int ep = p.epilogue;
-    // copy-out mapping: a thread owns ONE group of 4 columns (its constants and column sums live in 16 registers) and the
-    // rows my_r, my_r + rpp, ...; consecutive threads = consecutive 16 bytes of a row, then of the next row
-    const bool vec_c = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(Cg) & 15) == 0) && (n0 % 4 == 0) && (n_here % 4 == 0);
-    const int cols4 = n_here >> 2;
-    // rows per pass; capped by the column-sum scratch the host sized for the widest tile (a narrower last tile would take more)
-    const int rpp = vec_c ? min(kGemmThreads / cols4, kGemmThreads / max(1, (n_pad - 12) / 4)) : 1;
-    const int my_r = vec_c ? tid / cols4 : 0, my_c4 = tid - my_r * cols4;
-    const bool mine = vec_c && my_r < rpp;
-    const bool masked = ep == HRL_GEMM_EP_MASK_STATS;
-    const bool vec_y = masked && (p.ep_ldy % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.ep_y) & 15) == 0);
-    constexpr int kAhead = 4;                              // rows of the pre-activation tile in flight per thread
-    float4 yq[kAhead];
-    auto load_y = [&](int r) -> float4 {
-        const float *yp = p.ep_y + (long long)(m0 + r) * p.ep_ldy + n0 + 4 * my_c4;
-        if (vec_y) return __ldg(reinterpret_cast<const float4 *>(yp));
-        return make_float4(__ldg(yp), __ldg(yp + 1), __ldg(yp + 2), __ldg(yp + 3));
-    };
-    if (masked && mine) {
-#pragma unroll
-        for (int u = 0; u < kAhead; u++) {
-            const int r = my_r + u * rpp;
-            yq[u] = r < rows_a ? load_y(r) : make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-    }
-    __syncthreads();                                     // every warpgroup is done with the stages
-    {
-        // accumulator fragment of m64nN: register 4 j + i holds row 16 (warp % 4) + lane / 4 + 8 (i / 2), column 8 j + 2 (lane % 4) + i % 2
-        const int r0 = (wg & 1) * 64 + (warp & 3) * 16 + (lane >> 2);
-        const int cb = (wg >> 1) * nw + 2 * (lane & 3);
-#pragma unroll
-        for (int j = 0; j < NW / 8; j++) {
-            const int col = cb + 8 * j;
-            float b0 = 0.f, b1 = 0.f;
-            if (p.bias != nullptr) {
-                if (col < n_here) b0 = __ldg(p.bias + n0 + col);
-                if (col + 1 < n_here) b1 = __ldg(p.bias + n0 + col + 1);
-            }
-            *reinterpret_cast<float2 *>(tile + r0 * ldt + col) = make_float2(acc[4 * j] + b0, acc[4 * j + 1] + b1);
-            *reinterpret_cast<float2 *>(tile + (r0 + 8) * ldt + col) = make_float2(acc[4 * j + 2] + b0, acc[4 * j + 3] + b1);
-        }
-    }
-    __syncthreads();
-    {
-        const bool stats = (ep == HRL_GEMM_EP_STATS || masked) && p.col_partials != nullptr;
-        float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
-        if (mine) {
-            float k_sc[4] = {1.f, 1.f, 1.f, 1.f}, k_sh[4] = {0.f, 0.f, 0.f, 0.f}, k_mu[4] = {0.f, 0.f, 0.f, 0.f}, k_rs[4] = {1.f, 1.f, 1.f, 1.f};
-            if (masked || ep == HRL_GEMM_EP_STATS) {
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    const int col = n0 + 4 * my_c4 + e;
-                    if (p.ep_scale) k_sc[e] = __ldg(p.ep_scale + col);
-                    if (p.ep_shift) k_sh[e] = __ldg(p.ep_shift + col);
-                    if (p.ep_mean) k_mu[e] = __ldg(p.ep_mean + col);
-                    if (p.ep_rstd) k_rs[e] = __ldg(p.ep_rstd + col);
-                }
-            }
-            for (int r0 = my_r; r0 < rows_a; r0 += kAhead * rpp) {
-#pragma unroll
-                for (int u = 0; u < kAhead; u++) {
-                    const int r = r0 + u * rpp;
-                    if (r >= rows_a) break;
-                    float4 v = reinterpret_cast<const float4 *>(tile + r * ldt)[my_c4];
-                    if (ep == HRL_GEMM_EP_RELU) {
-                        v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
-                    } else if (ep == HRL_GEMM_EP_STATS) {
-                        const float d[4] = {v.x - k_mu[0], v.y - k_mu[1], v.z - k_mu[2], v.w - k_mu[3]};
-#pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            s1[e] += d[e];
-                            s2[e] = fmaf(d[e], d[e], s2[e]);
-                        }
-                    } else if (masked) {
-                        const float4 y = yq[u];
-                        const int rn = r + kAhead * rpp;
-                        if (rn < rows_a) yq[u] = load_y(rn);              // the row this slot serves next
-                        const float yv[4] = {y.x, y.y, y.z, y.w};
-                        float vv[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                        for (int e = 0; e < 4; e++) {
-                            const float z = fmaf(yv[e], k_sc[e], k_sh[e]);
-                            const float d = z > 0.f ? vv[e] : 0.f;
-                            const float xh = (yv[e] - k_mu[e]) * k_rs[e];
-                            vv[e] = d;
-                            s1[e] += d;
-                            s2[e] = fmaf(d, xh, s2[e]);
-                        }
-                        v = make_float4(vv[0], vv[1], vv[2], vv[3]);
-                    }
-                    reinterpret_cast<float4 *>(Cg + (long long)(m0 + r) * p.ldc + n0)[my_c4] = v;
-                }
-            }
-        } else if (!vec_c) {
-            for (int r = warp; r < rows_a; r += kGemmThreads / 32) {
-                const float *src = tile + r * ldt;
-                float *dst = Cg + (long long)(m0 + r) * p.ldc + n0;
-                for (int c1 = lane; c1 < n_here; c1 += 32) dst[c1] = (ep == HRL_GEMM_EP_RELU) ? fmaxf(src[c1], 0.f) : src[c1];
-            }
-        }
-        if (stats) {       // (the statistics epilogues require vec_c: checked by the host)
-            // per-thread column sums -> shared memory (behind the tile) -> fixed-order sum over the row passes -> global partials
-            float *red = tile + kTileM * ldt;                 // [rpp][2][n_pad]
-            if (mine) {
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    red[(my_r * 2 + 0) * n_pad + 4 * my_c4 + e] = s1[e];
-                    red[(my_r * 2 + 1) * n_pad + 4 * my_c4 + e] = s2[e];
-                }
-            }
-            __syncthreads();
-            for (int i = tid; i < 2 * n_here; i += kGemmThreads) {
-                const int which = i / n_here, col = i - which * n_here;
-                float acc = 0.f;
-                for (int w = 0; w < rpp; w++) acc += red[(w * 2 + which) * n_pad + col];
-                p.col_partials[((long long)blockIdx.x * 2 + which) * p.N + n0 + col] = acc;
-            }
-        }
-    }
 }
 
 template <int KIND>
@@ -274,7 +135,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tower_kernel(const GemmP
     float acc[kNW / 2];
 #pragma unroll
     for (int i = 0; i < kNW / 2; i++) acc[i] = 0.f;
-    uint32_t a_hi[2][4], a_lo[2][4];                       // fragment registers, double-buffered across the k8 steps
+    float a_hi[2][4], a_lo[2][4];                          // fragment registers, double-buffered across the k8 steps
 
     const int ra = (wg & 1) * 64 + (warp & 3) * 16 + g;    // the thread's fragment rows ra, ra + 8 inside the tile
     const bool live0 = ra < rows_a, live1 = ra + 8 < rows_a;
@@ -324,10 +185,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tower_kernel(const GemmP
 #pragma unroll
             for (int e = 0; e < 4; e++) asm volatile("" : "+f"(v[e]));
 #pragma unroll
-            for (int e = 0; e < 4; e++) {
-                a_hi[buf][e] = __float_as_uint(v[e]) & 0xFFFFE000u;
-                a_lo[buf][e] = __float_as_uint(v[e] - __uint_as_float(a_hi[buf][e]));
-            }
+            for (int e = 0; e < 4; e++) split_tf32(v[e], a_hi[buf][e], a_lo[buf][e]);
             if ((p.debug & 3) != 1) {
                 wgmma_fence();
                 wgmma_tf32_rs(acc, a_lo[buf], wgmma_desc(b_hi + 32 * ks));
@@ -350,7 +208,7 @@ __global__ void __launch_bounds__(kGemmThreads, 1) gemm_tower_kernel(const GemmP
     wgmma_wait_all(acc);
     cp_async_wait<0>();
 
-    epilogue(p, acc, smem, m0, rows_a);
+    gemm_epilogue<kNW>(p, acc, smem, m0, rows_a, 0, p.N, 0);
 }
 
 template <int KIND>

@@ -14,7 +14,7 @@
 //     output columns of 2 consecutive rows (16-byte stores).  Which hardware lane computes an output does not change it;
 //   * operand transform on fragment load: x*p + y*q + r (A: the BatchNorm backward of two sources) or x*p + r (B: the
 //     previous layer's BatchNorm-apply) with per-row constants held in registers, optional ReLU, then the hi/lo split of
-//     split_tf32 (gemm_common.cuh), so the tensor core gets the values the wgmma kernel gives it.  Per k8 step the three
+//     split_tf32 (common.cuh), so the tensor core gets the values the wgmma kernel gives it.  Per k8 step the three
 //     products run in the wgmma kernel's order: a_lo*b_hi, a_hi*b_lo, a_hi*b_hi;
 //   * tile: 96 rows x 288 columns x one K slice of `chunks_per_split` chunks, 12 warps of 48 x 48 (2 x 6), 72 fp32
 //     accumulators a thread.  A warp whose rows or columns lie past the operand skips its MMAs: a 27-row product pays for
@@ -63,16 +63,11 @@ __device__ __forceinline__ float transform(float x, float y, float p, float q, f
     return relu ? fmaxf(v, 0.f) : v;
 }
 
-// the 3xTF32 split of gemm_common.cuh's split_tf32: hi = the 13 low mantissa bits cleared, lo = v - hi (exact)
-__device__ __forceinline__ void split(float v, uint32_t &hi, uint32_t &lo) {
-    hi = __float_as_uint(v) & 0xFFFFE000u;
-    lo = __float_as_uint(v - __uint_as_float(hi));
-}
-
-__device__ __forceinline__ void mma_tf32(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+__device__ __forceinline__ void mma_tf32(float (&d)[4], const float (&a)[4], float b0, float b1) {
     asm("mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+        : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])),
+          "r"(__float_as_uint(b0)), "r"(__float_as_uint(b1)));
 }
 
 // per-row constants of this thread's 6 rows of an operand (rows 16 i + 2 g + e of the warp's 48, i < 3, e < 2): p, q, r
@@ -103,7 +98,7 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[3][6][4], const float *st
     for (int ks = 0; ks < kChunk / 8; ks++) {
         const int k0 = 8 * ks + t, k1 = k0 + 4;
         const bool v0 = !TAIL || k0 < k_left, v1 = !TAIL || k1 < k_left;
-        uint32_t ahi[3][4], alo[3][4];
+        float ahi[3][4], alo[3][4];
 #pragma unroll
         for (int i = 0; i < 3; i++) {
             const int m = mw + 16 * i + 2 * g;
@@ -122,7 +117,7 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[3][6][4], const float *st
                 if (!v1) v[2] = v[3] = 0.f;
             }
 #pragma unroll
-            for (int e = 0; e < 4; e++) split(v[e], ahi[i][e], alo[i][e]);
+            for (int e = 0; e < 4; e++) split_tf32(v[e], ahi[i][e], alo[i][e]);
         }
 #pragma unroll
         for (int jp = 0; jp < 3; jp++) {
@@ -138,11 +133,11 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[3][6][4], const float *st
                 if (!v0) v[0][0] = v[1][0] = 0.f;
                 if (!v1) v[0][1] = v[1][1] = 0.f;
             }
-            uint32_t bhi[2][2], blo[2][2];
+            float bhi[2][2], blo[2][2];
 #pragma unroll
             for (int j = 0; j < 2; j++)
 #pragma unroll
-                for (int h = 0; h < 2; h++) split(v[j][h], bhi[j][h], blo[j][h]);
+                for (int h = 0; h < 2; h++) split_tf32(v[j][h], bhi[j][h], blo[j][h]);
             // small terms first, as the wgmma kernel: a_lo*b_hi, a_hi*b_lo, a_hi*b_hi
 #pragma unroll
             for (int i = 0; i < 3; i++)

@@ -41,12 +41,13 @@ __host__ __device__ __forceinline__ int hrl_padded_rows_dev(int N) {      // == 
 // dense element (row = (o,q), col = (i,p)) of the convolution, straight into packed B-operand images of the wgmma GEMM
 // (csrc/gemm_kernel.cu): image[chunk = k / 32][hi | lo][row][slot (k % 32) / 4 ^ (row & 7)][k % 4]
 __device__ __forceinline__ void pack_store(float *image, int n_pad, int row, int k, float v) {
-    const float hi = __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
+    float hi, lo;
+    split_tf32(v, hi, lo);
     const long long chunk = k >> 5;
     const int j = (k & 31) >> 2, e = k & 3;
     float *base = image + chunk * (2ll * n_pad * 32) + (long long)row * 32 + (((j ^ (row & 7)) << 2) + e);
     base[0] = hi;
-    base[(long long)n_pad * 32] = v - hi;
+    base[(long long)n_pad * 32] = lo;
 }
 
 // the same element in a bf16 image (HrlGemmArgs.bf16): image[chunk][row][64 bytes, slot (k % 32) / 8 ^ ((row >> 1) & 3)][k % 8]
