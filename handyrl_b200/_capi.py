@@ -76,6 +76,8 @@ class HrlGemmArgs(C.Structure):
 
 
 MAX_BOARD_JOBS = 8
+# rows of a packed board-convolution image (hrl_board_pack_many, hrl_gemm_fused's packed B operand): features x cells
+MAX_BOARD_ROWS = 288
 
 
 class HrlPackJob(C.Structure):

@@ -26,7 +26,7 @@ import ctypes as C
 import torch
 
 from . import _capi, nets
-from ._capi import GEMM_EPILOGUES, MAX_BOARD_JOBS, HrlFoldJob, HrlGemmArgs, HrlPackJob, check, lib
+from ._capi import GEMM_EPILOGUES, MAX_BOARD_JOBS, MAX_BOARD_ROWS, HrlFoldJob, HrlGemmArgs, HrlPackJob, check, lib
 from .ops import _count, _ptr, _stream_ptr
 
 
@@ -40,10 +40,15 @@ def _operand(o, t, t2=None, consts=None, relu=False, kmajor=True, by_row=False, 
 
 
 def supports(model):
-    """The engine covers nets.BoardNet as it stands (3x3 convolutions with BatchNorm in the tower, 1x1 squeeze heads)."""
+    """The engine covers nets.BoardNet as it stands (3x3 convolutions with BatchNorm in the tower, 1x1 squeeze heads) when every
+    convolution's packed image fits (width x cells <= MAX_BOARD_ROWS rows) and the heads fit their kernels (at most 16 cells,
+    64 squeeze outputs and 32 actions).  Each tower BatchNorm must be affine, track running statistics and have a numeric
+    momentum: the engine reads its weight, bias and running buffers and applies the momentum update."""
     if type(model) is not nets.BoardNet or len(model.tower) == 0:
         return False
     if not all(len(blk) == 2 and isinstance(blk[1], torch.nn.BatchNorm2d) for blk in model.tower):
+        return False
+    if not all(bn.affine and bn.track_running_stats and isinstance(bn.momentum, (int, float)) for bn in (blk[1] for blk in model.tower)):
         return False
     if model.stem.kernel_size != (3, 3) or any(blk[0].kernel_size != (3, 3) or blk[0].bias is not None for blk in model.tower):
         return False
@@ -51,7 +56,7 @@ def supports(model):
     dense = model.stem.out_channels * cells
     heads = (model.p_squeeze.out_channels + model.v_squeeze.out_channels +
              (model.r_squeeze.out_channels if model.r_squeeze is not None else 0)) * cells
-    return cells <= 16 and dense % 4 == 0 and dense * dense <= (1 << 20) and heads <= 64 and model.p_out.out_features <= 32
+    return cells <= 16 and dense % 4 == 0 and dense <= MAX_BOARD_ROWS and heads <= 64 and model.p_out.out_features <= 32
 
 
 class FusedBoardNet:

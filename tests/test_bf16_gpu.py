@@ -16,11 +16,9 @@ import torch
 import torch.nn.functional as F
 
 from conftest import GOLDEN
+from tower_ref import U16, U32, _close, _conv, _conv_in, _conv_w, _transform_ref, _wgrad_bound, accum_bound, r16
 
 pytestmark = pytest.mark.gpu
-
-U32 = 2.0 ** -23          # fp32 accumulation, truncating: relative error of one addition
-U16 = 2.0 ** -8           # bf16 round to nearest: relative error of one rounding <= 2^-9 (8 stored mantissa bits)
 
 # the shapes of test_gemm_gpu.py: M, N, K, a_kmajor, b_kmajor, bias, splits
 CASES = [
@@ -35,18 +33,6 @@ CASES = [
     (64, 16, 8, True, True, False, 1),
     (129, 272, 40, False, True, False, 2),
 ]
-
-
-def r16(t):
-    """t rounded to bf16 (nearest even), as float64"""
-    return t.bfloat16().double()
-
-
-def accum_bound(K, splits=1):
-    """fp32 accumulation error of K exact terms in `splits` K slices, relative to sum|a||b| (test_gemm_gpu.py)"""
-    from handyrl_b200._capi import lib
-    k_slice = -(-K // lib().hrl_gemm_effective_splits(K, splits))
-    return 1.2e-7 * (0.8 * k_slice ** 0.5 + 4)
 
 
 @pytest.mark.parametrize('M,N,K,a_k,b_k,with_bias,splits', CASES)
@@ -152,19 +138,6 @@ def test_conv_pack_bf16_images(Cout, Cin, taps):
     wb = w.bfloat16()
     assert torch.equal(unpack(fwd, Cout, Cin), wb.reshape(Cout, Cin, taps).permute(0, 2, 1))
     assert torch.equal(unpack(adj, Cin, Cout), wb.reshape(Cout, Cin, taps).flip(2).permute(1, 2, 0))
-
-
-def _transform_ref(x, p, r, y=None, q=None, relu=False):
-    """the kernel's operand transform fmaf(x, p, fmaf(y, q, r)) in float32 (each fmaf exact in float64, rounded once), then
-    bf16 rounding; also the elements whose float32 value sits at a bf16 rounding boundary (one float32 ulp decides them)"""
-    inner = r.double() if y is None else (y.double() * q.double() + r.double()).float().double()
-    t = (x.double() * p.double() + inner).float()
-    if relu:
-        t = t.clamp_min(0)
-    up, dn = torch.nextafter(t, torch.full_like(t, float('inf'))), torch.nextafter(t, torch.full_like(t, -float('inf')))
-    edge = up.bfloat16() != dn.bfloat16()
-    ulp = (t.abs().bfloat16().float() * 2.0 ** -7).double()          # at most one bf16 ulp of the element
-    return r16(t), torch.where(edge, ulp, torch.zeros_like(ulp))
 
 
 @pytest.mark.parametrize('epilogue', ['stats', 'mask_stats'])
@@ -379,29 +352,6 @@ def test_bf16_graph_and_eager_steps_are_bit_identical():
 
 
 # ---- the dense small-board convolution and the fused tower, product by product ----------------------------------------
-def _conv(a, w, b=None):
-    return F.conv2d(a, w, b, padding=w.shape[-1] // 2)
-
-
-def _conv_in(shape, w, dy):
-    return torch.nn.grad.conv2d_input(shape, w, dy, padding=w.shape[-1] // 2)
-
-
-def _conv_w(a, shape, dy):
-    return torch.nn.grad.conv2d_weight(a, shape, dy, padding=shape[-1] // 2)
-
-
-def _close(got, want, bound, what):
-    err = (got.double() - want).abs()
-    assert (err <= bound).all(), (what, (err - bound).max().item(), (err / (bound + 1e-300)).max().item())
-
-
-def _wgrad_bound(K, splits, cells):
-    """a weight gradient of the dense products: K samples in `splits` slices, then hrl_board_fold's fp32 sums over the
-    slices and over the output cells"""
-    return accum_bound(K, splits) + (splits + cells + 1) * U32
-
-
 @pytest.mark.parametrize('N', [100, 2048])
 def test_board_conv_bf16_against_float64(N):
     """ops.board_conv in bf16 mode (the dense small-board convolution of fastnet, TicTacToe-sized boards): forward, input

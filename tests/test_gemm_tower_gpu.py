@@ -10,11 +10,11 @@ relu(x*p + r), or x*p + y*q + r of two sources, per reduction index) times a pac
   forward on the wgmma kernel (traced with torch.profiler).
 """
 import ctypes as C
-import re
-import time
 
 import pytest
 import torch
+
+from tower_ref import traced_gemms
 
 pytestmark = pytest.mark.gpu
 
@@ -207,29 +207,6 @@ def test_two_launches_are_bit_identical():
     (c1, p1), (c2, p2) = launch(c, 'mask_stats', ep), launch(c, 'mask_stats', ep)
     torch.cuda.synchronize()
     assert torch.equal(c1.view(torch.int32), c2.view(torch.int32)) and torch.equal(p1.view(torch.int32), p2.view(torch.int32))
-
-
-_GEMM_RE = re.compile(r'(gemm_tower_kernel|gemm_wgrad_kernel|gemm_tf32x3_kernel)<([^>]*)>')
-
-
-def traced_gemms(fn, attempts=3):
-    """The GEMM kernels fn() launches, as {(kernel, template arguments)} from a torch.profiler (CUPTI) trace (taken again when
-    the tracer dropped every GEMM record)."""
-    acts = [torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA]
-    seen = set()
-    for _ in range(attempts):
-        with torch.profiler.profile(activities=acts) as prof:
-            fn()
-            torch.cuda.synchronize()
-            time.sleep(0.002)
-        names = set()
-        for e in prof.events():
-            names.add(e.name)
-            names.update(k.name for k in getattr(e, 'kernels', []))
-        seen = {(m.group(1), m.group(2).replace(' ', '')) for m in map(_GEMM_RE.search, names) if m}
-        if seen:
-            break
-    return seen
 
 
 def test_fused_tower_dispatch():
