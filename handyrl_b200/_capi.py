@@ -125,6 +125,16 @@ class HrlReplaySampleArgs(C.Structure):
     ]
 
 
+class HrlDistillArgs(C.Structure):
+    _fields_ = [
+        ('B', C.c_int32), ('T', C.c_int32), ('P', C.c_int32), ('Pa', C.c_int32), ('A', C.c_int32), ('burn_in', C.c_int32),
+        ('policy_raw', C.c_void_p), ('teacher_raw', C.c_void_p), ('action_mask', C.c_void_p), ('turn_mask', C.c_void_p),
+        ('window_weight', C.c_void_p), ('step_count', C.c_void_p), ('coef', C.c_float), ('anneal_steps', C.c_int64),
+        ('dpolicy_raw', C.c_void_p), ('losses', C.c_void_p), ('sums', C.c_void_p),
+        ('workspace', C.c_void_p), ('workspace_bytes', C.c_size_t), ('io_bf16', C.c_int32),
+    ]
+
+
 # every symbol include/hrl_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     'hrl_loss_workspace_bytes': (C.c_size_t, [C.c_int32] * 5),
@@ -193,6 +203,8 @@ SYMBOLS = {
     'hrl_hidden_visible_bwd': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     'hrl_hidden_blend_fwd': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     'hrl_hidden_blend_bwd': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
+    'hrl_distill_workspace_bytes': (C.c_size_t, [C.c_int32] * 5),
+    'hrl_distill_fwd_bwd': (C.c_int, [C.POINTER(HrlDistillArgs), C.c_void_p]),
     'hrl_last_error': (C.c_char_p, []),
     'hrl_abi_version': (C.c_int32, []),
 }

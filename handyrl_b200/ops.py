@@ -220,6 +220,60 @@ def _launch(a, buffers, form):
     _count()
 
 
+def distill_fwd_bwd(policy, teacher, batch, args, buffers, step_count, coef, anneal_steps=0, window_weight=None, sums=None):
+    """The policy distillation term (hrl_distill_fwd_bwd, csrc/distill_kernel.cu; the law in distill.py), launched after the
+    fused loss pass that wrote `buffers` (LossBuffers with gradients) on the same batch: adds c_n * d kl / d policy to
+    buffers.dpolicy and, when c_n > 0, c_n * kl to buffers.losses' total.  policy / teacher: the student's and the teacher's
+    raw (B, T, Pa, A) float32 logits; step_count: FlatAdam.step_count (n, read on the device); coef, anneal_steps: c0 and N.
+    sums: a (2,) float32 CUDA tensor that receives [kl, c_n * kl] (allocated on `buffers` when None).  Returns sums."""
+    if policy.dtype != torch.float32 or teacher.dtype != torch.float32:
+        raise _capi.HrlError('handyrl_b200: distillation takes float32 logits (bf16 logit I/O is not supported)')
+    for t, name in ((policy, 'policy'), (teacher, 'teacher')):
+        if not (t.is_cuda and t.is_contiguous()):
+            raise _capi.HrlError('handyrl_b200: %s logits must be a contiguous CUDA tensor' % name)
+    if teacher.shape != policy.shape:
+        raise ValueError('distillation: the teacher policy is shaped %s, the student\'s %s' % (tuple(teacher.shape), tuple(policy.shape)))
+    B, T, Pa, A = policy.shape
+    P = batch['turn_mask'].shape[2]
+    assert buffers.dims == (B, T, P, Pa, A) and buffers.dpolicy is not None and buffers.policy_dtype == torch.float32
+    if not (step_count.is_cuda and step_count.dtype == torch.int64 and step_count.numel() == 1):
+        raise _capi.HrlError('handyrl_b200: step_count must be a one-element int64 CUDA tensor')
+    if window_weight is not None and not (window_weight.is_cuda and window_weight.dtype == torch.float32 and
+                                          window_weight.is_contiguous() and window_weight.numel() == B):
+        raise _capi.HrlError('handyrl_b200: window_weight must be a contiguous float32 CUDA tensor of B=%d weights' % B)
+    if sums is None:
+        if getattr(buffers, 'distill_sums', None) is None:
+            buffers.distill_sums = torch.zeros(2, dtype=torch.float32, device=policy.device)
+        sums = buffers.distill_sums
+    if not (sums.is_cuda and sums.dtype == torch.float32 and sums.is_contiguous() and sums.numel() == 2):
+        raise _capi.HrlError('handyrl_b200: sums must be a contiguous float32 CUDA tensor of 2')
+    if getattr(buffers, 'distill_workspace', None) is None:
+        buffers.distill_workspace = torch.zeros(lib().hrl_distill_workspace_bytes(B, T, P, Pa, A), dtype=torch.uint8,
+                                                device=policy.device)
+    amask, tmask = batch['action_mask'], batch['turn_mask']
+    burn_in = int(args.get('burn_in_steps', 0))
+    key = (policy.data_ptr(), teacher.data_ptr(), amask.data_ptr(), tmask.data_ptr(), 0 if window_weight is None else window_weight.data_ptr(),
+           step_count.data_ptr(), float(coef), int(anneal_steps), burn_in, buffers.dpolicy.data_ptr(), buffers.losses.data_ptr(),
+           sums.data_ptr())
+    cached = getattr(buffers, '_cached_distill', None)      # static buffers (CUDA-graph replays): the same argument block
+    if cached is None or cached[0] != key:
+        keep = [_dev_f32(amask, 'action_mask'), _dev_f32(tmask, 'turn_mask')]
+        a = _capi.HrlDistillArgs()
+        a.B, a.T, a.P, a.Pa, a.A, a.burn_in = B, T, P, Pa, A, burn_in
+        a.policy_raw, a.teacher_raw, a.action_mask, a.turn_mask = _ptr(policy), _ptr(teacher), _ptr(keep[0]), _ptr(keep[1])
+        a.window_weight, a.step_count = _ptr(window_weight), _ptr(step_count)
+        a.coef, a.anneal_steps = float(coef), int(anneal_steps)
+        a.dpolicy_raw, a.losses, a.sums = _ptr(buffers.dpolicy), _ptr(buffers.losses), _ptr(sums)
+        a.workspace, a.workspace_bytes = _ptr(buffers.distill_workspace), buffers.distill_workspace.numel()
+        cached = (key, a, keep)
+        if keep[0] is amask and keep[1] is tmask:
+            buffers._cached_distill = cached
+    check(lib().hrl_distill_fwd_bwd(C.byref(cached[1]), _stream_ptr()))
+    buffers._distill_keep = cached[2]       # the launch is asynchronous: keep temporaries alive
+    _count()
+    return sums
+
+
 def summarize_diagnostics(sums):
     """Diagnostics sums (a sequence in DIAG_KEYS order, or a dict keyed by DIAG_KEYS; missing entries count as 0) -> means:
       rho     mean unclipped importance ratio pi(a)/mu(a)        clip    fraction of samples with rho > 1 (clipped at 1)

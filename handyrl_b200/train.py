@@ -29,6 +29,7 @@ import numpy as np
 import torch
 
 from . import ops, fastnet, priority, symmetry
+from . import distill as distill_mod
 from .batch import tree_map, tree_leaves, make_batch, gather_windows, sample_window
 from ._capi import DIAG_KEYS, LOSS_KEYS, NUM_DIAG, NUM_LOSS, NUM_LOSS_DIAG
 
@@ -45,13 +46,14 @@ def _as_format(o, memory_format):
     return o
 
 
-def forward_raw(model, hidden, batch, args, memory_format=None):
+def forward_raw(model, hidden, batch, args, memory_format=None, train=True):
     """Run the net over a batch and return its RAW outputs shaped (B, T, Pa, ...).
 
     Feed-forward nets see all B*T*Pa observations at once; recurrent nets are stepped over T
     with the hidden state masked by observation_mask, burn-in steps without gradient and in
     eval mode, exactly as the reference does (train.py:142-174) -- but WITHOUT the mask
-    epilogue of train.py:176-184, which the fused loss kernel applies on the fly.
+    epilogue of train.py:176-184, which the fused loss kernel applies on the fly.  train=False keeps a net in eval mode
+    after burn-in too (a distillation teacher): the steps t >= burn_in then leave the mode as it is.
     """
     observations = batch['observation']
     B, T, Pa = batch['action'].shape[:3]
@@ -88,7 +90,7 @@ def forward_raw(model, hidden, batch, args, memory_format=None):
             with torch.no_grad():
                 out_t = _call_model(model, obs_t, visible)
         else:
-            if not model.training:
+            if train and not model.training:
                 model.train()
             out_t = _call_model(model, obs_t, visible)
         new_hidden = out_t.pop('hidden', None)
@@ -613,10 +615,21 @@ def nonfinite_guard(args):
     return bool(args.get('skip_nonfinite'))
 
 
-def accum_slots(diagnostics, skip_nonfinite):
+def accum_slots(diagnostics, skip_nonfinite, distill=False):
     """Float64 slots of the learner's epoch accumulator (LearnerStep.accum): the NUM_LOSS loss sums, then the NUM_DIAG
-    diagnostics sums when diagnostics are on, then the count of rejected steps when the guard is on."""
-    return NUM_LOSS + (NUM_DIAG if diagnostics else 0) + (1 if skip_nonfinite else 0)
+    diagnostics sums when diagnostics are on, then the count of rejected steps when the guard is on, then the two
+    distillation sums (kl, c_n * kl) when distillation is on."""
+    return NUM_LOSS + (NUM_DIAG if diagnostics else 0) + (1 if skip_nonfinite else 0) + (NUM_DISTILL if distill else 0)
+
+
+# the distillation sums [kl, c_n * kl] (distill.py): the last slots of the accumulator and of the bucket tail
+NUM_DISTILL = 2
+
+
+def _distill_slots(diagnostics, skip_nonfinite):
+    """The slice of the distillation sums in an accumulator of accum_slots(diagnostics, skip_nonfinite, True) slots."""
+    n = accum_slots(diagnostics, skip_nonfinite)
+    return slice(n, n + NUM_DISTILL)
 
 
 # the loss pass's diagnostics sums: where they sit behind the loss sums, in the accumulator and in the gradient bucket's tail
@@ -787,13 +800,17 @@ class PendingModel:
     `replay_ratio` to the epoch's ReplayRatioLimiter.end_epoch() figures under train_args['replay_ratio'], and report() prints
     them (replay_ratio_line) after those lines and before the validation lines.  Under train_args['save_replay'] the Trainer
     sets `replay` to the GpuBatcher.snapshot() taken at the boundary, and with the priorities ('prio', the prio_snap layout)
-    resolve() leaves them in `priority_state` (what LearnerStep.priority_state_dict() returns)."""
+    resolve() leaves them in `priority_state` (what LearnerStep.priority_state_dict() returns).  With distillation
+    (`distill`), the accumulator ends in the epoch's sums of kl and c_n * kl: report() leaves them in `distill` and prints
+    distill.line() after the loss and diagnostics lines and before the skipped line."""
 
     def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host=None, steps=0, diagnostics=False,
-                 skip_nonfinite=False, batch_cnt=0):
+                 skip_nonfinite=False, batch_cnt=0, distill=False):
         self.stepper, self.done, self.host_state, self.host_losses = stepper, done_event, host_state, host_losses
         self.heads, self.template, self.host, self.steps = heads, template, host or {}, steps
         self.has_diagnostics, self.skip_nonfinite, self.batch_cnt = bool(diagnostics), bool(skip_nonfinite), batch_cnt
+        self.has_distill = bool(distill)
+        self.distill = None
         self.ema_state = None
         self.optim_state = None
         self.validation = None
@@ -805,18 +822,22 @@ class PendingModel:
     def report(self):
         """Read the epoch's sums from the host copy (already arrived) and print the epoch's lines; returns the loss sums."""
         host = self.host_losses.tolist()
-        if len(host) != accum_slots(self.has_diagnostics, self.skip_nonfinite):
-            raise ValueError('PendingModel: %d accumulator slots, the layout has %d'
-                             % (len(host), accum_slots(self.has_diagnostics, self.skip_nonfinite)))
+        n_slots = accum_slots(self.has_diagnostics, self.skip_nonfinite, self.has_distill)
+        if len(host) != n_slots:
+            raise ValueError('PendingModel: %d accumulator slots, the layout has %d' % (len(host), n_slots))
         loss, diag, skipped = _accum_layout(self.has_diagnostics, self.skip_nonfinite)
         sums = dict(zip(LOSS_KEYS, host[loss]))
         dcnt = sums['dcnt']
         self.diagnostics = ops.summarize_diagnostics(host[diag]) if self.has_diagnostics else None
         self.skipped = int(host[skipped][0]) if self.skip_nonfinite else 0
+        if self.has_distill:
+            self.distill = dict(zip(('kl', 'term'), host[_distill_slots(self.has_diagnostics, self.skip_nonfinite)]))
         if dcnt > 0:
             print(loss_line('loss', sums, self.heads))
             if self.diagnostics is not None:
                 print(ops.format_diagnostics(self.diagnostics))
+            if self.distill is not None:
+                print(distill_mod.line(self.distill['kl'], self.distill['term'], dcnt))
         if self.skipped:
             print(skipped_line(self.skipped, self.batch_cnt))
         if self.replay_ratio is not None:
@@ -942,6 +963,15 @@ class LearnerStep:
     ranks of B/k windows would take.  `micro_batches` is k; launches_per_step counts all k micro-batches.  Validation
     passes run in the same micro-batches; time_loss_kernel needs k = 1.
 
+    distill (default: train_args['distill'], off; distill.py) and teacher (an nn.Module, or None: built from the key's file,
+    distill.teacher_net): policy distillation.  Each micro-batch first runs the teacher -- in eval mode, under no_grad, on the
+    module path (optimize_small_boards in the step's tensor_cores mode, its own channels-last probe, forward_raw with its own
+    init_hidden and train=False), never on the fused tower -- then the student, the fused loss kernel, one more launch
+    (ops.distill_fwd_bwd) that adds c_n * KL(teacher || student) to the policy gradient and to the loss row's total, and the
+    backward.  Its two sums [kl, c_n * kl] (distill_col of the loss row) follow the bucket tail and end the accumulator
+    (`distill_accum`); the teacher's weights are in no bucket, hand-off or checkpoint.  With c_n = 0 the step is bit for bit
+    the step without the key.  Validation passes are unchanged.
+
     A feature that adds device state registers it in __init__, where it allocates it: in `_mutable` (or `_zeroed`) when a
     step or validation pass changes it, so that the capture's warm-up leaves it as it was, and in `_handoff` (a _Handoff)
     when the epoch boundary carries it to the host; end_epoch, _snapshot and _restore have no per-feature code.
@@ -951,7 +981,13 @@ class LearnerStep:
                  max_norm=4.0, weight_decay=1e-5, time_loss_kernel=False, channels_last=True, cudnn_benchmark=True,
                  small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None,
                  weight_ema=None, save_optimizer=None, validation=None, skip_nonfinite=None, save_replay=None,
-                 gradient_accumulation=None):
+                 gradient_accumulation=None, distill=None, teacher=None):
+        self.distill = distill_mod.config({'distill': distill} if distill is not None else args, teacher_given=teacher is not None)
+        if self.distill is None and teacher is not None:
+            self.distill = distill_mod.config({'distill': {}}, teacher_given=True)
+        if self.distill is not None and teacher is None:
+            teacher = distill_mod.teacher_net(self.distill, model)      # the default net copies the student before any rewrite
+        self.teacher = teacher
         k = micro_batch_count(args.get('gradient_accumulation') if gradient_accumulation is None else gradient_accumulation)
         if k > 1 and example_batch['action'].shape[0] % k:
             raise ValueError('gradient_accumulation = %d does not divide the batch of %d windows' % (k, example_batch['action'].shape[0]))
@@ -971,8 +1007,13 @@ class LearnerStep:
         if diagnostics is None:
             diagnostics = bool(args.get('diagnostics', False))
         self.diagnostics = diagnostics
-        n_sums = accum_slots(diagnostics, self.skip_nonfinite)             # accumulator: loss sums [+ diagnostics] [+ skips]
+        distilling = self.teacher is not None
+        n_sums = accum_slots(diagnostics, self.skip_nonfinite, distilling)  # accumulator: loss sums [+ diagnostics] [+ skips] [+ distill]
         self.n_tail = _LOSS_DIAG.stop if diagnostics else NUM_LOSS         # bucket tail: [+ the loss pass's diagnostics]
+        # distillation: its sums follow the tail, in the loss row's columns [distill_col, n_tail), which the loss pass leaves
+        # unused (or writes zeros to, for the optimiser's diagnostics entries, before the distillation launch runs)
+        self.distill_col = self.n_tail if distilling else None
+        self.n_tail += NUM_DISTILL if distilling else 0
         # the learner owns its precision contract (1e-5 of the reference's fp32 arithmetic): PyTorch's default lets
         # cuDNN convolutions run on TF32 tensor cores (10-bit mantissa).  train_args['allow_tf32'] = True opts out.
         if allow_tf32 is None:
@@ -999,6 +1040,16 @@ class LearnerStep:
         if cudnn_benchmark:
             torch.backends.cudnn.benchmark = True
         self.model.train()
+        self.teacher_format = None
+        self.launches_per_teacher = 0
+        if self.teacher is not None:
+            self.teacher = self.teacher.to(self.device).eval()
+            self.teacher.requires_grad_(False)
+            teacher_rewritten = fastnet.optimize_small_boards(self.teacher, tensor_cores=tensor_cores) if small_boards else 0
+            teacher_cl = channels_last and not (teacher_rewritten and self._uses_dense_convs(example_batch, self.teacher))
+            self.teacher_format = torch.channels_last if teacher_cl else None
+            if teacher_cl:
+                self.teacher = self.teacher.to(memory_format=torch.channels_last)
         self.time_loss_kernel = time_loss_kernel
         self.kernel_events = []
         self._timed_loss = None          # time_loss_kernel: the loss kernel launched between the two step graphs
@@ -1086,9 +1137,11 @@ class LearnerStep:
                             for i in range(k)]
         self.loss_rows = torch.zeros((k, NUM_LOSS + NUM_DIAG), dtype=torch.float32, device=self.device)
         self.advantage = torch.zeros((B, T, P, 1), dtype=torch.float32, device=self.device) if self.prio_state is not None else None
-        self.hidden0 = None
+        self.hidden0 = self.teacher_hidden0 = None
         if hasattr(self.model, 'init_hidden'):
             self.hidden0 = tree_map(lambda h: h.to(self.device), self.model.init_hidden([Bm, P]))
+        if self.teacher is not None and hasattr(self.teacher, 'init_hidden'):
+            self.teacher_hidden0 = tree_map(lambda h: h.to(self.device), self.teacher.init_hidden([Bm, P]))
         from . import tower
         if fused_tower and small_boards and self.hidden0 is None and tower.supports(self.model) and \
                 torch.is_tensor(example_batch['observation']) and example_batch['observation'].shape[-2] * example_batch['observation'].shape[-1] <= 16:
@@ -1099,7 +1152,9 @@ class LearnerStep:
         self._mutable.append(self.accum)
         loss, diag, skipped = _accum_layout(diagnostics, self.skip_nonfinite)
         self.loss_accum = self.accum[loss]
-        self.diag_accum = None
+        self.diag_accum = self.distill_accum = None
+        if distilling:
+            self.distill_accum = self.accum[_distill_slots(diagnostics, self.skip_nonfinite)]
         if diagnostics:
             self.diag_accum = self.accum[diag]
             self.opt.diag = self.diag_accum[NUM_LOSS_DIAG:]        # the optimiser's entries: accumulated by its own kernel
@@ -1122,19 +1177,21 @@ class LearnerStep:
         self.stream = torch.cuda.Stream(device=self.device)
         self._warm = PackedBatch(self.layout).fill(example_batch)
 
-    def _uses_dense_convs(self, example_batch):
-        """One no-grad probe call of the net on a two-sample slice: do its convolutions take the dense small-board path
-        (then activations stay NCHW) or cuDNN (then NHWC, whose implicit-GEMM kernels are the fast ones)?"""
+    def _uses_dense_convs(self, example_batch, model=None):
+        """One no-grad probe call of the net (or of `model`, the teacher) on a two-sample slice: do its convolutions take the
+        dense small-board path (then activations stay NCHW) or cuDNN (then NHWC, whose implicit-GEMM kernels are the fast
+        ones)?"""
+        model = self.model if model is None else model
         before = fastnet.BoardConv2d.dense_calls
         obs = tree_map(lambda o: o[:1, :1].flatten(0, 2).to(self.device), example_batch['observation'])
         hidden = None
-        if hasattr(self.model, 'init_hidden'):
-            hidden = tree_map(lambda h: h.to(self.device), self.model.init_hidden([obs_rows(obs)]))
-        was_training = self.model.training
-        self.model.eval()
+        if hasattr(model, 'init_hidden'):
+            hidden = tree_map(lambda h: h.to(self.device), model.init_hidden([obs_rows(obs)]))
+        was_training = model.training
+        model.eval()
         with torch.no_grad():
-            self.model(obs, hidden)
-        self.model.train(was_training)
+            model(obs, hidden)
+        model.train(was_training)
         return fastnet.BoardConv2d.dense_calls > before
 
     # -- the device work of one step, on the current stream (inputs already in self.dev)
@@ -1198,6 +1255,7 @@ class LearnerStep:
         callable) for the caller to run: _device_step runs it in place, time_loss_kernel between two graphs."""
         self._begin_step()          # (guard_saved is taken before micro-batch 0: a rejected step restores all k forwards)
         for i, (dev, weight) in enumerate(zip(self._micro, self._win_weight)):
+            teacher = self._teacher_policy(dev) if self.teacher is not None else None
             outs = self._forward(dev)
             if self.loss_buf is None:
                 self._build_loss_buffers(outs)
@@ -1208,8 +1266,12 @@ class LearnerStep:
                 yield loss
             else:
                 loss()
+            if teacher is not None:
+                ops.distill_fwd_bwd(outs['policy'], teacher, dev, self.args, buf, self.opt.step_count, self.distill['coef'],
+                                    self.distill['anneal_steps'], window_weight=weight,
+                                    sums=self.loss_rows[i, self.distill_col:self.distill_col + NUM_DISTILL])
             self._net_backward(outs, buf, accumulate=i > 0)
-            del outs, loss      # this micro-batch's activations and autograd graph go back to the pool before the next forward
+            del outs, loss, teacher     # this micro-batch's activations and autograd graph go back to the pool before the next forward
         # the loss sums [+ the loss pass's diagnostics] ride the gradient bucket: one row is copied, k rows are summed
         if self.micro_batches == 1:
             self.opt.extra_slots[:self.n_tail].copy_(self.loss_rows[0, :self.n_tail])
@@ -1230,19 +1292,31 @@ class LearnerStep:
             self.opt.step()
             tail = self.opt.extra_slots
             self.last_losses.copy_(tail[:NUM_LOSS])
+        n_commit = self.n_tail if self.distill_col is None else self.distill_col
         if self.skip_nonfinite:         # one launch: accumulate an accepted step, or count a rejected one and restore its buffers
-            ops.step_commit(self.opt.skip, tail[:self.n_tail], self.accum, self.skipped,
+            ops.step_commit(self.opt.skip, tail[:n_commit], self.accum, self.skipped,
                             self._guarded_buffers() if self.guard_saved is not None else None, self.guard_saved)
         else:
             self.loss_accum.add_(self.last_losses)
             if self.diagnostics:
                 self.accum[_LOSS_DIAG].add_(tail[_LOSS_DIAG])
+        if self.distill_accum is not None:      # a rejected step adds none of its sums
+            sums = tail[self.distill_col:self.n_tail]
+            self.distill_accum.add_(sums.masked_fill(self.opt.skip.bool(), 0.0) if self.skip_nonfinite else sums)
         if self.avg is not None:        # after the optimiser: step_count already counts this step
             ops.weight_ema_update(self.avg, self.state.bytes[:self.state.i_off].view(torch.float32), self.opt.step_count,
                                   self.weight_ema, self.avg_seeded, skip=self.opt.skip)
         if self.prio_state is not None:     # after the optimiser: a rejected step stores no priority
             ops.priority_update(self.prio_state, self.advantage, self.dev['turn_mask'], self.args.get('burn_in_steps', 0),
                                 skip=self.opt.skip if self.skip_nonfinite else None)
+
+    def _teacher_policy(self, dev):
+        """The teacher's raw policy (B', T, Pa, A) on the windows of `dev`: eval mode, no gradient, the module path."""
+        before = ops.LAUNCHES['n']
+        with torch.no_grad():
+            outs = forward_raw(self.teacher, self.teacher_hidden0, dev, self.args, self.teacher_format, train=False)
+        self.launches_per_teacher = ops.LAUNCHES['n'] - before
+        return outs['policy'].float().contiguous()
 
     def _guarded_buffers(self):
         """The buffers a step's forward moves (BatchNorm running statistics, num_batches_tracked): StateStore bytes
@@ -1678,7 +1752,8 @@ class LearnerStep:
             done.record(self.copy_stream)
         self._last_done = done
         return PendingModel(self, done, host['state'], host['losses'], heads, template, host=host, steps=int(steps),
-                            diagnostics=self.diagnostics, skip_nonfinite=self.skip_nonfinite, batch_cnt=batch_cnt)
+                            diagnostics=self.diagnostics, skip_nonfinite=self.skip_nonfinite, batch_cnt=batch_cnt,
+                            distill=self.teacher is not None)
 
 
 # --------------------------------------------------------------------------- batcher + trainer
@@ -2237,7 +2312,12 @@ class Trainer:
     with one optimiser step (LearnerStep), so the net's activations take 1/k of the memory.  k must divide batch_size
     (ValueError otherwise); with several GPUs each rank runs k micro-batches of its batch_size / num_gpus windows, and when
     batch_size % (num_gpus * k) != 0 the trainer prints one line and uses one GPU.  Steps, the learning-rate law and the
-    printed lines are unchanged; BatchNorm normalises each micro-batch with its own statistics."""
+    printed lines are unchanged; BatchNorm normalises each micro-batch with its own statistics.
+
+    train_args['distill'] = {'teacher': path, 'net': 'module:function', 'coef': c0, 'anneal_steps': N} (distill.py): the
+    teacher is built and loaded here (ValueError for a bad key, file or net), and every step adds the annealed term
+    c_n * KL(teacher || student) on the trained policy rows (LearnerStep).  Each epoch prints 'distill = kl:<kl> term:<c_n kl>'
+    (both over dcnt) after the loss and diagnostics lines.  Helper ranks build their teacher from the same key."""
 
     def __init__(self, args, model):
         ratio = replay_ratio(args)
@@ -2250,6 +2330,9 @@ class Trainer:
         self.validation = validation_rate(args)
         self.symmetry = symmetry.config(args)
         self.priority = priority.config(args)
+        self.distill = distill_mod.config(args)
+        # the teacher of train_args['distill'], built now (a deep copy of the net as received, before the learner rewrites it)
+        self.teacher = distill_mod.teacher_net(self.distill, model) if self.distill is not None else None
         self.validate_every = max(1, int(round(1.0 / self.validation))) if self.validation is not None else 0
         self.save_optimizer = bool(args.get('save_optimizer', False))
         self.checkpoint_files = None         # numbers the .ema.pth and .optim.pth files of one epoch alike
@@ -2414,7 +2497,7 @@ class Trainer:
             self.fleet = multigpu.Fleet(self.world, self.args, self.cpu_template, list(self.episodes), self.lr,
                                         optim_state=optim_state)
             pg = self.fleet.process_group
-        self.stepper = LearnerStep(self.model, self.args, batch, self.lr, process_group=pg)
+        self.stepper = LearnerStep(self.model, self.args, batch, self.lr, process_group=pg, teacher=self.teacher)
         if optim_state is not None:
             self.stepper.load_optimizer_state(optim_state)
         seed = self.ema_files.seed_path() if self.ema_files is not None else None

@@ -29,6 +29,8 @@
  *   hrl_replay_sample /
  *   hrl_replay_priority_update <- prioritised replay: Batcher.select_episode's recency law (train.py:291-315) times a
  *                            per-episode priority, with importance weights; no reference counterpart
+ *   hrl_distill_fwd_bwd   <- an annealed KL(teacher || student) term on the trained policy rows ("kickstarting"), launched
+ *                            after hrl_loss_fwd_bwd; no reference counterpart
  *   hrl_gemm_tf32x3       <- the Linear/Conv contractions of the user's net inside train.py:142-146 (+ autograd, :369)
  *
  * Conventions
@@ -678,6 +680,41 @@ int hrl_replay_sample(const HrlReplaySampleArgs *args, void *stream);
 int hrl_replay_priority_update(int32_t B, int32_t T, int32_t P, int32_t burn_in, const float *tap_advantage,
                                const float *turn_mask, float epsilon, const int32_t *win_slot, const int64_t *win_serial,
                                float *prio, const int64_t *prio_serial, float *max_prio, const int32_t *skip, void *stream);
+
+/*
+ * Policy distillation from a teacher net ("kickstarting"): an annealed KL(teacher || student) term on the policy rows the fused
+ * loss trains, launched right after hrl_loss_fwd_bwd on the same batch.  Row (b, t, q) of the (B,T,Pa,A) logits, trained when
+ * t >= burn_in (or T == 1), f = sum_p turn_mask[b,t,p] when Pa == 1, else turn_mask[b,t,q] (the mask epilogue's own factor):
+ *     zS = f * student - action_mask         zT = f * teacher - action_mask
+ *     kl = sum_rows w_b * f * sum_a pT * (log pT - log pS)      pT = softmax(zT), pS = softmax(zS); terms with pT == 0 add 0
+ *     c  = coef * max(0, 1 - n / anneal_steps)                   (coef when anneal_steps == 0; n = *step_count at launch)
+ * w_b = window_weight[b] (1 when NULL).  sums = [kl, c * kl] (overwritten); when c > 0, losses[HRL_LOSS_TOTAL] += c * kl and
+ * dpolicy_raw += c * w_b * f * f * (pS - pT) on trained rows with w_b * f != 0; when c == 0 neither is written.  Rows of weight 0
+ * are never read.  Block partials are folded in fp64 in a fixed order by the last CTA, which resets the workspace counter:
+ * repeated launches and graph replays give identical bits.  Pa must be 1 or P, A <= 1024, P <= 64; io_bf16 logits are
+ * refused (HRL_ERR_UNSUPPORTED).
+ */
+typedef struct HrlDistillArgs {
+    int32_t B, T, P, Pa, A;
+    int32_t burn_in;
+    const float *policy_raw;      /* (B,T,Pa,A) the student's raw logits (what hrl_loss_fwd_bwd read)          */
+    const float *teacher_raw;     /* (B,T,Pa,A) the teacher's raw logits on the same batch                      */
+    const float *action_mask;     /* (B,T,Pa,A) 0 legal / 1e32 illegal                                          */
+    const float *turn_mask;       /* (B,T,P)                                                                    */
+    const float *window_weight;   /* (B) importance weights (prioritised replay), or NULL = 1                   */
+    const int64_t *step_count;    /* [1] the optimiser's step count before this step                           */
+    float coef;                   /* c0 >= 0                                                                    */
+    int64_t anneal_steps;         /* N >= 0; 0 = constant coefficient                                           */
+    float *dpolicy_raw;           /* (B,T,Pa,A) added to                                                        */
+    float *losses;                /* [HRL_NUM_LOSS] of the loss pass: only the total is added to               */
+    float *sums;                  /* [2] out: kl, c * kl                                                        */
+    void *workspace;              /* >= hrl_distill_workspace_bytes(...), first 64 bytes zero on the first call  */
+    size_t workspace_bytes;
+    int32_t io_bf16;              /* must be 0                                                                  */
+} HrlDistillArgs;
+
+size_t hrl_distill_workspace_bytes(int32_t B, int32_t T, int32_t P, int32_t Pa, int32_t A);
+int hrl_distill_fwd_bwd(const HrlDistillArgs *args, void *stream);
 
 /* Text of the last error raised on the calling thread ("" if none). */
 const char *hrl_last_error(void);
