@@ -798,8 +798,9 @@ def _conv_product(pix, image, rows, cin, taps, table, hw, bias=None, bf16=False)
 # Deferred weight gradients.  A recurrent net applies the same convolution at every time step (and DRC cells several times per step):
 # computing its weight gradient per application means T x repeats small products, slice reductions and gradient accumulations --
 # ~1,000 launches of a 4,400-launch Geister step, in a chain that is launch-bound.  Inside `deferred_weight_gradients()` the backward of
-# conv_implicit only records its (dy, x) pair; on exit ONE segmented product per weight reduces over all its pairs (hrl_gemm_fused with
-# `segments`), its ones row yields the bias gradient, and hrl_conv_wgrad_reduce2 adds the result into weight.grad / bias.grad.
+# conv_implicit only records its (dy, x) pair; on exit ONE segmented product per weight and board geometry reduces over all its pairs
+# (hrl_gemm_fused with `segments`), its ones row yields the bias gradient, and hrl_conv_wgrad_reduce2 adds the result into
+# weight.grad / bias.grad.
 _DEFER = {'on': False, 'pending': {}}
 
 
@@ -893,7 +894,9 @@ class _ConvImplicit(torch.autograd.Function):
             dx = _conv_product(dy2, adj, Cin, Cout, taps, table, H * W, bf16=ctx.bf16).view(N, H, W, Cin).permute(0, 3, 1, 2)
         if (ctx.needs_input_grad[1] and _DEFER['on'] and pw.is_leaf and (pb is None or (pb.is_leaf and ctx.needs_input_grad[2]))
                 and (pw.grad is None or pw.grad.is_contiguous())):
-            job = _DEFER['pending'].setdefault((pw.data_ptr(), ctx.bf16),
+            # one job per board geometry: its product reads every pair through the job's neighbour table (a weight applied to
+            # two board shapes, or with both paddings, gets one flush per geometry, each adding into the same .grad)
+            job = _DEFER['pending'].setdefault((pw.data_ptr(), ctx.bf16, H, W, ctx.wrap),
                                                {'w': pw, 'b': pb, 'pairs': [], 'geom': (table, H * W), 'bf16': ctx.bf16})
             if not job['pairs'] or job['pairs'][0][0].shape[0] == dy2.shape[0]:      # (pairs of one product cover the same pixels)
                 job['pairs'].append((dy2, xl.permute(0, 2, 3, 1).reshape(-1, Cin)))

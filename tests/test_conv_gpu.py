@@ -1,63 +1,14 @@
-"""Convolutions over a board as implicit tensor-core products (ops.conv_implicit: hrl_gemm_fused conv_mode 1 / 2, hrl_conv_pack,
-hrl_conv_wgrad_reduce) against float64 F.conv2d: zero `same` padding (Geister's ConvLSTM cells, reference geister.py:18-56) and
-wrap-around padding (Hungry Geese's TorusConv2d, reference hungry_geese.py:20-37); output, input gradient, weight and bias gradient."""
+"""Convolutions over a board as implicit tensor-core products (ops.conv_implicit) inside the nets: zero `same` padding (Geister's
+ConvLSTM cells, reference geister.py:18-56) and wrap-around padding (Hungry Geese's TorusConv2d, reference hungry_geese.py:20-37),
+fastnet's routing of board convolutions, deferred weight gradients, and batches past 2^22 pixels.  The products themselves,
+element by element against float64 on every shape they admit, are test_conv_products_gpu.py."""
 import pytest
 import torch
 import torch.nn.functional as F
 
+from tower_ref import _close, conv_ref, conv_ref_input, conv_ref_weight, conv_src
+
 pytestmark = pytest.mark.gpu
-
-CASES = [
-    # N, Cin, Cout, H, W, kh, kw, wrap, bias
-    (37, 64, 128, 6, 6, 3, 3, False, True),       # Geister ConvLSTM gates: [x, h] 64 maps -> 4 x 32 gate maps
-    (21, 32, 32, 7, 11, 3, 3, True, True),        # Hungry Geese torus block
-    (9, 36, 20, 6, 6, 3, 3, False, False),        # channel counts that are not multiples of 32: padded chunks
-    (130, 8, 12, 3, 3, 3, 3, False, True),        # fewer cells (9) than a chunk has elements
-    (5, 16, 288, 5, 4, 1, 3, True, False),        # one-row kernel, widest operand tile
-    (3, 288, 8, 4, 4, 3, 1, False, True),
-]
-
-
-@pytest.mark.parametrize('N,Cin,Cout,H,W,kh,kw,wrap,bias', CASES)
-@pytest.mark.parametrize('channels_last', [True, False])
-def test_conv_implicit_matches_float64(N, Cin, Cout, H, W, kh, kw, wrap, bias, channels_last):
-    from handyrl_b200 import ops
-    g = torch.Generator(device='cuda').manual_seed(N * 1000 + Cin)
-    x = torch.randn(N, Cin, H, W, device='cuda', generator=g)
-    w = torch.randn(Cout, Cin, kh, kw, device='cuda', generator=g) * 0.2
-    b = torch.randn(Cout, device='cuda', generator=g) if bias else None
-    dy = torch.randn(N, Cout, H, W, device='cuda', generator=g)
-    if channels_last:
-        x, dy = x.contiguous(memory_format=torch.channels_last), dy.contiguous(memory_format=torch.channels_last)
-    assert ops.conv_implicit_supported(x, w)
-    xs, ws = x.clone().requires_grad_(True), w.clone().requires_grad_(True)
-    bs = b.clone().requires_grad_(True) if bias else None
-    ops.conv_weights_changed()
-    y = ops.conv_implicit(xs, ws, bs, wrap)
-    y.backward(dy)
-
-    xd, wd = x.double().requires_grad_(True), w.double().requires_grad_(True)
-    bd = b.double().requires_grad_(True) if bias else None
-    if wrap:
-        xp = F.pad(xd, (kw // 2, kw // 2, kh // 2, kh // 2), mode='circular')
-        yd = F.conv2d(xp, wd, bd)
-    else:
-        yd = F.conv2d(xd, wd, bd, padding=(kh // 2, kw // 2))
-    yd.backward(dy.double())
-
-    def close(got, want, what, tol=3e-6, red=Cin * kh * kw):
-        # 3xTF32 products: ~1e-6 of sum |a||b|; the bound below is in units of the result's largest magnitude
-        scale = want.abs().max().item() + 1e-12
-        err = (got.double() - want).abs().max().item()
-        assert err <= tol * scale * (1 + red ** 0.5 / 8), (what, err, scale)
-
-    assert y.shape == yd.shape
-    close(y, yd, 'output')
-    close(xs.grad, xd.grad, 'input gradient', red=Cout * kh * kw)
-    close(ws.grad, wd.grad, 'weight gradient', red=N * H * W)
-    if bias:
-        close(bs.grad, bd.grad, 'bias gradient', tol=1e-5, red=1)
-
 
 def test_rewritten_modules_use_the_implicit_products():
     """fastnet routes nn.Conv2d (zeros / circular `same` padding) over boards too large for the dense form to conv_implicit."""
@@ -75,6 +26,57 @@ def test_rewritten_modules_use_the_implicit_products():
         y = net(x)
         assert ops.LAUNCHES['n'] > before
         assert (y.double() - ref(x.double())).abs().max().item() < 1e-4
+
+
+ROUTES = {        # route, kernel, board, Cin, padding_mode, tensor_cores
+    'dense_1x3': ('dense', (1, 3), (3, 3), 8, 'zeros', True),                 # at most 16 cells: one dense product
+    'dense_5x1': ('dense', (5, 1), (4, 4), 8, 'zeros', True),
+    'implicit_3x1': ('implicit', (3, 1), (6, 6), 8, 'zeros', True),
+    'implicit_1x5_torus': ('implicit', (1, 5), (7, 11), 8, 'circular', True),
+    'implicit_1x3_small_torus': ('implicit', (1, 3), (3, 3), 8, 'circular', True),   # the dense form is zero padding only
+    'conv_same_cin6': ('conv_same', (1, 3), (6, 6), 6, 'zeros', True),        # Cin % 4 != 0: no implicit product
+    'conv_same_fp32': ('conv_same', (3, 1), (6, 6), 8, 'zeros', False),       # tensor_cores=False
+    'cudnn_torus_cin6': ('cudnn', (1, 3), (6, 6), 6, 'circular', True),       # wrap-around padding the implicit path refuses
+    'cudnn_1x1': ('cudnn', (1, 1), (6, 6), 8, 'zeros', True),                 # nothing to gain over a plain product
+    'cudnn_17x17': ('cudnn', (3, 1), (17, 17), 8, 'zeros', True),             # more than 256 cells
+}
+
+
+@pytest.mark.parametrize('name', list(ROUTES))
+def test_board_conv_routes_non_square_kernels(name, monkeypatch):
+    """fastnet.BoardConv2d runs a stride-1 `same` convolution over a board as a dense product (at most 16 cells, zero padding),
+    as the implicit products (conv_implicit_supported), as _ConvSame (zero padding they refuse, or tensor_cores=False: cuDNN's
+    forward with an input gradient by the flipped, channel-transposed kernel) or else as cuDNN.  Each route, with a non-square
+    kernel, against float64: output, input, weight and bias gradients."""
+    from handyrl_b200 import fastnet
+    monkeypatch.setattr(torch.backends.cudnn, 'allow_tf32', False)
+    route, (kh, kw), (H, W), Cin, mode, tensor_cores = ROUTES[name]
+    Cout, N = 12, 5
+    torch.manual_seed(sum(map(ord, name)))
+    conv = torch.nn.Conv2d(Cin, Cout, (kh, kw), padding=(kh // 2, kw // 2), padding_mode=mode).cuda()
+    assert fastnet.optimize_small_boards(torch.nn.Sequential(conv), tensor_cores=tensor_cores) == 1
+    x = torch.randn(N, Cin, H, W, device='cuda')
+    dy = torch.randn(N, Cout, H, W, device='cuda')
+    xs = x.clone().requires_grad_(True)
+    fastnet.new_step()
+    dense_before = fastnet.BoardConv2d.dense_calls
+    y = conv(xs)
+    y.backward(dy)
+    fn = type(y.grad_fn).__name__
+    taken = ('dense' if fastnet.BoardConv2d.dense_calls > dense_before else 'implicit' if fn.startswith('_ConvImplicit')
+             else 'conv_same' if fn.startswith('_ConvSame') else 'cudnn' if fn.startswith('Convolution') else fn)
+    assert taken == route, (taken, fn)
+
+    src = conv_src(H, W, kh, kw, mode == 'circular')
+    xd, wd, bd, dyd = x.double(), conv.weight.detach().double(), conv.bias.detach().double(), dy.double()
+
+    def bound(mag):          # fp32-class products (3xTF32, or cuDNN fp32 in any algorithm) with room to spare
+        return 2e-5 * mag + 1e-6 * mag.max()
+    _close(y, conv_ref(xd, wd, src, bd), bound(conv_ref(xd.abs(), wd.abs(), src, bd.abs())), 'output')
+    _close(xs.grad, conv_ref_input(dyd, wd, src), bound(conv_ref_input(dyd.abs(), wd.abs(), src)), 'input gradient')
+    _close(conv.weight.grad, conv_ref_weight(dyd, xd, src, kh, kw), bound(conv_ref_weight(dyd.abs(), xd.abs(), src, kh, kw)),
+           'weight gradient')
+    _close(conv.bias.grad, dyd.sum((0, 2, 3)), bound(dyd.abs().sum((0, 2, 3))), 'bias gradient')
 
 
 def test_reference_style_torus_convolution_is_recognised():

@@ -8,11 +8,11 @@ they lie, per-row operand transforms applied on fragment load, split-K slice par
   and unaligned operands to the wgmma kernel (traced with torch.profiler).
 """
 import ctypes as C
-import re
-import time
 
 import pytest
 import torch
+
+from tower_ref import traced_gemms
 
 pytestmark = pytest.mark.gpu
 
@@ -147,34 +147,11 @@ def test_same_bits_as_the_wgmma_kernel():
         t = torch.zeros((16384, 289), device='cuda')
         t[:, :288] = c[k]
         odd[k] = t
-    assert traced_gemms(lambda: launch(odd, 43, ws=torch.empty_like(ws))) == {('gemm_tf32x3_kernel', 'false,false,false,144')}
+    assert traced_gemms(lambda: launch(odd, 43, ws=torch.empty_like(ws)), runs=2, repeat=2) == {('gemm_tf32x3_kernel', 'false,false,false,144')}
     ws_wgmma = torch.empty_like(ws)
     launch(odd, 43, ws=ws_wgmma)
     torch.cuda.synchronize()
     assert torch.equal(ws.view(torch.int32), ws_wgmma.view(torch.int32))
-
-
-_GEMM_RE = re.compile(r'(gemm_wgrad_kernel|gemm_tf32x3_kernel)<([^>]*)>')
-
-
-def traced_gemms(fn, attempts=3):
-    """The GEMM kernels fn() launches, as {(kernel, template arguments)} from a torch.profiler (CUPTI) trace.  A trace without
-    any GEMM (the tracer can drop the record of a kernel that ends as the window closes) is taken again."""
-    acts = [torch.profiler.ProfilerActivity.CPU, torch.profiler.ProfilerActivity.CUDA]
-    seen = set()
-    for _ in range(attempts):
-        with torch.profiler.profile(activities=acts) as prof:
-            fn()
-            torch.cuda.synchronize()
-            time.sleep(0.002)
-        names = set()
-        for e in prof.events():
-            names.add(e.name)
-            names.update(k.name for k in getattr(e, 'kernels', []))
-        seen = {(m.group(1), m.group(2).replace(' ', '')) for m in map(_GEMM_RE.search, names) if m}
-        if seen:
-            break
-    return seen
 
 
 def test_tower_weight_gradients_take_the_wgrad_kernel():
@@ -192,7 +169,7 @@ def test_tower_weight_gradients_take_the_wgrad_kernel():
     out = eng.forward(x)
     dout = {k: torch.randn_like(v) for k, v in out.items()}
 
-    seen = traced_gemms(lambda: eng.backward(dout['policy'], dout['value']))
+    seen = traced_gemms(lambda: eng.backward(dout['policy'], dout['value']), runs=2, repeat=2)
     wgrad = {args for k, args in seen if k == 'gemm_wgrad_kernel'}
     assert wgrad == {'2,1', '2,0', '0,1'}, seen
     assert ('gemm_tf32x3_kernel', 'false,false,false,16') in seen, seen       # the stem: x2d rows of 27 floats
@@ -210,15 +187,15 @@ def test_convolution_weight_gradient_and_unaligned_operands_keep_the_wgmma_kerne
     def conv():
         ops.conv_implicit(x, w).backward(dy)
 
-    seen = traced_gemms(conv)
+    seen = traced_gemms(conv, runs=2, repeat=2)
     assert seen and all(k == 'gemm_tf32x3_kernel' for k, _ in seen), seen
     assert any(args.startswith('false,false,false,') for _, args in seen), seen    # the weight gradient (conv_mode 2)
 
     a = torch.randn(4000, 27, device='cuda', generator=g)                    # rows of 27 floats: not 16-byte aligned
     b = torch.randn(4000, 288, device='cuda', generator=g)
-    seen = traced_gemms(lambda: ops.gemm_tf32x3(a, b, a_kmajor=False, b_kmajor=False, splits=4))
+    seen = traced_gemms(lambda: ops.gemm_tf32x3(a, b, a_kmajor=False, b_kmajor=False, splits=4), runs=2, repeat=2)
     assert seen == {('gemm_tf32x3_kernel', 'false,false,false,144')}, seen
     b_off = torch.randn(4000 * 288 + 1, device='cuda', generator=g)[1:].view(4000, 288)      # base pointer off by 4 bytes
     a2 = torch.randn(4000, 288, device='cuda', generator=g)
-    seen = traced_gemms(lambda: ops.gemm_tf32x3(a2, b_off, a_kmajor=False, b_kmajor=False, splits=4))
+    seen = traced_gemms(lambda: ops.gemm_tf32x3(a2, b_off, a_kmajor=False, b_kmajor=False, splits=4), runs=2, repeat=2)
     assert seen == {('gemm_tf32x3_kernel', 'false,false,false,144')}, seen

@@ -1,7 +1,7 @@
-"""Float64 references and error bounds shared by the fused tower's tests (test_bf16_gpu.py, test_tower_products_gpu.py,
-test_gemm_tower_gpu.py): the board convolutions and their gradients, the operand transforms as the kernels compute them in
-fp32, the accumulation bounds of the products and of the weight-gradient fold, and a trace of the GEMM kernels a call
-launches."""
+"""Float64 references and error bounds shared by the tensor-core product tests (test_bf16_gpu.py, test_tower_products_gpu.py,
+test_gemm_tower_gpu.py, test_conv_products_gpu.py): the board convolutions and their gradients (zero or wrap-around padding,
+any odd kernel, by explicit index arithmetic), the operand transforms as the kernels compute them in fp32, the accumulation
+bounds of the products and of the weight-gradient fold, and a trace of the GEMM kernels a call launches."""
 import re
 import time
 
@@ -22,6 +22,12 @@ def accum_bound(K, splits=1):
     from handyrl_b200._capi import lib
     k_slice = -(-K // lib().hrl_gemm_effective_splits(K, splits))
     return 1.2e-7 * (0.8 * k_slice ** 0.5 + 4)
+
+
+def product_bound(K, splits=1):
+    """accum_bound, but never below U32 (32 + 8): a K slice of one 32-element chunk is 12 truncating wgmma accumulations (3xTF32)
+    whose worst case accum_bound's sqrt(K) form leaves out at small K (test_tower_products_gpu.tf32x3_bound of one chunk)"""
+    return max(accum_bound(K, splits), 40 * U32)
 
 
 def _conv(a, w, b=None):
@@ -63,7 +69,68 @@ def _transform_ref(x, p, r, y=None, q=None, relu=False, bf16=True):
     return r16(t), torch.where(edge, ulp, torch.zeros_like(ulp))
 
 
-_GEMM_RE = re.compile(r'(gemm_tower_kernel|gemm_wgrad_kernel|gemm_tf32x3_kernel)<([^>]*)>')
+def operand_ref(t, bf16):
+    """an untransformed operand as the products see it: (value, boundary term) of _transform_ref with p = 1, r = 0"""
+    one = torch.ones((), dtype=torch.float32, device=t.device)
+    return _transform_ref(t, one, torch.zeros_like(one), bf16=bf16)
+
+
+_CONV_SRC = {}
+
+
+def conv_src(H, W, kh, kw, wrap):
+    """src[cell, tap] (CPU, int64): the input cell tap (a, b) of output cell (y, x) reads, (y + a - kh//2, x + b - kw//2) taken
+    modulo H and W (wrap) or H*W -- an extra zero cell -- off the board.  Index arithmetic only: valid for kernels larger than
+    the board, whose wrapped taps read the same cell more than once."""
+    key = (H, W, kh, kw, bool(wrap))
+    if key not in _CONV_SRC:
+        src = torch.empty(H * W, kh * kw, dtype=torch.long)
+        for y in range(H):
+            for x in range(W):
+                for a in range(kh):
+                    for b in range(kw):
+                        yy, xx = y + a - kh // 2, x + b - kw // 2
+                        if wrap:
+                            yy, xx = yy % H, xx % W
+                        src[y * W + x, a * kw + b] = yy * W + xx if 0 <= yy < H and 0 <= xx < W else H * W
+        _CONV_SRC[key] = src
+    return _CONV_SRC[key]
+
+
+def _conv_cols(x, src):
+    """x (N, C, H, W) -> (N, C, cells, taps): the input each tap of each output cell reads"""
+    N, Cin, H, W = x.shape
+    xp = torch.cat([x.reshape(N, Cin, H * W), x.new_zeros(N, Cin, 1)], 2)
+    return xp[:, :, src.to(x.device)]
+
+
+def conv_ref(x, w, src, b=None):
+    """y[n, o, cell] = sum over (i, tap) of w[o, i, tap] x[n, i, src[cell, tap]] (+ b[o])"""
+    N, _, H, W = x.shape
+    y = torch.einsum('nipt,oit->nop', _conv_cols(x, src), w.reshape(w.shape[0], w.shape[1], -1))
+    if b is not None:
+        y = y + b[None, :, None]
+    return y.reshape(N, -1, H, W)
+
+
+def conv_ref_input(dy, w, src):
+    """the input gradient of conv_ref: dy[n, o, cell] w[o, i, tap] scattered onto x[n, i, src[cell, tap]]"""
+    N, Cout, H, W = dy.shape
+    Cin = w.shape[1]
+    g = torch.einsum('nop,oit->nipt', dy.reshape(N, Cout, H * W), w.reshape(Cout, Cin, -1))
+    dx = dy.new_zeros(N, Cin, H * W + 1)
+    dx.index_add_(2, src.to(dy.device).reshape(-1), g.reshape(N, Cin, -1))
+    return dx[:, :, :H * W].reshape(N, Cin, H, W)
+
+
+def conv_ref_weight(dy, x, src, kh, kw):
+    """the weight gradient of conv_ref: sum over (n, cell) of dy[n, o, cell] x[n, i, src[cell, tap]]"""
+    N, Cout = dy.shape[:2]
+    dw = torch.einsum('nop,nipt->oit', dy.reshape(N, Cout, -1), _conv_cols(x, src))
+    return dw.reshape(Cout, x.shape[1], kh, kw)
+
+
+_GEMM_RE = re.compile(r'(gemm_tower_kernel|gemm_wgrad_kernel|gemm_tf32x3_kernel|gemm_bf16_kernel)<([^>]*)>')
 
 
 def traced_gemms(fn, attempts=3, runs=1, repeat=1):
