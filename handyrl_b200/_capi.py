@@ -11,7 +11,7 @@ import threading
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libhrl_b200.so')
 
-HRL_ABI_VERSION = 2
+HRL_ABI_VERSION = 3
 ALGO_ID = {'MC': 0, 'TD': 1, 'UPGO': 2, 'VTRACE': 3}
 LOSS_KEYS = ('p', 'v', 'r', 'ent', 'total', 'dcnt')
 NUM_LOSS = 6
@@ -146,17 +146,11 @@ SYMBOLS = {
                            [C.c_void_p] * 5 + [C.c_void_p]),
     'hrl_sumsq_num_partials': (C.c_int32, []),
     'hrl_grad_sumsq': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
-    'hrl_clip_adam_step': (C.c_int, [C.c_void_p] * 4 + [C.c_int64] + [C.c_void_p] * 3 +
-                           [C.c_double] * 5 + [C.c_void_p, C.c_void_p]),
-    'hrl_clip_adam_step_diag': (C.c_int, [C.c_void_p] * 4 + [C.c_int64] + [C.c_void_p] * 3 +
-                                [C.c_double] * 5 + [C.c_void_p, C.c_void_p, C.c_void_p]),
-    'hrl_clip_adam_step_guarded': (C.c_int, [C.c_void_p] * 4 + [C.c_int64] + [C.c_void_p] * 3 + [C.c_double] * 5 +
-                                   [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'hrl_clip_adam_step': (C.c_int, [C.c_void_p] * 4 + [C.c_int64] + [C.c_void_p] * 3 + [C.c_double] * 5 +
+                           [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     'hrl_step_commit': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                   C.c_void_p]),
-    'hrl_weight_ema': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_int32, C.c_void_p]),
-    'hrl_weight_ema_guarded': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_int32, C.c_void_p,
-                                         C.c_void_p]),
+    'hrl_weight_ema': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_int32, C.c_void_p, C.c_void_p]),
     'hrl_sum_rows': (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_void_p, C.c_void_p]),
     'hrl_peer_allreduce_sumsq': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int64, C.c_int64,
                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -173,14 +167,12 @@ SYMBOLS = {
     'hrl_gemm_fused': (C.c_int, [C.POINTER(HrlGemmArgs), C.c_void_p]),
     'hrl_bn_finalize_fwd': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_float] +
                             [C.c_void_p] * 8),
-    'hrl_bn_finalize_bwd': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 9),
-    'hrl_bn_finalize_bwd_accumulate': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 8 +
-                                       [C.c_int32, C.c_void_p]),
+    'hrl_bn_finalize_bwd': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64] + [C.c_void_p] * 8 +
+                            [C.c_int32, C.c_void_p]),
     'hrl_heads_num_blocks': (C.c_int32, [C.c_int64]),
     'hrl_heads_fwd': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_int32] * 5 + [C.c_float] + [C.c_void_p] * 7),
-    'hrl_heads_bwd': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_int32] * 5 + [C.c_float] + [C.c_void_p] * 16),
-    'hrl_heads_bwd_accumulate': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_int32] * 5 + [C.c_float] + [C.c_void_p] * 15 +
-                                 [C.c_int32, C.c_void_p]),
+    'hrl_heads_bwd': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64] + [C.c_int32] * 5 + [C.c_float] + [C.c_void_p] * 15 +
+                      [C.c_int32, C.c_void_p]),
     'hrl_gemm_set_debug': (None, [C.c_int]),
     'hrl_gemm_padded_rows': (C.c_int32, [C.c_int64]),
     'hrl_board_pack_floats': (C.c_size_t, [C.c_int64, C.c_int64]),

@@ -281,61 +281,29 @@ extern "C" int hrl_grad_sumsq(const float *grad, int64_t n, float *partials, voi
     return HRL_OK;
 }
 
-namespace hrl {
-template <bool DIAG, bool GUARD>
-static int clip_adam_step(const char *name, float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
-                          const float *partials, const float *lr, int64_t *step, double max_norm, double beta1, double beta2,
-                          double eps, double weight_decay, float *grad_norm_out, double *diag, const float *tail, int32_t n_tail,
-                          int32_t *skip, void *stream) {
+extern "C" int hrl_clip_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
+                                  const float *partials, const float *lr, int64_t *step, double max_norm, double beta1,
+                                  double beta2, double eps, double weight_decay, float *grad_norm_out, double *diag_accum,
+                                  const float *tail, int32_t n_tail, int32_t *skip, void *stream) {
+    using namespace hrl;
     HRL_REQUIRE(param && grad && exp_avg && exp_avg_sq && partials && lr && step && n > 0, HRL_ERR_BAD_ARG,
-                "%s: NULL pointer or n <= 0", name);
-    HRL_REQUIRE(!DIAG || diag, HRL_ERR_BAD_ARG, "%s: diag_accum is NULL", name);
-    HRL_REQUIRE(!GUARD || (skip && n_tail >= 0 && (tail || n_tail == 0)), HRL_ERR_BAD_ARG,
-                "%s: skip is NULL, or tail is NULL with n_tail > 0, or n_tail < 0", name);
+                "hrl_clip_adam_step: NULL pointer or n <= 0");
+    HRL_REQUIRE(!skip || (n_tail >= 0 && (tail || n_tail == 0)), HRL_ERR_BAD_ARG,
+                "hrl_clip_adam_step: tail is NULL with n_tail > 0, or n_tail < 0");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     int grid = (int)((n + kOptThreads - 1) / kOptThreads);
     if (grid > kPartials) grid = kPartials;
-    clip_adam_kernel<DIAG, GUARD><<<grid, kOptThreads, 0, s>>>(param, grad, exp_avg, exp_avg_sq, n, partials, lr, step, max_norm,
-                                                               beta1, beta2, eps, weight_decay, grad_norm_out, diag, tail,
-                                                               n_tail, skip);
+    auto kernel = diag_accum ? (skip ? clip_adam_kernel<true, true> : clip_adam_kernel<true, false>)
+                             : (skip ? clip_adam_kernel<false, true> : clip_adam_kernel<false, false>);
+    kernel<<<grid, kOptThreads, 0, s>>>(param, grad, exp_avg, exp_avg_sq, n, partials, lr, step, max_norm, beta1, beta2, eps,
+                                        weight_decay, grad_norm_out, diag_accum, tail, n_tail, skip);
     HRL_CUDA_CHECK(cudaGetLastError());
-    if (GUARD)
+    if (skip)
         bump_step_guarded_kernel<<<1, 1, 0, s>>>(step, skip);
     else
         bump_step_kernel<<<1, 1, 0, s>>>(step);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
-}
-}  // namespace hrl
-
-extern "C" int hrl_clip_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
-                                  const float *partials, const float *lr, int64_t *step, double max_norm, double beta1,
-                                  double beta2, double eps, double weight_decay, float *grad_norm_out, void *stream) {
-    return hrl::clip_adam_step<false, false>("hrl_clip_adam_step", param, grad, exp_avg, exp_avg_sq, n, partials, lr, step,
-                                             max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, nullptr, nullptr, 0,
-                                             nullptr, stream);
-}
-
-extern "C" int hrl_clip_adam_step_diag(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
-                                       const float *partials, const float *lr, int64_t *step, double max_norm, double beta1,
-                                       double beta2, double eps, double weight_decay, float *grad_norm_out, double *diag_accum,
-                                       void *stream) {
-    return hrl::clip_adam_step<true, false>("hrl_clip_adam_step_diag", param, grad, exp_avg, exp_avg_sq, n, partials, lr, step,
-                                            max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, diag_accum, nullptr, 0,
-                                            nullptr, stream);
-}
-
-extern "C" int hrl_clip_adam_step_guarded(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n,
-                                          const float *partials, const float *lr, int64_t *step, double max_norm, double beta1,
-                                          double beta2, double eps, double weight_decay, float *grad_norm_out,
-                                          const float *tail, int32_t n_tail, double *diag_accum, int32_t *skip, void *stream) {
-    if (diag_accum)
-        return hrl::clip_adam_step<true, true>("hrl_clip_adam_step_guarded", param, grad, exp_avg, exp_avg_sq, n, partials, lr,
-                                               step, max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, diag_accum, tail,
-                                               n_tail, skip, stream);
-    return hrl::clip_adam_step<false, true>("hrl_clip_adam_step_guarded", param, grad, exp_avg, exp_avg_sq, n, partials, lr,
-                                            step, max_norm, beta1, beta2, eps, weight_decay, grad_norm_out, nullptr, tail,
-                                            n_tail, skip, stream);
 }
 
 extern "C" int hrl_step_commit(const int32_t *skip, const float *tail, int32_t n_tail, double *accum, double *skip_count,
@@ -356,33 +324,22 @@ extern "C" int hrl_step_commit(const int32_t *skip, const float *tail, int32_t n
     return HRL_OK;
 }
 
-namespace hrl {
-template <bool GUARD>
-static int weight_ema(const char *name, float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
-                      const int32_t *skip, void *stream) {
-    HRL_REQUIRE(avg && state && step && n > 0 && (!GUARD || skip), HRL_ERR_BAD_ARG, "%s: NULL pointer or n <= 0", name);
+extern "C" int hrl_weight_ema(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
+                              const int32_t *skip, void *stream) {
+    using namespace hrl;
+    HRL_REQUIRE(avg && state && step && n > 0, HRL_ERR_BAD_ARG, "hrl_weight_ema: NULL pointer or n <= 0");
     HRL_REQUIRE(((reinterpret_cast<uintptr_t>(avg) | reinterpret_cast<uintptr_t>(state)) & 15) == 0, HRL_ERR_BAD_ARG,
-                "%s: avg and state must be 16-byte aligned", name);
-    HRL_REQUIRE(decay > 0.f && decay < 1.f, HRL_ERR_BAD_ARG, "%s: decay must lie in (0, 1), got %g", name, (double)decay);
+                "hrl_weight_ema: avg and state must be 16-byte aligned");
+    HRL_REQUIRE(decay > 0.f && decay < 1.f, HRL_ERR_BAD_ARG, "hrl_weight_ema: decay must lie in (0, 1), got %g", (double)decay);
     const int64_t n4 = n >> 2;
     int64_t grid = (n4 + kOptThreads - 1) / kOptThreads;
     if (grid < 1) grid = 1;                     // n < 4: block 0 does the tail alone
     if (grid > 4 * kNumSM) grid = 4 * kNumSM;
-    weight_ema_kernel<GUARD><<<(int)grid, kOptThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(avg, state, n, step, decay,
-                                                                                                    seeded ? 1 : 0, skip);
+    auto kernel = skip ? weight_ema_kernel<true> : weight_ema_kernel<false>;
+    kernel<<<(int)grid, kOptThreads, 0, reinterpret_cast<cudaStream_t>(stream)>>>(avg, state, n, step, decay, seeded ? 1 : 0,
+                                                                                  skip);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
-}
-}  // namespace hrl
-
-extern "C" int hrl_weight_ema(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
-                              void *stream) {
-    return hrl::weight_ema<false>("hrl_weight_ema", avg, state, n, step, decay, seeded, nullptr, stream);
-}
-
-extern "C" int hrl_weight_ema_guarded(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
-                                      const int32_t *skip, void *stream) {
-    return hrl::weight_ema<true>("hrl_weight_ema_guarded", avg, state, n, step, decay, seeded, skip, stream);
 }
 
 extern "C" int hrl_sum_rows(const float *rows, int32_t k, int64_t ld, int32_t n, float *out, void *stream) {

@@ -7,7 +7,7 @@
 //                         (samples x C*HW) activation matrix, the constants the next product's operand transform applies:
 //                         scale = gamma*rstd, shift = beta - mean*scale (plus mean and rstd for the backward)
 //   hrl_bn_finalize_bwd   column sums of dZ and dZ*xhat (epilogue MASK_STATS) -> dgamma, dbeta and the per-column constants
-//                         of dY = dZ*p + Y*q + r (the BatchNorm backward as an operand transform); the _accumulate form adds
+//                         of dY = dZ*p + Y*q + r (the BatchNorm backward as an operand transform); with `accumulate` it adds
 //                         dgamma / dbeta to what they hold (micro-batches after the first of a gradient-accumulation step)
 //   hrl_heads_fwd / _bwd  the 1x1-conv "squeeze" outputs (already a product) -> LeakyReLU -> bias-free Linear policy /
 //                         tanh value / return heads, and their backward including the parameter gradients
@@ -244,9 +244,9 @@ extern "C" int hrl_bn_finalize_fwd(const float *col_partials, int32_t tiles, int
     return HRL_OK;
 }
 
-extern "C" int hrl_bn_finalize_bwd_accumulate(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows,
-                                              const float *gamma, const float *mean_col, const float *rstd_col, float *dgamma, float *dbeta,
-                                              float *p_col, float *q_col, float *r_col, int32_t accumulate, void *stream) {
+extern "C" int hrl_bn_finalize_bwd(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows, const float *gamma,
+                                   const float *mean_col, const float *rstd_col, float *dgamma, float *dbeta, float *p_col, float *q_col,
+                                   float *r_col, int32_t accumulate, void *stream) {
     HRL_REQUIRE(col_partials && dbeta && tiles > 0 && C > 0 && HW > 0 && rows > 0, HRL_ERR_BAD_ARG, "hrl_bn_finalize_bwd: NULL pointer or bad shape");
     HRL_REQUIRE(gamma == nullptr || (mean_col && rstd_col && dgamma && p_col && q_col && r_col), HRL_ERR_BAD_ARG,
                 "hrl_bn_finalize_bwd: with gamma, every BatchNorm output is required");
@@ -255,13 +255,6 @@ extern "C" int hrl_bn_finalize_bwd_accumulate(const float *col_partials, int32_t
                                                                                        accumulate ? 1 : 0);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
-}
-
-extern "C" int hrl_bn_finalize_bwd(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows, const float *gamma,
-                                   const float *mean_col, const float *rstd_col, float *dgamma, float *dbeta, float *p_col, float *q_col,
-                                   float *r_col, void *stream) {
-    return hrl_bn_finalize_bwd_accumulate(col_partials, tiles, C, HW, rows, gamma, mean_col, rstd_col, dgamma, dbeta, p_col, q_col, r_col, 0,
-                                          stream);
 }
 
 static int heads_dims(int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps, int32_t A, HeadsDims &d) {
@@ -285,11 +278,10 @@ extern "C" int hrl_heads_fwd(const float *pre, int64_t ld, int64_t M, int32_t ce
     return HRL_OK;
 }
 
-extern "C" int hrl_heads_bwd_accumulate(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps,
-                                        int32_t A, float slope, const float *Wp, const float *Wv, const float *Wr, const float *value,
-                                        const float *dpolicy, const float *dvalue, const float *dret, float *dpre, float *dWp, float *dWv,
-                                        float *dWr, float *dbias_p, float *dbias_v, float *dbias_r, float *workspace, int32_t accumulate,
-                                        void *stream_) {
+extern "C" int hrl_heads_bwd(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps, int32_t A,
+                             float slope, const float *Wp, const float *Wv, const float *Wr, const float *value, const float *dpolicy,
+                             const float *dvalue, const float *dret, float *dpre, float *dWp, float *dWv, float *dWr, float *dbias_p,
+                             float *dbias_v, float *dbias_r, float *workspace, int32_t accumulate, void *stream_) {
     HeadsDims d;
     if (int e = heads_dims(cells, pmaps, vmaps, rmaps, A, d)) return e;
     HRL_REQUIRE(pre && Wp && dpolicy && dpre && dWp && dbias_p && workspace && M > 0 && (!vmaps || (Wv && value && dvalue && dWv && dbias_v)) &&
@@ -316,12 +308,4 @@ extern "C" int hrl_heads_bwd_accumulate(const float *pre, int64_t ld, int64_t M,
     heads_fold_kernel<<<(at + 127) / 128, 128, 0, stream>>>(workspace, blocks, plan, accumulate ? 1 : 0);
     HRL_CUDA_CHECK(cudaGetLastError());
     return HRL_OK;
-}
-
-extern "C" int hrl_heads_bwd(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps, int32_t A,
-                             float slope, const float *Wp, const float *Wv, const float *Wr, const float *value, const float *dpolicy,
-                             const float *dvalue, const float *dret, float *dpre, float *dWp, float *dWv, float *dWr, float *dbias_p,
-                             float *dbias_v, float *dbias_r, float *workspace, void *stream) {
-    return hrl_heads_bwd_accumulate(pre, ld, M, cells, pmaps, vmaps, rmaps, A, slope, Wp, Wv, Wr, value, dpolicy, dvalue, dret, dpre, dWp, dWv,
-                                    dWr, dbias_p, dbias_v, dbias_r, workspace, 0, stream);
 }

@@ -398,7 +398,7 @@ class FlatAdam:
         # every step adds its pre-clip norm statistics to, in the step's own launch; None = off
         self.diag = None
         # guard against non-finite steps: a one-element int32 CUDA tensor the step sets to 1 when it rejected itself (the
-        # pre-clip norm or one of the first `guard_tail` extra slots of the bucket not finite; hrl_clip_adam_step_guarded),
+        # pre-clip norm or one of the first `guard_tail` extra slots of the bucket not finite; hrl_clip_adam_step),
         # else 0; None = off
         self.skip = None
         self.guard_tail = 0
@@ -428,12 +428,7 @@ class FlatAdam:
         if self.skip is not None:
             assert self.skip.is_cuda and self.skip.dtype == torch.int32 and self.skip.numel() == 1
             assert 0 <= self.guard_tail <= self.extra and grad.numel() >= self.n_pad + self.extra
-            check(lib().hrl_clip_adam_step_guarded(*fixed, _ptr(grad[self.n_pad:]), self.guard_tail, _ptr(self.diag),
-                                                   _ptr(self.skip), s))
-        elif self.diag is not None:
-            check(lib().hrl_clip_adam_step_diag(*fixed, _ptr(self.diag), s))
-        else:
-            check(lib().hrl_clip_adam_step(*fixed, s))
+        check(lib().hrl_clip_adam_step(*fixed, _ptr(self.diag), _ptr(grad[self.n_pad:]), self.guard_tail, _ptr(self.skip), s))
 
     def step(self):
         s = _stream_ptr()
@@ -452,7 +447,7 @@ def _check_skip(skip):
 def weight_ema_update(avg, state_f32, step_count, decay, seeded, skip=None):
     """avg <- fmaf(w, state_f32 - avg, avg) in place, w = max(1 - decay, 1 / t) (1 - decay when `seeded`), t = the int64 device
     counter `step_count` as it stands when the launch runs (hrl_weight_ema, csrc/optim_kernel.cu).  One launch, graph-capturable.
-    `skip` (FlatAdam.skip of a guarded optimiser): the launch changes nothing when that step was rejected (hrl_weight_ema_guarded)."""
+    `skip` (FlatAdam.skip of a guarded optimiser, or None): the launch changes nothing when that step was rejected."""
     for t, name in ((avg, 'avg'), (state_f32, 'state_f32')):
         if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
             raise _capi.HrlError('handyrl_b200: %s must be a contiguous float32 CUDA tensor' % name)
@@ -460,13 +455,10 @@ def weight_ema_update(avg, state_f32, step_count, decay, seeded, skip=None):
         raise _capi.HrlError('handyrl_b200: avg (%d) and state_f32 (%d) differ in size' % (avg.numel(), state_f32.numel()))
     if not (step_count.is_cuda and step_count.dtype == torch.int64 and step_count.numel() == 1):
         raise _capi.HrlError('handyrl_b200: step_count must be a one-element int64 CUDA tensor')
-    if skip is None:
-        check(lib().hrl_weight_ema(_ptr(avg), _ptr(state_f32), avg.numel(), _ptr(step_count), float(decay), int(bool(seeded)),
-                                   _stream_ptr()))
-    else:
+    if skip is not None:
         _check_skip(skip)
-        check(lib().hrl_weight_ema_guarded(_ptr(avg), _ptr(state_f32), avg.numel(), _ptr(step_count), float(decay),
-                                           int(bool(seeded)), _ptr(skip), _stream_ptr()))
+    check(lib().hrl_weight_ema(_ptr(avg), _ptr(state_f32), avg.numel(), _ptr(step_count), float(decay), int(bool(seeded)),
+                               _ptr(skip), _stream_ptr()))
     _count()
 
 

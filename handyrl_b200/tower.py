@@ -257,7 +257,7 @@ class FusedBoardNet:
             dpolicy, dvalue = dpolicy.contiguous(), dvalue.contiguous()
             dreturn = dreturn.contiguous() if self.rmaps else None
             acc = int(accumulate)
-            check(lib().hrl_heads_bwd_accumulate(_ptr(self.Hpre), self.ldh, M_, self.cells, self.pmaps, self.vmaps, self.rmaps, self.A, self.slope,
+            check(lib().hrl_heads_bwd(_ptr(self.Hpre), self.ldh, M_, self.cells, self.pmaps, self.vmaps, self.rmaps, self.A, self.slope,
                                       _ptr(m.p_out.weight), _ptr(m.v_out.weight), _ptr(m.r_out.weight) if self.rmaps else None,
                                       _ptr(self.value), _ptr(dpolicy), _ptr(dvalue),
                                       _ptr(dreturn), _ptr(self.dHpre),
@@ -277,9 +277,9 @@ class FusedBoardNet:
             for l in range(L - 1, -1, -1):
                 blk, st = m.tower[l], self.bn[l]
                 bnm = blk[1]
-                check(lib().hrl_bn_finalize_bwd_accumulate(_ptr(self.cp), self.tiles, self.width, self.cells, M_, _ptr(bnm.weight),
-                                                           _ptr(st['mean']), _ptr(st['rstd']), _ptr(g(bnm.weight)), _ptr(g(bnm.bias)),
-                                                           _ptr(st['p']), _ptr(st['q']), _ptr(st['r']), acc, _stream_ptr()))
+                check(lib().hrl_bn_finalize_bwd(_ptr(self.cp), self.tiles, self.width, self.cells, M_, _ptr(bnm.weight),
+                                                _ptr(st['mean']), _ptr(st['rstd']), _ptr(g(bnm.weight)), _ptr(g(bnm.bias)),
+                                                _ptr(st['p']), _ptr(st['q']), _ptr(st['r']), acc, _stream_ptr()))
                 _count()
                 dy = dict(t=self.dZ[l], t2=self.Y[l], consts=(st['p'], st['q'], st['r']))            # dY_l from dZ_l on the fly
                 if l > 0:
@@ -295,8 +295,8 @@ class FusedBoardNet:
                 else:
                     self._gemm(dy, dict(t=self.Wb[0], packed=True), self.dZ0, K=D, N=D, epilogue='mask_stats', ep=dict(y=self.A0))
             # stem: bias gradient from the column sums of dZ0, weight gradient over the raw observations
-            check(lib().hrl_bn_finalize_bwd_accumulate(_ptr(self.cp), self.tiles, self.width, self.cells, M_, None, None, None, None,
-                                                       _ptr(g(m.stem.bias)), None, None, None, acc, _stream_ptr()))
+            check(lib().hrl_bn_finalize_bwd(_ptr(self.cp), self.tiles, self.width, self.cells, M_, None, None, None, None,
+                                            _ptr(g(m.stem.bias)), None, None, None, acc, _stream_ptr()))
             _count()
             self._wgrad(dict(t=self.dZ0, kmajor=False), dict(t=self.x2d, kmajor=False), D, self.K0, ('stem', 0), [(g(m.stem.weight), 0)])
             self._fold_all(accumulate)

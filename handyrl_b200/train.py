@@ -615,32 +615,27 @@ def nonfinite_guard(args):
     return bool(args.get('skip_nonfinite'))
 
 
-def accum_slots(diagnostics, skip_nonfinite, distill=False):
-    """Float64 slots of the learner's epoch accumulator (LearnerStep.accum): the NUM_LOSS loss sums, then the NUM_DIAG
-    diagnostics sums when diagnostics are on, then the count of rejected steps when the guard is on, then the two
-    distillation sums (kl, c_n * kl) when distillation is on."""
-    return NUM_LOSS + (NUM_DIAG if diagnostics else 0) + (1 if skip_nonfinite else 0) + (NUM_DISTILL if distill else 0)
-
-
-# the distillation sums [kl, c_n * kl] (distill.py): the last slots of the accumulator and of the bucket tail
+# the distillation sums [kl, c_n * kl] (distill.py)
 NUM_DISTILL = 2
 
-
-def _distill_slots(diagnostics, skip_nonfinite):
-    """The slice of the distillation sums in an accumulator of accum_slots(diagnostics, skip_nonfinite, True) slots."""
-    n = accum_slots(diagnostics, skip_nonfinite)
-    return slice(n, n + NUM_DISTILL)
+AccumLayout = collections.namedtuple('AccumLayout', 'loss distill diag skipped n_tail n')
 
 
-# the loss pass's diagnostics sums: where they sit behind the loss sums, in the accumulator and in the gradient bucket's tail
-_LOSS_DIAG = slice(NUM_LOSS, NUM_LOSS + NUM_LOSS_DIAG)
+def accum_layout(diagnostics=False, skip_nonfinite=False, distill=False):
+    """The AccumLayout of the learner's float64 epoch accumulator (LearnerStep.accum) with these options on: the slices
+    `loss`, `distill`, `diag` and `skipped` (None when their option is off) and the size `n`.  Its first n_tail slots are
+    the step's float32 tail at the same offsets -- each row of LearnerStep.loss_rows and the gradient bucket's extra slots
+    start with it -- so a step adds its whole tail to the accumulator in one piece:
 
+        tail         [loss NUM_LOSS | distill NUM_DISTILL, when distilling | the loss pass's diagnostics NUM_LOSS_DIAG]
+        accumulator  [tail | the optimiser's diagnostics NUM_DIAG - NUM_LOSS_DIAG | skipped 1, with the guard]
 
-def _accum_layout(diagnostics, skip_nonfinite):
-    """(loss, diag, skipped) slices of an accumulator of accum_slots(diagnostics, skip_nonfinite) slots; `diag` is None
-    without diagnostics and `skipped` (one slot) None without the guard."""
-    n = NUM_LOSS + (NUM_DIAG if diagnostics else 0)
-    return slice(0, NUM_LOSS), slice(NUM_LOSS, n) if diagnostics else None, slice(n, n + 1) if skip_nonfinite else None
+    `diag` is both kinds of diagnostics in DIAG_KEYS order."""
+    d = NUM_LOSS + (NUM_DISTILL if distill else 0)
+    n = d + (NUM_DIAG if diagnostics else 0)
+    return AccumLayout(loss=slice(0, NUM_LOSS), distill=slice(NUM_LOSS, d) if distill else None,
+                       diag=slice(d, n) if diagnostics else None, skipped=slice(n, n + 1) if skip_nonfinite else None,
+                       n_tail=d + (NUM_LOSS_DIAG if diagnostics else 0), n=n + (1 if skip_nonfinite else 0))
 
 
 def skipped_line(skipped, steps):
@@ -794,22 +789,21 @@ class PendingModel:
     optimiser state ('optim', the optim_snap layout), it leaves that state in the OptimizerStateFormat dict in `optim_state`,
     scheduled at step count `steps`.  With validation passes ('val'), it prints their lines after the loss line and leaves
     their sums in `validation` (what LearnerStep.pop_validation() returns).  `host_losses` holds the learner's accumulator in
-    the layout `diagnostics` and
-    `skip_nonfinite` give (accum_slots); with the guard, the number of the epoch's `batch_cnt` steps that were rejected is left
+    the layout `diagnostics`, `skip_nonfinite` and
+    `distill` give (accum_layout, in `slots`); with the guard, the number of the epoch's `batch_cnt` steps that were rejected is left
     in `skipped` and, when it is not zero, printed (skipped_line) after the loss and diagnostics lines.  The Trainer sets
     `replay_ratio` to the epoch's ReplayRatioLimiter.end_epoch() figures under train_args['replay_ratio'], and report() prints
     them (replay_ratio_line) after those lines and before the validation lines.  Under train_args['save_replay'] the Trainer
     sets `replay` to the GpuBatcher.snapshot() taken at the boundary, and with the priorities ('prio', the prio_snap layout)
     resolve() leaves them in `priority_state` (what LearnerStep.priority_state_dict() returns).  With distillation
-    (`distill`), the accumulator ends in the epoch's sums of kl and c_n * kl: report() leaves them in `distill` and prints
+    (`distill`), the accumulator holds the epoch's sums of kl and c_n * kl: report() leaves them in `distill` and prints
     distill.line() after the loss and diagnostics lines and before the skipped line."""
 
     def __init__(self, stepper, done_event, host_state, host_losses, heads, template, host=None, steps=0, diagnostics=False,
                  skip_nonfinite=False, batch_cnt=0, distill=False):
         self.stepper, self.done, self.host_state, self.host_losses = stepper, done_event, host_state, host_losses
         self.heads, self.template, self.host, self.steps = heads, template, host or {}, steps
-        self.has_diagnostics, self.skip_nonfinite, self.batch_cnt = bool(diagnostics), bool(skip_nonfinite), batch_cnt
-        self.has_distill = bool(distill)
+        self.slots, self.batch_cnt = accum_layout(diagnostics, skip_nonfinite, distill), batch_cnt
         self.distill = None
         self.ema_state = None
         self.optim_state = None
@@ -822,16 +816,15 @@ class PendingModel:
     def report(self):
         """Read the epoch's sums from the host copy (already arrived) and print the epoch's lines; returns the loss sums."""
         host = self.host_losses.tolist()
-        n_slots = accum_slots(self.has_diagnostics, self.skip_nonfinite, self.has_distill)
-        if len(host) != n_slots:
-            raise ValueError('PendingModel: %d accumulator slots, the layout has %d' % (len(host), n_slots))
-        loss, diag, skipped = _accum_layout(self.has_diagnostics, self.skip_nonfinite)
-        sums = dict(zip(LOSS_KEYS, host[loss]))
+        slots = self.slots
+        if len(host) != slots.n:
+            raise ValueError('PendingModel: %d accumulator slots, the layout has %d' % (len(host), slots.n))
+        sums = dict(zip(LOSS_KEYS, host[slots.loss]))
         dcnt = sums['dcnt']
-        self.diagnostics = ops.summarize_diagnostics(host[diag]) if self.has_diagnostics else None
-        self.skipped = int(host[skipped][0]) if self.skip_nonfinite else 0
-        if self.has_distill:
-            self.distill = dict(zip(('kl', 'term'), host[_distill_slots(self.has_diagnostics, self.skip_nonfinite)]))
+        self.diagnostics = ops.summarize_diagnostics(host[slots.diag]) if slots.diag is not None else None
+        self.skipped = int(host[slots.skipped][0]) if slots.skipped is not None else 0
+        if slots.distill is not None:
+            self.distill = dict(zip(('kl', 'term'), host[slots.distill]))
         if dcnt > 0:
             print(loss_line('loss', sums, self.heads))
             if self.diagnostics is not None:
@@ -939,7 +932,7 @@ class LearnerStep:
     capture steps) the weights train exactly as without the key and no priority moves.
 
     skip_nonfinite (default: train_args['skip_nonfinite'], off): a step whose pre-clip gradient norm or one of whose six loss
-    sums is not finite is rejected on the device (ops.FlatAdam.skip, hrl_clip_adam_step_guarded), and the learner is left
+    sums is not finite is rejected on the device (ops.FlatAdam.skip, hrl_clip_adam_step with a skip flag), and the learner is left
     bit for bit as if its batch had never been drawn: weights, Adam's moments and step count, the BatchNorm buffers (saved by
     one device-to-device copy at the start of every step and put back by hrl_step_commit), the epoch's loss and diagnostics
     sums and the weight average.  Only the count of rejected steps (`skipped`, the accumulator's last slot; handed over as
@@ -968,9 +961,9 @@ class LearnerStep:
     module path (optimize_small_boards in the step's tensor_cores mode, its own channels-last probe, forward_raw with its own
     init_hidden and train=False), never on the fused tower -- then the student, the fused loss kernel, one more launch
     (ops.distill_fwd_bwd) that adds c_n * KL(teacher || student) to the policy gradient and to the loss row's total, and the
-    backward.  Its two sums [kl, c_n * kl] (distill_col of the loss row) follow the bucket tail and end the accumulator
-    (`distill_accum`); the teacher's weights are in no bucket, hand-off or checkpoint.  With c_n = 0 the step is bit for bit
-    the step without the key.  Validation passes are unchanged.
+    backward.  Its two sums [kl, c_n * kl] follow the loss sums in the loss row, the bucket tail and the accumulator
+    (`distill_accum`; accum_layout); the teacher's weights are in no bucket, hand-off or checkpoint.  With c_n = 0 the step
+    is bit for bit the step without the key.  Validation passes are unchanged.
 
     A feature that adds device state registers it in __init__, where it allocates it: in `_mutable` (or `_zeroed`) when a
     step or validation pass changes it, so that the capture's warm-up leaves it as it was, and in `_handoff` (a _Handoff)
@@ -1007,13 +1000,7 @@ class LearnerStep:
         if diagnostics is None:
             diagnostics = bool(args.get('diagnostics', False))
         self.diagnostics = diagnostics
-        distilling = self.teacher is not None
-        n_sums = accum_slots(diagnostics, self.skip_nonfinite, distilling)  # accumulator: loss sums [+ diagnostics] [+ skips] [+ distill]
-        self.n_tail = _LOSS_DIAG.stop if diagnostics else NUM_LOSS         # bucket tail: [+ the loss pass's diagnostics]
-        # distillation: its sums follow the tail, in the loss row's columns [distill_col, n_tail), which the loss pass leaves
-        # unused (or writes zeros to, for the optimiser's diagnostics entries, before the distillation launch runs)
-        self.distill_col = self.n_tail if distilling else None
-        self.n_tail += NUM_DISTILL if distilling else 0
+        self.slots = accum_layout(diagnostics, self.skip_nonfinite, self.teacher is not None)    # accumulator and bucket tail
         # the learner owns its precision contract (1e-5 of the reference's fp32 arithmetic): PyTorch's default lets
         # cuDNN convolutions run on TF32 tensor cores (10-bit mantissa).  train_args['allow_tf32'] = True opts out.
         if allow_tf32 is None:
@@ -1061,7 +1048,7 @@ class LearnerStep:
             peer_allreduce = self.world > 1 and os.environ.get('HRL_PEER_ALLREDUCE', '1') != '0'
         self.peer = ops.PeerAllReduce(self.pg, self.device) if (peer_allreduce and self.world > 1) else None
         self.state = StateStore(self.model, self.device)
-        self.opt = ops.FlatAdam(params, lr=lr, weight_decay=weight_decay, max_norm=max_norm, extra=self.n_tail,
+        self.opt = ops.FlatAdam(params, lr=lr, weight_decay=weight_decay, max_norm=max_norm, extra=self.slots.n_tail,
                                 grad_alloc=self.peer.alloc if self.peer is not None else None,
                                 param_storage=self.state.flat_param)
         self.state.index_params(self.model)
@@ -1075,7 +1062,7 @@ class LearnerStep:
             [self.opt.exp_avg, self.opt.exp_avg_sq, self.opt.step_count]
         self._zeroed = []
         snap = torch.empty_like(self.state.bytes)
-        self.acc_snap = torch.zeros(n_sums, dtype=torch.float64, device=self.device)       # filled by epoch_schedule
+        self.acc_snap = torch.zeros(self.slots.n, dtype=torch.float64, device=self.device)       # filled by epoch_schedule
         self._handoff = [_Handoff('state', snap, [(snap, self.state.bytes)]), _Handoff('losses', self.acc_snap, [])]
         self.avg_bytes = self.avg = None       # moving average of the fp32 state: a copy of bytes [0, i_off)
         self.avg_seeded = False
@@ -1130,12 +1117,12 @@ class LearnerStep:
             self._handoff.append(_Handoff('prio', self.prio_snap, self._prio_copies(self.prio_snap)))
         Bm = B // k                      # windows per micro-batch: what the net and the loss kernel see at once
         # micro-batch i: views of rows [i*Bm, (i+1)*Bm) of every (batch-major) tensor of the packed batch and of the window
-        # weights (k = 1: the whole batch); its loss pass writes its sums to row i of loss_rows ([NUM_LOSS sums | NUM_DIAG
-        # diagnostics]) and its rows of the advantage tap (_build_loss_buffers)
+        # weights (k = 1: the whole batch); its loss pass writes its sums to row i of loss_rows (the tail's columns, then the
+        # zeros of the optimiser's diagnostics entries) and its rows of the advantage tap (_build_loss_buffers)
         self._micro = [tree_map(lambda t, i=i: t[i * Bm:(i + 1) * Bm], self.dev) for i in range(k)]
         self._win_weight = [self.prio_state.win_weight[i * Bm:(i + 1) * Bm] if self.prio_state is not None else None
                             for i in range(k)]
-        self.loss_rows = torch.zeros((k, NUM_LOSS + NUM_DIAG), dtype=torch.float32, device=self.device)
+        self.loss_rows = torch.zeros((k, NUM_LOSS + NUM_DISTILL + NUM_DIAG), dtype=torch.float32, device=self.device)
         self.advantage = torch.zeros((B, T, P, 1), dtype=torch.float32, device=self.device) if self.prio_state is not None else None
         self.hidden0 = self.teacher_hidden0 = None
         if hasattr(self.model, 'init_hidden'):
@@ -1148,21 +1135,20 @@ class LearnerStep:
             self.engine = tower.FusedBoardNet(self.model, Bm * T * Pa, self.device, bf16=tensor_cores == 'bf16')
         self.loss_buf = self._loss_bufs = None      # built by the first forward (_build_loss_buffers)
         self.last_losses = torch.zeros(NUM_LOSS, device=self.device)
-        self.accum = torch.zeros(n_sums, dtype=torch.float64, device=self.device)
+        self.accum = torch.zeros(self.slots.n, dtype=torch.float64, device=self.device)
         self._mutable.append(self.accum)
-        loss, diag, skipped = _accum_layout(diagnostics, self.skip_nonfinite)
-        self.loss_accum = self.accum[loss]
+        self.loss_accum = self.accum[self.slots.loss]
         self.diag_accum = self.distill_accum = None
-        if distilling:
-            self.distill_accum = self.accum[_distill_slots(diagnostics, self.skip_nonfinite)]
+        if self.slots.distill is not None:
+            self.distill_accum = self.accum[self.slots.distill]
         if diagnostics:
-            self.diag_accum = self.accum[diag]
+            self.diag_accum = self.accum[self.slots.diag]
             self.opt.diag = self.diag_accum[NUM_LOSS_DIAG:]        # the optimiser's entries: accumulated by its own kernel
         # guard against non-finite steps: the count of rejected steps is the accumulator's last slot; the buffers the forward
         # moves (StateStore bytes [f_off, nbytes)) are saved at the start of every step and put back when it is rejected
         self.skipped = self.guard_saved = None
         if self.skip_nonfinite:
-            self.skipped = self.accum[skipped]
+            self.skipped = self.accum[self.slots.skipped]
             self.opt.skip = torch.zeros(1, dtype=torch.int32, device=self.device)
             self.opt.guard_tail = NUM_LOSS
             self._mutable.append(self.opt.skip)
@@ -1221,9 +1207,9 @@ class LearnerStep:
         self._loss_bufs = []
         for i in range(self.micro_batches):
             buf = copy.copy(base)
-            buf.losses = self.loss_rows[i, :NUM_LOSS]
+            buf.losses = self.loss_rows[i, self.slots.loss]
             if self.diagnostics:
-                buf.diagnostics = self.loss_rows[i, NUM_LOSS:]
+                buf.diagnostics = self.loss_rows[i, self.slots.diag]
             if self.advantage is not None:
                 buf.advantage = self.advantage[i * Bm:(i + 1) * Bm]
             self._loss_bufs.append(buf)
@@ -1269,14 +1255,16 @@ class LearnerStep:
             if teacher is not None:
                 ops.distill_fwd_bwd(outs['policy'], teacher, dev, self.args, buf, self.opt.step_count, self.distill['coef'],
                                     self.distill['anneal_steps'], window_weight=weight,
-                                    sums=self.loss_rows[i, self.distill_col:self.distill_col + NUM_DISTILL])
+                                    sums=self.loss_rows[i, self.slots.distill])
             self._net_backward(outs, buf, accumulate=i > 0)
             del outs, loss, teacher     # this micro-batch's activations and autograd graph go back to the pool before the next forward
-        # the loss sums [+ the loss pass's diagnostics] ride the gradient bucket: one row is copied, k rows are summed
+        # the tail (loss sums [+ distillation] [+ the loss pass's diagnostics]) rides the gradient bucket: one row is copied,
+        # k rows are summed
+        n = self.slots.n_tail
         if self.micro_batches == 1:
-            self.opt.extra_slots[:self.n_tail].copy_(self.loss_rows[0, :self.n_tail])
+            self.opt.extra_slots[:n].copy_(self.loss_rows[0, :n])
         else:
-            ops.sum_rows(self.loss_rows, self.n_tail, self.opt.extra_slots)
+            ops.sum_rows(self.loss_rows, n, self.opt.extra_slots)
         self._finish_step()
 
     def _finish_step(self):
@@ -1285,30 +1273,24 @@ class LearnerStep:
             reduced = self.peer(self.opt.n_pad, self.opt.partials)      # all-reduce + norm partials, one kernel
             self.opt.step_reduced(reduced)
             tail = reduced[self.opt.n_pad:]
-            self.last_losses.copy_(tail[:NUM_LOSS])
         else:
             if self.world > 1:
                 torch.distributed.all_reduce(self.opt.flat_grad, op=torch.distributed.ReduceOp.SUM, group=self.pg)
             self.opt.step()
             tail = self.opt.extra_slots
-            self.last_losses.copy_(tail[:NUM_LOSS])
-        n_commit = self.n_tail if self.distill_col is None else self.distill_col
+        self.last_losses.copy_(tail[:NUM_LOSS])
+        n = self.slots.n_tail
         if self.skip_nonfinite:         # one launch: accumulate an accepted step, or count a rejected one and restore its buffers
-            ops.step_commit(self.opt.skip, tail[:n_commit], self.accum, self.skipped,
+            ops.step_commit(self.opt.skip, tail[:n], self.accum[:n], self.skipped,
                             self._guarded_buffers() if self.guard_saved is not None else None, self.guard_saved)
         else:
-            self.loss_accum.add_(self.last_losses)
-            if self.diagnostics:
-                self.accum[_LOSS_DIAG].add_(tail[_LOSS_DIAG])
-        if self.distill_accum is not None:      # a rejected step adds none of its sums
-            sums = tail[self.distill_col:self.n_tail]
-            self.distill_accum.add_(sums.masked_fill(self.opt.skip.bool(), 0.0) if self.skip_nonfinite else sums)
+            self.accum[:n].add_(tail[:n])
         if self.avg is not None:        # after the optimiser: step_count already counts this step
             ops.weight_ema_update(self.avg, self.state.bytes[:self.state.i_off].view(torch.float32), self.opt.step_count,
                                   self.weight_ema, self.avg_seeded, skip=self.opt.skip)
         if self.prio_state is not None:     # after the optimiser: a rejected step stores no priority
             ops.priority_update(self.prio_state, self.advantage, self.dev['turn_mask'], self.args.get('burn_in_steps', 0),
-                                skip=self.opt.skip if self.skip_nonfinite else None)
+                                skip=self.opt.skip)
 
     def _teacher_policy(self, dev):
         """The teacher's raw policy (B', T, Pa, A) on the windows of `dev`: eval mode, no gradient, the module path."""
@@ -1714,7 +1696,7 @@ class LearnerStep:
         enqueues this at the same step, so all ranks keep identical learning rates without a broadcast."""
         self.acc_snap.copy_(self.accum)
         self.accum.zero_()
-        dcnt = self.acc_snap[5:6].float()
+        dcnt = self.acc_snap[self.slots.loss][-1:].float()     # dcnt: the last of the loss sums
         fresh = self.ema * 0.8 + dcnt * (0.2 / (1e-2 + batch_cnt))
         self.ema.copy_(torch.where(dcnt > 0, fresh, self.ema))
         self.opt.lr.copy_(self.ema * (default_lr / (1 + steps * 1e-5)))

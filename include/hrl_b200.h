@@ -18,9 +18,8 @@
  *   hrl_grad_sumsq /
  *   hrl_clip_adam_step    <- handyrl/train.py:370-371 (clip_grad_norm_(params, 4.0) + Adam.step,
  *                            Adam(lr, weight_decay=1e-5) of train.py:331)
- *   hrl_clip_adam_step_guarded /
- *   hrl_step_commit       <- the same step, rejected on the device when its loss or gradient is not finite; no
- *                            reference counterpart
+ *   hrl_step_commit       <- with the guard of hrl_clip_adam_step: the same step, rejected on the device when its loss
+ *                            or gradient is not finite; no reference counterpart
  *   hrl_weight_ema        <- a per-step moving average of the weights; no reference counterpart (scripts/aux_swa.py
  *                            averages epoch checkpoints)
  *   hrl_gather_pad        <- handyrl/train.py:33-124  (make_batch: window slice + pad + collate)
@@ -53,7 +52,7 @@
 extern "C" {
 #endif
 
-#define HRL_ABI_VERSION 2
+#define HRL_ABI_VERSION 3
 
 typedef enum {
     HRL_OK = 0,
@@ -222,33 +221,27 @@ int hrl_grad_sumsq(const float *grad, int64_t n, float *partials, void *stream);
 int hrl_clip_adam_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq,
                        int64_t n, const float *partials, const float *lr, int64_t *step,
                        double max_norm, double beta1, double beta2, double eps, double weight_decay,
-                       float *grad_norm_out /* may be NULL */, void *stream);
-/* The same step, also adding g, g^2, [g > max_norm] and 1 (g = the pre-clip norm) to diag_accum[0..3] (device doubles,
- * the HRL_DIAG_GNORM .. HRL_DIAG_STEPS entries of a diagnostics accumulator) -- in the same launch. */
-int hrl_clip_adam_step_diag(float *param, const float *grad, float *exp_avg, float *exp_avg_sq,
-                            int64_t n, const float *partials, const float *lr, int64_t *step,
-                            double max_norm, double beta1, double beta2, double eps, double weight_decay,
-                            float *grad_norm_out /* may be NULL */, double *diag_accum, void *stream);
-
+                       float *grad_norm_out /* may be NULL */, double *diag_accum /* may be NULL */,
+                       const float *tail, int32_t n_tail, int32_t *skip /* may be NULL */, void *stream);
 /*
- * Guarded form of the same step (opt-in; a batch carrying a NaN or Inf must not poison the learner).  The step is rejected
+ * diag_accum != NULL: the same launch also adds g, g^2, [g > max_norm] and 1 (g = the pre-clip norm) to diag_accum[0..3]
+ * (device doubles, the HRL_DIAG_GNORM .. HRL_DIAG_STEPS entries of a diagnostics accumulator).
+ *
+ * skip != NULL: the guarded step (opt-in; a batch carrying a NaN or Inf must not poison the learner).  The step is rejected
  * when the pre-clip norm -- the fp64 fold of the fp32 partials -- is not finite, or when one of tail[0 .. n_tail) is not
  * finite (tail: the loss sums in the reduced bucket).  A finite gradient whose fp32 sum of squares overflows makes a
  * partial Inf, so it is rejected too.  Every block folds the same partials and reads the same tail, so all blocks (and all
  * ranks of a sharded learner, which see the same reduced bucket) decide alike without communicating.
- *   accepted: the arithmetic of hrl_clip_adam_step (hrl_clip_adam_step_diag when diag_accum != NULL), bit for bit;
+ *   accepted: the arithmetic of the unguarded step, bit for bit;
  *   rejected: param, exp_avg, exp_avg_sq and diag_accum are not written, and *step is not incremented.
- * *grad_norm_out is written either way.  *skip (device int32) is set to 1 when rejected, 0 when accepted.
+ * *grad_norm_out is written either way.  *skip (device int32) is set to 1 when rejected, 0 when accepted.  skip == NULL:
+ * tail and n_tail are ignored and every step is taken.
  */
-int hrl_clip_adam_step_guarded(float *param, const float *grad, float *exp_avg, float *exp_avg_sq,
-                               int64_t n, const float *partials, const float *lr, int64_t *step,
-                               double max_norm, double beta1, double beta2, double eps, double weight_decay,
-                               float *grad_norm_out /* may be NULL */, const float *tail, int32_t n_tail,
-                               double *diag_accum /* may be NULL */, int32_t *skip, void *stream);
 
 /*
  * The accumulation that follows a guarded step, in one launch that reads *skip:
- *   accepted: accum[i] += (double)tail[i] for i < n_tail (the epoch's loss sums, then the loss pass's diagnostics sums);
+ *   accepted: accum[i] += (double)tail[i] for i < n_tail (the step's bucket tail: the epoch's loss sums, then the
+ *             distillation and loss-pass diagnostics sums when they are on);
  *   rejected: *skip_count += 1, and nbytes bytes of `saved` are copied back to `state` (the buffers -- BatchNorm running
  *             statistics, num_batches_tracked -- as they were before the step's forward moved them).
  * skip_count must not lie in accum[0 .. n_tail).  state and saved are 16-byte aligned; nbytes may be 0.
@@ -264,12 +257,11 @@ int hrl_step_commit(const int32_t *skip, const float *tail, int32_t n_tail, doub
  * where *step is the optimiser's step counter after this step's increment (hrl_clip_adam_step), read on the device so
  * that a captured CUDA graph replays correctly.  The first step (t = 1, w = 1) stores state[i] exactly and early steps
  * form an equal running mean; seeded != 0 (an average resumed from a saved one) uses w = 1 - decay from its first step.  Elementwise and
- * deterministic; avg and state 16-byte aligned, any n > 0, decay in (0, 1).
+ * deterministic; avg and state 16-byte aligned, any n > 0, decay in (0, 1).  After a guarded step (skip != NULL, the
+ * flag of hrl_clip_adam_step) nothing is written when *skip says the step was rejected.
  */
-int hrl_weight_ema(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded, void *stream);
-/* The same after a guarded step: nothing is written when *skip (hrl_clip_adam_step_guarded) says the step was rejected. */
-int hrl_weight_ema_guarded(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
-                           const int32_t *skip, void *stream);
+int hrl_weight_ema(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded,
+                   const int32_t *skip /* may be NULL */, void *stream);
 
 /*
  * Gradient accumulation (opt-in; a batch trained as k micro-batches with one optimiser step): the fused loss pass of
@@ -424,33 +416,24 @@ int hrl_gemm_fused(const HrlGemmArgs *args, void *stream);
  *                         -> policy = . Wp^T (A x pmaps*cells), value = tanh(. Wv^T), return = . Wr^T; the backward
  *                         writes dpre and the gradients of Wp / Wv / Wr and of the squeeze biases (fixed-order sums;
  *                         workspace: hrl_heads_num_blocks(M) * (A*pin + vin + rin + maps) floats).
- *   hrl_bn_finalize_bwd_accumulate / hrl_heads_bwd_accumulate: the same, except that with accumulate != 0 the parameter
- *                         gradients (dgamma, dbeta; dWp, dWv, dWr and the squeeze-bias gradients) are ADDED to what those
- *                         buffers hold (each fp32 result rounded first), for the micro-batches after the first of a
- *                         gradient-accumulation step.  dpre and p_col / q_col / r_col are written as before.  accumulate == 0
- *                         is the plain form bit for bit.
+ *   accumulate (hrl_bn_finalize_bwd, hrl_heads_bwd): 0 writes the parameter gradients (dgamma, dbeta; dWp, dWv, dWr
+ *                         and the squeeze-bias gradients); != 0 ADDS them to what those buffers hold (each fp32 result
+ *                         rounded first), for the micro-batches after the first of a gradient-accumulation step.  dpre and
+ *                         p_col / q_col / r_col are written either way.
  */
 int hrl_bn_finalize_fwd(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows, const float *gamma,
                         const float *beta, float eps, float momentum, float *running_mean, float *running_var,
                         int64_t *batches_tracked, float *mean_col, float *rstd_col, float *scale_col, float *shift_col, void *stream);
 int hrl_bn_finalize_bwd(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows, const float *gamma,
                         const float *mean_col, const float *rstd_col, float *dgamma, float *dbeta, float *p_col, float *q_col,
-                        float *r_col, void *stream);
-int hrl_bn_finalize_bwd_accumulate(const float *col_partials, int32_t tiles, int32_t C, int32_t HW, int64_t rows, const float *gamma,
-                                   const float *mean_col, const float *rstd_col, float *dgamma, float *dbeta, float *p_col, float *q_col,
-                                   float *r_col, int32_t accumulate, void *stream);
+                        float *r_col, int32_t accumulate, void *stream);
 int32_t hrl_heads_num_blocks(int64_t M);
 int hrl_heads_fwd(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps, int32_t A,
                   float slope, const float *Wp, const float *Wv, const float *Wr, float *policy, float *value, float *ret, void *stream);
 int hrl_heads_bwd(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps, int32_t A,
                   float slope, const float *Wp, const float *Wv, const float *Wr, const float *value, const float *dpolicy,
                   const float *dvalue, const float *dret, float *dpre, float *dWp, float *dWv, float *dWr, float *dbias_p,
-                  float *dbias_v, float *dbias_r, float *workspace, void *stream);
-int hrl_heads_bwd_accumulate(const float *pre, int64_t ld, int64_t M, int32_t cells, int32_t pmaps, int32_t vmaps, int32_t rmaps,
-                             int32_t A, float slope, const float *Wp, const float *Wv, const float *Wr, const float *value,
-                             const float *dpolicy, const float *dvalue, const float *dret, float *dpre, float *dWp, float *dWv,
-                             float *dWr, float *dbias_p, float *dbias_v, float *dbias_r, float *workspace, int32_t accumulate,
-                             void *stream);
+                  float *dbias_v, float *dbias_r, float *workspace, int32_t accumulate, void *stream);
 
 /*
  * Weight of a stride-1 "same" convolution (Cout,Cin,kh,kw; odd kernel, zero padding) <-> the dense matrix

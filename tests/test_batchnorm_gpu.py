@@ -263,10 +263,10 @@ def test_tower_bn_finalize_bwd(tiles, HW, stem):
     pqr = [torch.full((Cn * HW,), 7.0, device='cuda') for _ in range(3)]
     stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     if stem:
-        check(lib().hrl_bn_finalize_bwd(_p(cp), tiles, Cn, HW, rows, None, None, None, None, _p(dbeta), *map(_p, pqr), stream))
+        check(lib().hrl_bn_finalize_bwd(_p(cp), tiles, Cn, HW, rows, None, None, None, None, _p(dbeta), *map(_p, pqr), 0, stream))
     else:
         check(lib().hrl_bn_finalize_bwd(_p(cp), tiles, Cn, HW, rows, _p(gamma), _p(mean_col), _p(rstd_col), _p(dgamma), _p(dbeta),
-                                        *map(_p, pqr), stream))
+                                        *map(_p, pqr), 0, stream))
     torch.cuda.synchronize()
     p64 = cp.double().cpu().view(tiles, 2, Cn, HW)
     s, q = p64[:, 0].sum(dim=(0, 2)), p64[:, 1].sum(dim=(0, 2))

@@ -59,7 +59,7 @@ def test_appended_abi_fields():
     for n in ('HrlGemmArgs', 'HrlPackJob'):
         assert getattr(_capi, n)._fields_[-1][0] == 'bf16'
     assert _capi.SYMBOLS['hrl_conv_pack_bf16'] == _capi.SYMBOLS['hrl_conv_pack']
-    assert _capi.HRL_ABI_VERSION == 2
+    assert _capi.HRL_ABI_VERSION == 3
 
 
 def ptxas_report():

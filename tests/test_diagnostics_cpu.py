@@ -78,7 +78,7 @@ def test_diagnostics_line_is_parseable():
 
 def test_diag_indices_and_symbols_mirror_the_header():
     from handyrl_b200 import _capi
-    for name in ('hrl_loss_fwd_bwd_diag', 'hrl_loss_diag_workspace_bytes', 'hrl_clip_adam_step_diag'):
+    for name in ('hrl_loss_fwd_bwd_diag', 'hrl_loss_diag_workspace_bytes', 'hrl_clip_adam_step'):
         assert name in _capi.SYMBOLS
     names = ['HRL_DIAG_' + k.upper() for k in _capi.DIAG_KEYS]
     src = ('#include <stdio.h>\n#include "hrl_b200.h"\nint main(){' + ''.join('printf("%%d\\n", (int)%s);' % n for n in names) +

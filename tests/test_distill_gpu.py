@@ -236,7 +236,7 @@ def test_zero_coefficient_is_the_step_without_the_key(which, tmp_path):
     make, batch_fn, args = _nets()[which]
     off, out_off = _run(make, batch_fn, args)
     on, out_on = _run(make, batch_fn, dict(args, distill={'teacher': _teacher_file(tmp_path, make), 'coef': 0.0}))
-    assert off.distill_col is None and on.distill_col is not None
+    assert off.slots.distill is None and on.slots.distill is not None
     assert (off.engine is not None) == (on.engine is not None) == (which == 'boardnet')
     if which == 'torus':
         # two learners of this module-path net built alike with the key off already differ in the last bits from the second
@@ -328,7 +328,7 @@ def test_annealing_and_prioritised_weights(tmp_path):
     for n in range(6):
         stepper.step(stepper.new_packed().fill(batch_fn(n)))
         stepper.stream.synchronize()
-        kl, term = stepper.opt.extra_slots[stepper.distill_col:stepper.n_tail].tolist()
+        kl, term = stepper.opt.extra_slots[stepper.slots.distill].tolist()
         assert kl > 0
         assert term / kl == pytest.approx(2.0 * max(0.0, 1 - n / 4), rel=1e-6, abs=1e-7), n
     # the window weights of prioritised replay multiply the term: all weights 2 give twice the sums
@@ -352,8 +352,8 @@ def test_gradient_accumulation_sums_the_micro_batches(tmp_path):
     spec = {'teacher': _teacher_file(tmp_path, make), 'coef': 1.0}
     stepper, _ = _run(make, batch_fn, dict(args, distill=spec, gradient_accumulation=2), steps=1)
     stepper.stream.synchronize()
-    rows = stepper.loss_rows[:, stepper.distill_col:stepper.n_tail].double()
-    assert torch.allclose(stepper.opt.extra_slots[stepper.distill_col:stepper.n_tail].double(), rows.sum(0), rtol=1e-6)
+    rows = stepper.loss_rows[:, stepper.slots.distill].double()
+    assert torch.allclose(stepper.opt.extra_slots[stepper.slots.distill].double(), rows.sum(0), rtol=1e-6)
     assert (rows[:, 0] > 0).all()
     assert stepper.launches_per_step > 0
 

@@ -319,7 +319,7 @@ def test_diagnostics_sum_the_micro_batches_loss_passes():
     """The diagnostics sums of a step are those of the k loss passes; the last one is recomputed from the fused tower's
     outputs of the last micro-batch (static buffers) by ops.loss_fwd_bwd(..., diagnostics=True)."""
     from handyrl_b200 import ops
-    from handyrl_b200._capi import NUM_LOSS, NUM_LOSS_DIAG
+    from handyrl_b200._capi import NUM_LOSS_DIAG
     from handyrl_b200.nets import tictactoe_net
     from handyrl_b200.synthetic import synthetic_batch
     from handyrl_b200.train import LearnerStep
@@ -331,8 +331,9 @@ def test_diagnostics_sum_the_micro_batches_loss_passes():
     stepper.pop_diagnostics()
     stepper.step(stepper.new_packed().fill(batch))
     diag = stepper.pop_diagnostics()
+    loss_pass_diag = slice(stepper.slots.diag.start, stepper.slots.diag.start + NUM_LOSS_DIAG)
     rows = stepper.loss_rows.double().cpu()
-    want = rows[:, NUM_LOSS:NUM_LOSS + NUM_LOSS_DIAG].sum(0)
+    want = rows[:, loss_pass_diag].sum(0)
     got = torch.tensor([diag[key] for key in list(diag)[:NUM_LOSS_DIAG]], dtype=torch.float64)
     torch.testing.assert_close(got, want, rtol=1e-6, atol=1e-6)
     assert diag['steps'] == 1.0
@@ -342,8 +343,8 @@ def test_diagnostics_sum_the_micro_batches_loss_passes():
         outs = {'policy': eng.policy.view(B, T, Pa, -1), 'value': eng.value.view(B, T, Pa, 1)}
         buf = ops.loss_fwd_bwd(outs, stepper._micro[-1], args, diagnostics=True)
         torch.cuda.current_stream().synchronize()
-    assert torch.equal(buf.losses.cpu(), stepper.loss_rows[-1, :NUM_LOSS].cpu())
-    assert torch.equal(buf.diagnostics[:NUM_LOSS_DIAG].cpu(), stepper.loss_rows[-1, NUM_LOSS:NUM_LOSS + NUM_LOSS_DIAG].cpu())
+    assert torch.equal(buf.losses.cpu(), stepper.loss_rows[-1, stepper.slots.loss].cpu())
+    assert torch.equal(buf.diagnostics[:NUM_LOSS_DIAG].cpu(), stepper.loss_rows[-1, loss_pass_diag].cpu())
 
 
 def test_prioritised_replay_stores_each_windows_own_priority():
@@ -380,7 +381,7 @@ def test_prioritised_replay_stores_each_windows_own_priority():
         buf = ops.loss_fwd_bwd(outs, mb, args, taps=True, window_weight=ps.win_weight[-Bm:])
         torch.cuda.current_stream().synchronize()
     assert torch.equal(buf.taps['advantage'].cpu(), stepper.advantage[-Bm:].cpu())
-    assert torch.equal(buf.losses.cpu(), stepper.loss_rows[-1, :6].cpu())
+    assert torch.equal(buf.losses.cpu(), stepper.loss_rows[-1, stepper.slots.loss].cpu())
 
 
 def test_validation_runs_in_micro_batches_and_leaves_the_learner_as_it_was():

@@ -1,7 +1,7 @@
-"""Guard against non-finite optimiser steps on the GPU: hrl_clip_adam_step_guarded, hrl_step_commit and hrl_weight_ema_guarded
-against the unguarded kernels and ATen, in eager launches and CUDA graphs; and a learner that meets a batch with a NaN in it is
-left bit for bit as if that batch had never been drawn (fused tower, module path, recurrent net; graph and eager; the epoch
-hand-off, the Trainer, sharded ranks).  NaN and Inf only ever enter as data values."""
+"""Guard against non-finite optimiser steps on the GPU: hrl_clip_adam_step, hrl_step_commit and hrl_weight_ema given a skip
+flag against the same entry points without one and ATen, in eager launches and CUDA graphs; and a learner that meets a batch
+with a NaN in it is left bit for bit as if that batch had never been drawn (fused tower, module path, recurrent net; graph and
+eager; the epoch hand-off, the Trainer, sharded ranks).  NaN and Inf only ever enter as data values."""
 import bz2
 import copy
 import os
@@ -43,7 +43,8 @@ def _clone(b):
 
 
 def _optimise(b, form, diag=False, n_tail=6):
-    """hrl_grad_sumsq + one of the three step forms on bucket b, in place, on the current stream."""
+    """hrl_grad_sumsq + hrl_clip_adam_step in one of its three forms on bucket b, in place, on the current stream: guarded
+    (a skip flag and the first n_tail tail words, with or without diag), diag, or plain."""
     from handyrl_b200 import ops
     from handyrl_b200._capi import check, lib
     n = b['param'].numel()
@@ -52,12 +53,11 @@ def _optimise(b, form, diag=False, n_tail=6):
     p = ops._ptr
     check(lib().hrl_grad_sumsq(p(b['grad']), n, p(partials), s))
     fixed = (p(b['param']), p(b['grad']), p(b['m']), p(b['v']), n, p(partials), p(b['lr']), p(b['step'])) + HP + (p(b['gnorm']),)
+    diag_accum = p(b['diag']) if diag else None
     if form == 'guarded':
-        check(lib().hrl_clip_adam_step_guarded(*fixed, p(b['grad'][n:]), n_tail, p(b['diag']) if diag else None, p(b['skip']), s))
-    elif diag:
-        check(lib().hrl_clip_adam_step_diag(*fixed, p(b['diag']), s))
+        check(lib().hrl_clip_adam_step(*fixed, diag_accum, p(b['grad'][n:]), n_tail, p(b['skip']), s))
     else:
-        check(lib().hrl_clip_adam_step(*fixed, s))
+        check(lib().hrl_clip_adam_step(*fixed, diag_accum, None, 0, None, s))
 
 
 def _assert_same(a, b, keys=('param', 'm', 'v', 'step', 'gnorm', 'diag'), what=''):

@@ -178,7 +178,7 @@ def test_binding_mirrors_the_header():
     assert 'hrl_gather_pad_sym' in _capi.SYMBOLS
     assert re.search(r'#define HRL_SYM_MAX_TRANSFORMS 64\b', header) and symmetry.MAX_TRANSFORMS == 64
     assert re.search(r'int hrl_gather_pad_sym\(const HrlGatherArgs \*args,', header)
-    assert _capi.HRL_ABI_VERSION == 2 and '#define HRL_ABI_VERSION 2' in header
+    assert _capi.HRL_ABI_VERSION == 3 and '#define HRL_ABI_VERSION 3' in header
 
 
 def test_sampler_draws_the_same_windows_with_the_key_on():

@@ -288,9 +288,9 @@ def _heads(pre, ld, M, cells, maps, A, W, slope, dout, acc, grads):
     dpre = torch.full((M, ld), -3.0, device='cuda')
     ws = torch.empty(lib().hrl_heads_num_blocks(M) * sum(t.numel() for t in grads.values()), device='cuda')
     g = lambda k: _ptr(grads.get(k))
-    check(lib().hrl_heads_bwd_accumulate(_ptr(pre), ld, M, cells, pm, vm, rm, A, slope, _ptr(W['p']), _ptr(W.get('v')), _ptr(W.get('r')),
-                                         _ptr(value), _ptr(dout['p']), _ptr(dout.get('v')), _ptr(dout.get('r')), _ptr(dpre),
-                                         g('wp'), g('wv'), g('wr'), g('bp'), g('bv'), g('br'), _ptr(ws), int(acc), _stream_ptr()))
+    check(lib().hrl_heads_bwd(_ptr(pre), ld, M, cells, pm, vm, rm, A, slope, _ptr(W['p']), _ptr(W.get('v')), _ptr(W.get('r')),
+                              _ptr(value), _ptr(dout['p']), _ptr(dout.get('v')), _ptr(dout.get('r')), _ptr(dpre),
+                              g('wp'), g('wv'), g('wr'), g('bp'), g('bv'), g('br'), _ptr(ws), int(acc), _stream_ptr()))
     torch.cuda.synchronize()
     return policy, value, ret, dpre
 
@@ -298,7 +298,7 @@ def _heads(pre, ld, M, cells, maps, A, W, slope, dout, acc, grads):
 @pytest.mark.parametrize('M', [1, 127, 128, 129])
 @pytest.mark.parametrize('maps,A', [((4, 0, 0), 32), ((2, 1, 1), 32), ((2, 1, 0), 9)])
 def test_heads_kernels_against_float64(maps, A, M):
-    """hrl_heads_fwd and hrl_heads_bwd_accumulate over 16 cells: LeakyReLU(0.1), the bias-free Linear heads and tanh, and their
+    """hrl_heads_fwd and hrl_heads_bwd over 16 cells: LeakyReLU(0.1), the bias-free Linear heads and tanh, and their
     gradients, with exact zeros in the squeeze outputs and NaN in the padding columns of `pre` (ld > NH)."""
     cells, slope = 16, 0.1
     pm, vm, rm = maps

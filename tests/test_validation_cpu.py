@@ -120,7 +120,7 @@ def test_binding_mirrors_the_header():
     assert _capi.SYMBOLS['hrl_loss_fwd'] == _capi.SYMBOLS['hrl_loss_fwd_bwd']
     header = open(os.path.join(ROOT, 'include', 'hrl_b200.h')).read()
     assert re.search(r'\bint hrl_loss_fwd\(const HrlLossArgs \*args, void \*stream\);', header)
-    assert _capi.HRL_ABI_VERSION == 2 and '#define HRL_ABI_VERSION 2' in header
+    assert _capi.HRL_ABI_VERSION == 3 and '#define HRL_ABI_VERSION 3' in header
 
 
 def test_loss_fwd_refuses_cpu_tensors():

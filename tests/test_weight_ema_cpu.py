@@ -20,11 +20,11 @@ def test_header_declares_and_binding_mirrors_hrl_weight_ema():
     C = ctypes
     text = re.sub(r'\s+', ' ', re.sub(r'/\*.*?\*/', '', open(os.path.join(ROOT, 'include', 'hrl_b200.h')).read(), flags=re.S))
     assert ('int hrl_weight_ema(float *avg, const float *state, int64_t n, const int64_t *step, float decay, int32_t seeded, '
-            'void *stream);') in text
-    assert _capi.HRL_ABI_VERSION == 2
+            'const int32_t *skip , void *stream);') in text
+    assert _capi.HRL_ABI_VERSION == 3
     res, argt = _capi.SYMBOLS['hrl_weight_ema']
     assert res is C.c_int
-    assert argt == [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_int32, C.c_void_p]
+    assert argt == [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_int32, C.c_void_p, C.c_void_p]
 
 
 def test_library_exports_hrl_weight_ema_and_refuses_bad_arguments():
@@ -35,8 +35,8 @@ def test_library_exports_hrl_weight_ema_and_refuses_bad_arguments():
 
     def refused():      # argument checks fail before anything touches a device
         buf, step = (ctypes.c_float * 8)(), (ctypes.c_int64 * 1)()
-        got.append((lib().hrl_weight_ema(None, None, 4, None, 0.9, 0, None), lib().hrl_last_error()))
-        got.append((lib().hrl_weight_ema(buf, buf, 4, step, 1.0, 0, None), lib().hrl_last_error()))
+        got.append((lib().hrl_weight_ema(None, None, 4, None, 0.9, 0, None, None), lib().hrl_last_error()))
+        got.append((lib().hrl_weight_ema(buf, buf, 4, step, 1.0, 0, None, None), lib().hrl_last_error()))
 
     th = threading.Thread(target=refused)         # the error text is per thread: keep this one's clean
     th.start()
