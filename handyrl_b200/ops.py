@@ -9,7 +9,7 @@ import ctypes as C
 import torch
 
 from . import _capi
-from ._capi import ALGO_ID, DIAG_KEYS, LOSS_KEYS, NUM_DIAG, NUM_LOSS, HrlLossArgs, check, lib
+from ._capi import ALGO_ID, DIAG_KEYS, GEMM_EPILOGUES, LOSS_KEYS, NUM_DIAG, NUM_LOSS, HrlLossArgs, check, lib
 
 # kernels of THIS library launched through the wrappers below (bench.py reports them as `gpu_launches`; a CUDA graph
 # replays the launches counted while it was captured)
@@ -548,56 +548,100 @@ def priority_update(state, advantage, turn_mask, burn_in, skip=None):
     _count()
 
 
-def gemm_tf32x3(a, b, bias=None, a_kmajor=True, b_kmajor=True, splits=1, out=None):
-    """C = A_op @ B_op^T (+ bias) on the tensor cores with fp32-class accuracy (hrl_gemm_tf32x3, csrc/gemm_kernel.cu).
+# K slices of a product: one CTA computes one output tile (_TILE_ROWS x _TILE_COLS) over one K slice, and a product is split over
+# as many slices as keep the _SMS SMs of an H100 busy, with at least _MIN_SLICE_K elements of K per slice
+_TILE_ROWS, _TILE_COLS, _SMS, _MIN_SLICE_K = 128, 288, 132, 64
 
-    a: (M, K) if a_kmajor else (K, M) -- the operand as it lies in memory; b likewise (N, K) / (K, N).
-    """
+
+def k_splits(rows, cols, K, segments=1):
+    """K slices for a product of rows x cols outputs reducing over K (each of `segments` pairs of a segmented product getting its
+    own), counted as the library produces them (hrl_gemm_effective_splits: whole 32-element chunks, no empty slice)."""
+    tiles = -(-rows // _TILE_ROWS) * -(-cols // _TILE_COLS)
+    return lib().hrl_gemm_effective_splits(K, max(1, min(K // _MIN_SLICE_K, _SMS // (tiles * segments))))
+
+
+def _operand(o, t, t2=None, consts=None, relu=False, kmajor=True, by_row=False, packed=False):
+    o.ptr, o.ptr2 = _ptr(t), _ptr(t2)
+    o.ld = 0 if packed else t.stride(0)
+    o.kmajor, o.relu, o.feature_is_row, o.packed = int(kmajor), int(relu), int(by_row), int(packed)
+    if consts is not None:
+        o.p, o.r = _ptr(consts[0]), _ptr(consts[-1])
+        o.q = _ptr(consts[1]) if len(consts) == 3 else None
+
+
+def gemm_fused(a, b, M, N, K, out=None, ws=None, splits=1, bias=None, epilogue='store', ep=None, col_partials=None, bf16=False,
+               conv=None, ones_row=False, segments=None):
+    """One hrl_gemm_fused launch (csrc/gemm_kernel.cu): C[M x N] = A_op @ B_op^T with the operands' transforms and the epilogue.
+
+    a, b: keyword arguments of _operand (the tensor `t` and its layout / transform).  out: C, or None to leave the product in
+    `ws` as its K-slice partials, M*N floats apart (one slice: the product itself).  ws: the workspace of a split or segmented
+    product (hrl_gemm_workspace_floats floats).  ep: the epilogue's tensors by name (y, scale, shift, mean, rstd).
+    conv: (conv_mode, neighbour table, cells, taps, channels) of an implicit convolution product; ones_row: its bias-gradient
+    column.  segments: the (dy, x) pairs of a segmented weight gradient.
+    Counts the launch, and the library's sum of the slice partials into `out`."""
+    g = _capi.HrlGemmArgs()
+    _operand(g.a, **a)
+    _operand(g.b, **b)
+    g.M, g.N, g.K, g.splits, g.bf16 = M, N, K, splits, int(bf16)
+    g.bias, g.epilogue, g.col_partials = _ptr(bias), GEMM_EPILOGUES[epilogue], _ptr(col_partials)
+    split = splits > 1 or segments is not None
+    if out is not None:
+        g.C, g.ldc = _ptr(out), out.stride(0)
+    else:
+        g.C, g.ldc = (None if split else _ptr(ws)), N
+    g.workspace = _ptr(ws) if split else None
+    if ep is not None:
+        if 'y' in ep:
+            g.ep_y, g.ep_ldy = _ptr(ep['y']), ep['y'].stride(0)
+        g.ep_scale, g.ep_shift = _ptr(ep.get('scale')), _ptr(ep.get('shift'))
+        g.ep_mean, g.ep_rstd = _ptr(ep.get('mean')), _ptr(ep.get('rstd'))
+    if conv is not None:
+        g.conv_mode, g.conv_off, g.conv_hw, g.conv_taps, g.conv_cin = conv[0], _ptr(conv[1]), *conv[2:]
+        g.conv_ones_row = int(ones_row)
+    if segments is not None:
+        seg_a = (C.c_void_p * len(segments))(*[dy.data_ptr() for dy, _ in segments])
+        seg_b = (C.c_void_p * len(segments))(*[x.data_ptr() for _, x in segments])
+        g.seg_a, g.seg_b, g.segments = C.cast(seg_a, C.c_void_p), C.cast(seg_b, C.c_void_p), len(segments)
+    check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
+    _count(2 if out is not None and splits > 1 and lib().hrl_gemm_effective_splits(K, splits) > 1 else 1)
+
+
+def _gemm_dense(a, b, bias, a_kmajor, b_kmajor, splits, out, partials, bf16):
     assert a.is_cuda and b.is_cuda and a.dtype == torch.float32 and b.dtype == torch.float32
     assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
     M, K = (a.shape[0], a.shape[1]) if a_kmajor else (a.shape[1], a.shape[0])
     N, Kb = (b.shape[0], b.shape[1]) if b_kmajor else (b.shape[1], b.shape[0])
     assert K == Kb, (a.shape, b.shape, a_kmajor, b_kmajor)
-    if out is None:
-        out = torch.empty((M, N), dtype=torch.float32, device=a.device)
-    ws = None
-    if splits > 1:
-        ws = torch.empty(lib().hrl_gemm_workspace_floats(M, N, K, splits), dtype=torch.float32, device=a.device)
-    check(lib().hrl_gemm_tf32x3(_ptr(a), a.stride(0), int(a_kmajor), _ptr(b), b.stride(0), int(b_kmajor), _ptr(bias), _ptr(out),
-                                out.stride(0), M, N, K, splits, _ptr(ws), _stream_ptr()))
-    _count(2 if splits > 1 else 1)
+    ws = partials
+    if partials is not None:
+        out = None
+    else:
+        if out is None:
+            out = torch.empty((M, N), dtype=torch.float32, device=a.device)
+        if splits > 1:
+            ws = torch.empty(lib().hrl_gemm_workspace_floats(M, N, K, splits), dtype=torch.float32, device=a.device)
+    gemm_fused(dict(t=a, kmajor=a_kmajor), dict(t=b, kmajor=b_kmajor), M, N, K, out=out, ws=ws, splits=splits, bias=bias, bf16=bf16)
     return out
+
+
+def gemm_tf32x3(a, b, bias=None, a_kmajor=True, b_kmajor=True, splits=1, out=None):
+    """C = A_op @ B_op^T (+ bias) on the tensor cores with fp32-class accuracy (3xTF32, hrl_gemm_fused).
+
+    a: (M, K) if a_kmajor else (K, M) -- the operand as it lies in memory; b likewise (N, K) / (K, N).
+    """
+    return _gemm_dense(a, b, bias, a_kmajor, b_kmajor, splits, out, None, False)
 
 
 def gemm_bf16(a, b, bias=None, a_kmajor=True, b_kmajor=True, splits=1, out=None, partials=None):
     """C = A_op @ B_op^T on the tensor cores with bf16 operands (hrl_gemm_fused with HrlGemmArgs.bf16): both operands rounded to
     the nearest bf16, products accumulated in fp32.  Layouts as gemm_tf32x3.  partials: a workspace of
     hrl_gemm_workspace_floats floats that receives the K-slice partials instead of C (no sum, nothing returned)."""
-    assert a.is_cuda and b.is_cuda and a.dtype == torch.float32 and b.dtype == torch.float32
-    assert a.dim() == 2 and b.dim() == 2 and a.stride(1) == 1 and b.stride(1) == 1
-    M, K = (a.shape[0], a.shape[1]) if a_kmajor else (a.shape[1], a.shape[0])
-    N, Kb = (b.shape[0], b.shape[1]) if b_kmajor else (b.shape[1], b.shape[0])
-    assert K == Kb, (a.shape, b.shape, a_kmajor, b_kmajor)
-    g = _capi.HrlGemmArgs()
-    g.a.ptr, g.a.ld, g.a.kmajor = _ptr(a), a.stride(0), int(a_kmajor)
-    g.b.ptr, g.b.ld, g.b.kmajor = _ptr(b), b.stride(0), int(b_kmajor)
-    g.M, g.N, g.K, g.splits, g.bf16 = M, N, K, splits, 1
-    g.bias = _ptr(bias)
-    if partials is not None:
-        g.C, g.ldc, g.workspace = None, N, _ptr(partials)
-    else:
-        if out is None:
-            out = torch.empty((M, N), dtype=torch.float32, device=a.device)
-        ws = torch.empty(lib().hrl_gemm_workspace_floats(M, N, K, splits), dtype=torch.float32, device=a.device) if splits > 1 else None
-        g.C, g.ldc, g.workspace = _ptr(out), out.stride(0), _ptr(ws)
-    check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
-    _count(2 if (splits > 1 and partials is None) else 1)
-    return out
+    return _gemm_dense(a, b, bias, a_kmajor, b_kmajor, splits, out, partials, True)
 
 
 class _LinearTC(torch.autograd.Function):
     """y = x @ w^T with all three products (forward, input gradient, weight gradient) on the tensor cores at fp32-class
-    accuracy (hrl_gemm_tf32x3).  The weight gradient reduces over the rows of x (samples): both operands are read
+    accuracy (gemm_tf32x3).  The weight gradient reduces over the rows of x (samples): both operands are read
     transposed on the fly and the reduction is split over enough K slices to fill the GPU."""
 
     @staticmethod
@@ -614,10 +658,7 @@ class _LinearTC(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             dx = gemm_tf32x3(dy, w, b_kmajor=False)                       # (M,N) x (N,K): w is read as stored
         if ctx.needs_input_grad[1]:
-            M = x.shape[0]
-            tiles = ((w.shape[0] + 127) // 128) * ((w.shape[1] + 287) // 288)
-            splits = max(1, min(M // 64, 132 // tiles))
-            dw = gemm_tf32x3(dy, x, a_kmajor=False, b_kmajor=False, splits=splits)
+            dw = gemm_tf32x3(dy, x, a_kmajor=False, b_kmajor=False, splits=k_splits(w.shape[0], w.shape[1], x.shape[0]))
         return dx, dw
 
 
@@ -654,11 +695,11 @@ def board_dense(weight, H, W):
 
 class _BoardConv(torch.autograd.Function):
     """A stride-1 "same" convolution over a tiny board, NCHW in and out, as dense products on the tensor cores:
-    forward   y = x2d @ dense(w)^T            (hrl_board_expand + hrl_gemm_tf32x3)
-    backward  dx = dy2d @ dense(w)            (hrl_gemm_tf32x3, the dense matrix read as stored)
-              dw = fold(sum_s dy2d_s^T x2d_s) (split-K hrl_gemm_tf32x3 leaving its slice partials, folded AND summed by
+    forward   y = x2d @ dense(w)^T            (hrl_board_expand + hrl_gemm_fused)
+    backward  dx = dy2d @ dense(w)            (hrl_gemm_fused, the dense matrix read as stored)
+              dw = fold(sum_s dy2d_s^T x2d_s) (split-K hrl_gemm_fused leaving its slice partials, folded AND summed by
                                                one hrl_board_fold launch: no dense gradient is ever materialised)
-    bf16: the same three products as hrl_gemm_fused on bf16 operands (gemm_bf16); the dense matrix and the fold stay fp32."""
+    The products are 3xTF32 (gemm_tf32x3), or with bf16 on bf16 operands (gemm_bf16); the dense matrix and the fold stay fp32."""
 
     @staticmethod
     def forward(ctx, x, weight, bf16=False):
@@ -687,22 +728,12 @@ class _BoardConv(torch.autograd.Function):
             dx = gemm(dy2, dense, b_kmajor=False).view(N, Cin, H, W)
         if ctx.needs_input_grad[1]:
             rows, cols = Cout * H * W, Cin * H * W
-            tiles = ((rows + 127) // 128) * ((cols + 287) // 288)
-            splits = lib().hrl_gemm_effective_splits(N, max(1, min(N // 64, 132 // tiles)))
+            splits = k_splits(rows, cols, N)
             dw = torch.empty((Cout, Cin, kh, kw), dtype=torch.float32, device=dy.device)
-            if splits > 1 and ctx.bf16:
-                ws = torch.empty(splits * rows * cols, dtype=torch.float32, device=dy.device)
-                gemm_bf16(dy2, x2, a_kmajor=False, b_kmajor=False, splits=splits, partials=ws)
-                _count(-1)
-            elif splits > 1:
-                ws = torch.empty(splits * rows * cols, dtype=torch.float32, device=dy.device)
-                check(lib().hrl_gemm_tf32x3(_ptr(dy2), dy2.stride(0), 0, _ptr(x2), x2.stride(0), 0, None, None, cols, rows, cols, N,
-                                            splits, _ptr(ws), _stream_ptr()))
-            else:
-                ws = gemm(dy2, x2, a_kmajor=False, b_kmajor=False).view(-1)
-                _count(-1)
+            ws = torch.empty(splits * rows * cols, dtype=torch.float32, device=dy.device)
+            gemm_fused(dict(t=dy2, kmajor=False), dict(t=x2, kmajor=False), rows, cols, N, ws=ws, splits=splits, bf16=ctx.bf16)
             check(lib().hrl_board_fold(_ptr(ws), splits, rows * cols, _ptr(dw), Cout, Cin, kh, kw, H, W, _stream_ptr()))
-            _count(2)
+            _count()
         return dx, dw, None
 
 
@@ -775,15 +806,8 @@ def _conv_product(pix, image, rows, cin, taps, table, hw, bias=None, bf16=False)
     """out[pixel][row] = sum over (tap, channel) of pix[neighbour(pixel, tap)][channel] * image[row][tap, channel]"""
     M = pix.shape[0]
     out = torch.empty((M, rows), dtype=torch.float32, device=pix.device)
-    g = _capi.HrlGemmArgs()
-    g.a.ptr, g.a.ld, g.a.kmajor = _ptr(pix), pix.stride(0), 1
-    g.b.ptr, g.b.kmajor, g.b.packed = _ptr(image), 1, 1
-    g.bias, g.C, g.ldc = _ptr(bias), _ptr(out), rows
-    g.M, g.N, g.K, g.splits = M, rows, taps * ((cin + 31) // 32 * 32), 1
-    g.conv_off, g.conv_mode, g.conv_hw, g.conv_taps, g.conv_cin = _ptr(table), 1, hw, taps, cin
-    g.bf16 = int(bf16)
-    check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
-    _count()
+    gemm_fused(dict(t=pix), dict(t=image, packed=True), M, rows, taps * ((cin + 31) // 32 * 32), out=out, bias=bias,
+               conv=(1, table, hw, taps, cin), bf16=bf16)
     return out
 
 
@@ -816,45 +840,29 @@ def _flush_weight_gradient(job):
     taps, (table, hw) = kh * kw, job['geom']
     # the ones row (bias gradient as one more column) is free unless that column opens a new 288-wide tile AND the extra tile's CTAs
     # take K slices away from the others (a weight used once: 1 tile x 132 slices vs 2 tiles x 66): then a column sum does it
-    cols, pixels0 = taps * Cin, pairs[0][0].shape[0]
+    cols, pixels = taps * Cin, pairs[0][0].shape[0]
     n0 = min(len(pairs), 64)
-
-    def slices(ncols_):
-        t_ = ((Cout + 127) // 128) * ((ncols_ + 287) // 288)
-        return lib().hrl_gemm_effective_splits(pixels0, max(1, min(pixels0 // 64, 132 // (t_ * n0))))
-    ones = b is not None and slices(cols + 1) >= slices(cols)
+    ones = b is not None and k_splits(Cout, cols + 1, pixels, n0) >= k_splits(Cout, cols, pixels, n0)
     if b is not None and not ones:
         if b.grad is None:
             b.grad = torch.zeros_like(b)
         for dy2, _ in pairs:
             b.grad.add_(dy2.sum(0))
     ncols = cols + (1 if ones else 0)
-    pixels = pairs[0][0].shape[0]
-    tiles = ((Cout + 127) // 128) * ((ncols + 287) // 288)
     for start in range(0, len(pairs), 64):
         chunk = pairs[start:start + 64]
         n = len(chunk)
-        per = lib().hrl_gemm_effective_splits(pixels, max(1, min(pixels // 64, 132 // (tiles * n))))
+        per = k_splits(Cout, ncols, pixels, n)
         ws = torch.empty((n * per, Cout, ncols), dtype=torch.float32, device=w.device)
-        seg_a = (C.c_void_p * n)(*[dy2.data_ptr() for dy2, _ in chunk])
-        seg_b = (C.c_void_p * n)(*[x2.data_ptr() for _, x2 in chunk])
-        g = _capi.HrlGemmArgs()
-        g.a.ptr, g.a.ld, g.a.kmajor = _ptr(chunk[0][0]), Cout, 0
-        g.b.ptr, g.b.ld, g.b.kmajor = _ptr(chunk[0][1]), Cin, 0
-        g.C, g.ldc = None, ncols
-        g.M, g.N, g.K, g.splits, g.workspace = Cout, ncols, pixels, per, _ptr(ws)
-        g.conv_off, g.conv_mode, g.conv_hw, g.conv_taps, g.conv_cin = _ptr(table), 2, hw, taps, Cin
-        g.seg_a, g.seg_b = C.cast(seg_a, C.c_void_p), C.cast(seg_b, C.c_void_p)
-        g.segments, g.conv_ones_row = n, int(ones)
-        g.bf16 = int(job['bf16'])
-        check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
+        gemm_fused(dict(t=chunk[0][0], kmajor=False), dict(t=chunk[0][1], kmajor=False), Cout, ncols, pixels, ws=ws, splits=per,
+                   conv=(2, table, hw, taps, Cin), ones_row=ones, segments=chunk, bf16=job['bf16'])
         for t, shape in ((w, w.shape), (b, None)):
             if t is not None and t.grad is None:
                 t.grad = torch.zeros_like(t, memory_format=torch.contiguous_format)
         assert w.grad.is_contiguous()
         check(lib().hrl_conv_wgrad_reduce2(_ptr(ws), n * per, ncols, _ptr(w.grad), _ptr(b.grad) if ones else None, Cout, Cin, taps, 1,
                                            _stream_ptr()))
-        _count(2)
+        _count()
 
 
 class _ConvImplicit(torch.autograd.Function):
@@ -896,20 +904,13 @@ class _ConvImplicit(torch.autograd.Function):
         if ctx.needs_input_grad[1]:
             x2 = xl.permute(0, 2, 3, 1).reshape(-1, Cin)
             pixels, cols = x2.shape[0], taps * Cin
-            tiles = ((Cout + 127) // 128) * ((cols + 287) // 288)
-            s = lib().hrl_gemm_effective_splits(pixels, max(1, min(pixels // 64, 132 // tiles)))
+            s = k_splits(Cout, cols, pixels)
             ws = torch.empty((s, Cout, cols), dtype=torch.float32, device=xl.device)
-            g = _capi.HrlGemmArgs()
-            g.a.ptr, g.a.ld, g.a.kmajor = _ptr(dy2), Cout, 0
-            g.b.ptr, g.b.ld, g.b.kmajor = _ptr(x2), Cin, 0
-            g.C, g.ldc = (None if s > 1 else _ptr(ws)), cols
-            g.M, g.N, g.K, g.splits, g.workspace = Cout, cols, pixels, s, (_ptr(ws) if s > 1 else None)
-            g.conv_off, g.conv_mode, g.conv_hw, g.conv_taps, g.conv_cin = _ptr(table), 2, H * W, taps, Cin
-            g.bf16 = int(ctx.bf16)
-            check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
+            gemm_fused(dict(t=dy2, kmajor=False), dict(t=x2, kmajor=False), Cout, cols, pixels, ws=ws, splits=s,
+                       conv=(2, table, H * W, taps, Cin), bf16=ctx.bf16)
             dw = torch.empty_like(w, memory_format=torch.contiguous_format)
             check(lib().hrl_conv_wgrad_reduce(_ptr(ws), s, _ptr(dw), Cout, Cin, taps, _stream_ptr()))
-            _count(2)
+            _count()
         if ctx.has_bias and ctx.needs_input_grad[2]:
             db = dy2.sum(0)
         return dx, dw, db, None, None

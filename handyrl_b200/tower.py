@@ -26,17 +26,8 @@ import ctypes as C
 import torch
 
 from . import _capi, nets
-from ._capi import GEMM_EPILOGUES, MAX_BOARD_JOBS, MAX_BOARD_ROWS, HrlFoldJob, HrlGemmArgs, HrlPackJob, check, lib
-from .ops import _count, _ptr, _stream_ptr
-
-
-def _operand(o, t, t2=None, consts=None, relu=False, kmajor=True, by_row=False, packed=False):
-    o.ptr, o.ptr2 = _ptr(t), _ptr(t2)
-    o.ld = 0 if packed else t.stride(0)
-    o.kmajor, o.relu, o.feature_is_row, o.packed = int(kmajor), int(relu), int(by_row), int(packed)
-    if consts is not None:
-        o.p, o.r = _ptr(consts[0]), _ptr(consts[-1])
-        o.q = _ptr(consts[1]) if len(consts) == 3 else None
+from ._capi import MAX_BOARD_JOBS, MAX_BOARD_ROWS, HrlFoldJob, HrlPackJob, check, lib
+from .ops import _count, _operand, _ptr, _stream_ptr, gemm_fused, k_splits  # noqa: F401 (_operand: the operand dicts of _gemm)
 
 
 def supports(model):
@@ -116,9 +107,7 @@ class FusedBoardNet:
         self.splits, self.ws_at = {}, {}
         ws_floats = 0
         for name, rows, colsn, count in (('stem', D, self.K0, 1), ('tower', D, D, self.depth), ('heads', self.NH, D, 1)):
-            tiles = ((rows + 127) // 128) * ((colsn + 287) // 288)
-            s = lib().hrl_gemm_effective_splits(M_, max(1, min(M_ // 64, 132 // tiles)))
-            self.splits[name] = s
+            s = self.splits[name] = k_splits(rows, colsn, M_)
             for i in range(count):
                 self.ws_at[(name, i)] = ws_floats
                 ws_floats += s * rows * colsn
@@ -128,26 +117,9 @@ class FusedBoardNet:
 
     # ------------------------------------------------------------------ helpers
     def _gemm(self, a, b, out, K, N, M=None, bias=None, epilogue='store', splits=1, partial=False, ep=None, ws=None):
-        g = HrlGemmArgs()
-        _operand(g.a, **a)
-        _operand(g.b, **b)
-        g.bias = _ptr(bias)
-        g.C = None if partial else _ptr(out)
-        g.ldc = out.stride(0) if out is not None else N
-        g.M, g.N, g.K = (self.M if M is None else M), N, K
-        g.splits = splits
-        g.epilogue = GEMM_EPILOGUES[epilogue]
-        g.bf16 = int(self.bf16)
-        g.workspace = _ptr(ws) if splits > 1 else None
-        if epilogue in ('stats', 'mask_stats'):
-            g.col_partials = _ptr(self.cp)
-        if ep is not None:
-            if 'y' in ep:
-                g.ep_y, g.ep_ldy = _ptr(ep['y']), ep['y'].stride(0)
-            g.ep_scale, g.ep_shift = _ptr(ep.get('scale')), _ptr(ep.get('shift'))
-            g.ep_mean, g.ep_rstd = _ptr(ep.get('mean')), _ptr(ep.get('rstd'))
-        check(lib().hrl_gemm_fused(C.byref(g), _stream_ptr()))
-        _count(2 if (splits > 1 and not partial) else 1)
+        """partial: leave the product in `ws` as its K-slice partials (gemm_fused with no output)."""
+        gemm_fused(a, b, self.M if M is None else M, N, K, out=None if partial else out, ws=ws, splits=splits, bias=bias, epilogue=epilogue,
+                   ep=ep, col_partials=self.cp if epilogue in ('stats', 'mask_stats') else None, bf16=self.bf16)
 
     def _pack_all(self, jobs):
         """jobs: dicts of HrlPackJob fields with tensors for the pointers -- one launch for up to MAX_BOARD_JOBS convolutions.
@@ -193,14 +165,9 @@ class FusedBoardNet:
         workspace region; queued for the fold onto the conv weights.  grads: list of (weight.grad tensor, first dense row)."""
         s = self.splits[region[0]]
         ws = self.ws[self.ws_at[region]:]
-        if s > 1:
-            self._gemm(a, b, None, K=self.M, N=cols, M=rows, splits=s, partial=True, ws=ws)
-            stride = rows * cols
-        else:
-            self._gemm(a, b, ws[:rows * cols].view(rows, cols), K=self.M, N=cols, M=rows)
-            stride = 0
+        self._gemm(a, b, None, K=self.M, N=cols, M=rows, splits=s, partial=True, ws=ws)
         for grad, row0 in grads:
-            self.fold_jobs.append((ws[row0 * cols:], s, stride, grad))
+            self.fold_jobs.append((ws[row0 * cols:], s, rows * cols if s > 1 else 0, grad))
 
     # ------------------------------------------------------------------ forward
     def forward(self, x):

@@ -139,7 +139,7 @@ def clip_adam(param, grad, m, v, lr, step, max_norm=4.0, b1=0.9, b2=0.999, eps=1
 def board_conv(x, w, b=None):
     """Reference of a stride-1 "same" convolution over a small board (what torch.nn.functional.conv2d computes inside the
     user's net, reference envs/tictactoe.py:20-31): plain float64 loops over taps, NCHW.  Checker of the tensor-core dense
-    path (hrl_board_expand + hrl_gemm_tf32x3) in __graft_entry__.smoke() and the tests."""
+    path (hrl_board_expand + hrl_gemm_fused) in __graft_entry__.smoke() and the tests."""
     x = np.asarray(x, np.float64)
     w = np.asarray(w, np.float64)
     N, Cin, H, W = x.shape

@@ -39,15 +39,14 @@ def gpu_name_and_power():
 def tower_products(rounds):
     """the forward / input-gradient / weight-gradient products of one cfg2 tower layer, 3xTF32 and bf16"""
     from handyrl_b200._capi import HrlGemmArgs, HrlPackJob, check, lib
-    from handyrl_b200.ops import _ptr
+    from handyrl_b200.ops import _ptr, k_splits
     M, D, C_, H = 16384, 288, 32, 3
     g = torch.Generator(device='cuda').manual_seed(1)
     w = torch.randn(C_, C_, 3, 3, device='cuda', generator=g) * 0.1
     x = torch.randn(M, D, device='cuda', generator=g)
     dy = torch.randn(M, D, device='cuda', generator=g)
     out = torch.empty(M, D, device='cuda')
-    tiles = (D + 127) // 128
-    splits = lib().hrl_gemm_effective_splits(M, max(1, min(M // 64, 132 // tiles)))
+    splits = k_splits(D, D, M)
     ws = torch.empty(splits * D * D, device='cuda')
     stream = torch.cuda.Stream()
     images, calls = {}, {}

@@ -1,4 +1,4 @@
-"""Time hrl_gemm_tf32x3 at the shapes of the TicTacToe tower (CUDA events, back to back, L2-warm) vs cuBLAS fp32."""
+"""Time ops.gemm_tf32x3 (3xTF32 hrl_gemm_fused) at the shapes of the TicTacToe tower (CUDA events, back to back, L2-warm) vs cuBLAS fp32."""
 import ctypes, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

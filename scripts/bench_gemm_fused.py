@@ -49,7 +49,7 @@ cases = {
     'wgrad plain (48 slices, partials)': lambda: eng._gemm(dict(t=X, kmajor=False), dict(t=Y, kmajor=False), None, K=M, N=D, M=D, splits=eng.splits['tower'], partial=True, ws=eng.ws),
     'wgrad both transformed': lambda: eng._gemm(dict(t=X, t2=Y, consts=(c[0], c[1], c[2]), kmajor=False, by_row=True),
                                                 dict(t=Y, consts=(c[3], c[4]), relu=True, kmajor=False, by_row=True), None, K=M, N=D, M=D,
-                                                splits=eng.splits['tower'], partial=True),
+                                                splits=eng.splits['tower'], partial=True, ws=eng.ws),
 }
 for k, fn in (cases.items() if __name__ == "__main__" else ()):
     print('%-40s %6.1f us' % (k, timeit(fn)))

@@ -357,7 +357,6 @@ def test_board_conv_bf16_against_float64(N):
     """ops.board_conv in bf16 mode (the dense small-board convolution of fastnet, TicTacToe-sized boards): forward, input
     gradient, and the weight gradient as one product (N = 100) or as split-K slice partials folded by hrl_board_fold."""
     from handyrl_b200 import ops
-    from handyrl_b200._capi import lib
     g = torch.Generator(device='cuda').manual_seed(N)
     Cin, Cout, H, W = 32, 32, 3, 3
     x = torch.randn(N, Cin, H, W, device='cuda', generator=g).requires_grad_(True)
@@ -370,7 +369,7 @@ def test_board_conv_bf16_against_float64(N):
     D = Cin * H * W
     _close(y, _conv(xr, wr), accum_bound(D) * _conv(xr.abs(), wr.abs()), 'y')
     _close(x.grad, _conv_in(x.shape, wr, dyr), accum_bound(D) * _conv_in(x.shape, wr.abs(), dyr.abs()), 'dx')
-    splits = lib().hrl_gemm_effective_splits(N, max(1, min(N // 64, 132 // 3)))
+    splits = ops.k_splits(Cout * H * W, Cin * H * W, N)
     assert (splits > 1) == (N > 1000)
     _close(w.grad, _conv_w(xr, w.shape, dyr), _wgrad_bound(N, splits, H * W) * _conv_w(xr.abs(), w.shape, dyr.abs()), 'dw')
     # rounding happened: against the unrounded operands the forward leaves its bound
