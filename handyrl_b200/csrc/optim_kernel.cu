@@ -100,6 +100,120 @@ __global__ void __launch_bounds__(kOptThreads) clip_adam_kernel(
     }
 }
 
+// ---- LAMB (You et al., 2020, Algorithm 2) on the same bucket: Adam's moments, one trust ratio per parameter tensor --------
+// The bucket is cut into chunks of at most kLambChunk words that never cross a tensor (hrl_lamb_plan); block c of both
+// launches owns chunk c.  Launch A updates the moments, writes the update direction u to a scratch bucket and the chunk's
+// fp64 sums of w^2 and u^2; launch B folds the sums of its tensor's chunks in a fixed order (so every block of a tensor, every
+// replay and every rank gets the same ratio) and applies w -= lr * lr_scale * r * u.
+constexpr int kLambChunk = 1024;   // words per chunk: 4 per thread of a kOptThreads block
+constexpr int kLambPlanWords = 5;  // int64 per chunk: start, length, tensor, that tensor's first chunk and chunk count
+
+__device__ __forceinline__ double block_sum_d(double x, double *red) {   // fixed order; red: kOptThreads / 32 doubles
+    x = warp_sum_d(x);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = x;
+    __syncthreads();
+    double s = 0.0;
+    for (int w = 0; w < kOptThreads / 32; w++) s += red[w];
+    __syncthreads();
+    return s;
+}
+
+// DIAG, GUARD: as clip_adam_kernel, whose global-norm fold, clip coefficient and guard decision this prologue repeats word
+// for word; a rejected step writes neither param, the moments, update, chunk_sums nor diag.
+template <bool DIAG, bool GUARD>
+__global__ void __launch_bounds__(kOptThreads) clip_lamb_moments_kernel(
+    const float *__restrict__ param, const float *__restrict__ grad, float *__restrict__ exp_avg,
+    float *__restrict__ exp_avg_sq, float *__restrict__ update, const int64_t *__restrict__ plan, double *__restrict__ chunk_sums,
+    const float *__restrict__ partials, const int64_t *step_p, double max_norm_d, double beta1_d, double beta2_d, double eps_d,
+    double wd_d, float *grad_norm_out, double *diag, const float *__restrict__ tail, int n_tail, int32_t *skip) {
+    const float max_norm = (float)max_norm_d, beta2 = (float)beta2_d, eps = (float)eps_d, wd = (float)wd_d;
+    __shared__ double red[kOptThreads / 32];
+    __shared__ float s_coef;
+    __shared__ int s_reject;
+    double acc = 0.0;
+    for (int i = threadIdx.x; i < kPartials; i += blockDim.x) acc += (double)partials[i];
+    acc = warp_sum_d(acc);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+        for (int w = 0; w < kOptThreads / 32; w++) s += red[w];
+        float total_norm = (float)sqrt(s);
+        float coef = max_norm / (total_norm + 1e-6f);  // torch clip_grad_norm_
+        s_coef = fminf(coef, 1.0f);
+        if (blockIdx.x == 0 && grad_norm_out) *grad_norm_out = total_norm;
+        bool reject = false;
+        if (GUARD) {
+            reject = !isfinite(s);
+            for (int i = 0; i < n_tail; i++) reject |= !isfinite(tail[i]);
+            s_reject = reject ? 1 : 0;
+            if (blockIdx.x == 0) *skip = reject ? 1 : 0;
+        }
+        if (DIAG && blockIdx.x == 0 && !reject) {
+            diag[0] += (double)total_norm;
+            diag[1] += (double)total_norm * (double)total_norm;
+            diag[2] += total_norm > max_norm ? 1.0 : 0.0;
+            diag[3] += 1.0;
+        }
+    }
+    __syncthreads();
+    if (GUARD && s_reject) return;
+    const float coef = s_coef;
+    const int64_t t = *step_p + 1;
+    const float bc1 = (float)(1.0 - pow(beta1_d, (double)t));
+    const float bc2_sqrt = (float)sqrt(1.0 - pow(beta2_d, (double)t));
+    const float omb1 = (float)(1.0 - beta1_d), omb2 = (float)(1.0 - beta2_d);
+    const int64_t start = plan[kLambPlanWords * blockIdx.x], len = plan[kLambPlanWords * blockIdx.x + 1];
+    double ww = 0.0, uu = 0.0;
+    for (int64_t i = start + threadIdx.x; i < start + len; i += blockDim.x) {
+        const float p = param[i];
+        const float g = grad[i] * coef;              // no wd * p here: LAMB adds the decay to the update direction
+        float m = exp_avg[i], v = exp_avg_sq[i];
+        m = m + (g - m) * omb1;
+        v = v * beta2 + omb2 * g * g;
+        const float u = (m / bc1) / (sqrtf(v) / bc2_sqrt + eps) + wd * p;
+        exp_avg[i] = m;
+        exp_avg_sq[i] = v;
+        update[i] = u;
+        ww += (double)p * (double)p;
+        uu += (double)u * (double)u;
+    }
+    ww = block_sum_d(ww, red);
+    uu = block_sum_d(uu, red);
+    if (threadIdx.x == 0) {
+        chunk_sums[2 * blockIdx.x] = ww;
+        chunk_sums[2 * blockIdx.x + 1] = uu;
+    }
+}
+
+// GUARD: nothing happens when *skip says launch A rejected the step.  ratio (may be NULL): r of tensor i -> ratio[i].
+template <bool GUARD>
+__global__ void __launch_bounds__(kOptThreads) lamb_apply_kernel(float *__restrict__ param, const float *__restrict__ update,
+                                                                 const int64_t *__restrict__ plan,
+                                                                 const double *__restrict__ chunk_sums, const float *__restrict__ lr_p,
+                                                                 double lr_scale, float *ratio, const int32_t *skip) {
+    if (GUARD && *skip) return;
+    const int64_t *me = plan + kLambPlanWords * blockIdx.x;
+    const int64_t start = me[0], len = me[1], tensor = me[2], first = me[3], count = me[4];
+    __shared__ double red[kOptThreads / 32];
+    __shared__ float s_step;
+    double ww = 0.0, uu = 0.0;          // thread t: chunks first + t, first + t + blockDim.x, ... -- the same split in every block
+    for (int64_t j = first + threadIdx.x; j < first + count; j += blockDim.x) {
+        ww += chunk_sums[2 * j];
+        uu += chunk_sums[2 * j + 1];
+    }
+    ww = block_sum_d(ww, red);
+    uu = block_sum_d(uu, red);
+    if (threadIdx.x == 0) {
+        const double r = (ww > 0.0 && uu > 0.0) ? sqrt(ww) / sqrt(uu) : 1.0;
+        s_step = (float)((double)*lr_p * lr_scale * r);
+        if (ratio && blockIdx.x == first) ratio[tensor] = (float)r;
+    }
+    __syncthreads();
+    const float step = s_step;
+    for (int64_t i = start + threadIdx.x; i < start + len; i += blockDim.x) param[i] = param[i] - step * update[i];
+}
+
 // ---- one-shot all-reduce over NVLink peer memory, fused with the sum-of-squares partials -------------------
 __device__ __forceinline__ void st_release_sys(uint32_t *p, uint32_t v) {
     asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
@@ -297,6 +411,59 @@ extern "C" int hrl_clip_adam_step(float *param, const float *grad, float *exp_av
                              : (skip ? clip_adam_kernel<false, true> : clip_adam_kernel<false, false>);
     kernel<<<grid, kOptThreads, 0, s>>>(param, grad, exp_avg, exp_avg_sq, n, partials, lr, step, max_norm, beta1, beta2, eps,
                                         weight_decay, grad_norm_out, diag_accum, tail, n_tail, skip);
+    HRL_CUDA_CHECK(cudaGetLastError());
+    if (skip)
+        bump_step_guarded_kernel<<<1, 1, 0, s>>>(step, skip);
+    else
+        bump_step_kernel<<<1, 1, 0, s>>>(step);
+    HRL_CUDA_CHECK(cudaGetLastError());
+    return HRL_OK;
+}
+
+extern "C" int64_t hrl_lamb_plan(const int64_t *numel, int32_t n_tensors, int64_t *plan) {
+    using namespace hrl;
+    HRL_REQUIRE(numel && n_tensors > 0, HRL_ERR_BAD_ARG, "hrl_lamb_plan: numel is NULL or n_tensors <= 0");
+    int64_t chunks = 0, off = 0;
+    for (int32_t i = 0; i < n_tensors; i++) {
+        HRL_REQUIRE(numel[i] > 0, HRL_ERR_BAD_ARG, "hrl_lamb_plan: tensor %d has %lld words", i, (long long)numel[i]);
+        const int64_t first = chunks, count = (numel[i] + kLambChunk - 1) / kLambChunk;
+        for (int64_t s = 0; s < numel[i]; s += kLambChunk, chunks++) {
+            if (plan) {
+                int64_t *c = plan + kLambPlanWords * chunks;
+                c[0] = off + s;
+                c[1] = numel[i] - s < kLambChunk ? numel[i] - s : kLambChunk;
+                c[2] = i;
+                c[3] = first;
+                c[4] = count;
+            }
+        }
+        off += numel[i];
+    }
+    HRL_REQUIRE(chunks <= INT32_MAX, HRL_ERR_UNSUPPORTED, "hrl_lamb_plan: %lld chunks", (long long)chunks);
+    return chunks;
+}
+
+extern "C" int hrl_clip_lamb_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, float *update, int64_t n,
+                                  const int64_t *plan, int32_t n_chunks, double *chunk_sums, const float *partials, const float *lr,
+                                  int64_t *step, double max_norm, double beta1, double beta2, double eps, double weight_decay,
+                                  double lr_scale, float *grad_norm_out, double *diag_accum, const float *tail, int32_t n_tail,
+                                  int32_t *skip, float *ratio, void *stream) {
+    using namespace hrl;
+    HRL_REQUIRE(param && grad && exp_avg && exp_avg_sq && update && plan && chunk_sums && partials && lr && step && n > 0 &&
+                    n_chunks > 0,
+                HRL_ERR_BAD_ARG, "hrl_clip_lamb_step: NULL pointer, n <= 0 or n_chunks <= 0");
+    HRL_REQUIRE(!skip || (n_tail >= 0 && (tail || n_tail == 0)), HRL_ERR_BAD_ARG,
+                "hrl_clip_lamb_step: tail is NULL with n_tail > 0, or n_tail < 0");
+    HRL_REQUIRE(lr_scale > 0.0 && isfinite(lr_scale), HRL_ERR_BAD_ARG, "hrl_clip_lamb_step: lr_scale must be finite and > 0, got %g",
+                lr_scale);
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    auto moments = diag_accum ? (skip ? clip_lamb_moments_kernel<true, true> : clip_lamb_moments_kernel<true, false>)
+                              : (skip ? clip_lamb_moments_kernel<false, true> : clip_lamb_moments_kernel<false, false>);
+    moments<<<n_chunks, kOptThreads, 0, s>>>(param, grad, exp_avg, exp_avg_sq, update, plan, chunk_sums, partials, step, max_norm,
+                                             beta1, beta2, eps, weight_decay, grad_norm_out, diag_accum, tail, n_tail, skip);
+    HRL_CUDA_CHECK(cudaGetLastError());
+    auto apply = skip ? lamb_apply_kernel<true> : lamb_apply_kernel<false>;
+    apply<<<n_chunks, kOptThreads, 0, s>>>(param, update, plan, chunk_sums, lr, lr_scale, ratio, skip);
     HRL_CUDA_CHECK(cudaGetLastError());
     if (skip)
         bump_step_guarded_kernel<<<1, 1, 0, s>>>(step, skip);

@@ -439,6 +439,63 @@ class FlatAdam:
         fastnet.new_step()          # cached adjoint weights of the convolutions are stale now
 
 
+def lamb_plan(numels):
+    """hrl_lamb_plan on the host: the (chunks, 5) int64 CPU tensor of the chunks a bucket of tensors of `numels` words (back to
+    back from word 0) is cut into -- per chunk its first word, its length, its tensor's index, and that tensor's first chunk
+    and chunk count."""
+    sizes = torch.tensor([int(k) for k in numels], dtype=torch.int64)
+    n_chunks = lib().hrl_lamb_plan(_ptr(sizes), sizes.numel(), None)
+    check(min(0, n_chunks))
+    plan = torch.empty((n_chunks, 5), dtype=torch.int64)
+    check(min(0, lib().hrl_lamb_plan(_ptr(sizes), sizes.numel(), _ptr(plan))))
+    return plan
+
+
+class FlatLamb(FlatAdam):
+    """clip_grad_norm_(max_norm) + LAMB (You et al., 2020, Algorithm 2) on FlatAdam's bucket: Adam's moments, the decay
+    added to the update direction u instead of the gradient, and one trust ratio r_i = |w_i| / |u_i| per parameter (1 when
+    either norm is 0), so w_i <- w_i - lr * lr_scale * r_i * u_i (hrl_clip_lamb_step).  The parameters' spans of the bucket
+    are cut into chunks (`plan`, lamb_plan) whose fp64 partial norms (`chunk_sums`) fold in a fixed order; `update` is the
+    scratch bucket for u.  `ratio`: None, or a float32 CUDA tensor of one entry per parameter that every step fills with the
+    r_i it applied.  Everything else -- buffers, guard, diagnostics, the peer all-reduce path -- is FlatAdam's."""
+
+    def __init__(self, params, lr, lr_scale=1.0, **kw):
+        super().__init__(params, lr, **kw)
+        device = self.flat_param.device
+        self.lr_scale = float(lr_scale)
+        self.plan = lamb_plan([p.numel() for p in self.params]).to(device)
+        self.update = torch.zeros(self.n_pad, dtype=torch.float32, device=device)
+        self.chunk_sums = torch.zeros(2 * self.plan.shape[0], dtype=torch.float64, device=device)
+        self.ratio = None
+
+    def step_reduced(self, reduced):
+        """clip + LAMB on an already all-reduced bucket whose sum-of-squares partials are in self.partials."""
+        self._clip_lamb(reduced, _stream_ptr())
+        _count(3)
+
+    def _clip_lamb(self, grad, s):
+        if self.diag is not None:
+            assert self.diag.is_cuda and self.diag.dtype == torch.float64 and self.diag.numel() == 4 and self.diag.is_contiguous()
+        if self.skip is not None:
+            assert self.skip.is_cuda and self.skip.dtype == torch.int32 and self.skip.numel() == 1
+            assert 0 <= self.guard_tail <= self.extra and grad.numel() >= self.n_pad + self.extra
+        if self.ratio is not None:
+            assert self.ratio.is_cuda and self.ratio.dtype == torch.float32 and self.ratio.numel() == len(self.params)
+        check(lib().hrl_clip_lamb_step(
+            _ptr(self.flat_param), _ptr(grad), _ptr(self.exp_avg), _ptr(self.exp_avg_sq), _ptr(self.update), self.n_pad,
+            _ptr(self.plan), self.plan.shape[0], _ptr(self.chunk_sums), _ptr(self.partials), _ptr(self.lr), _ptr(self.step_count),
+            self.max_norm, self.betas[0], self.betas[1], self.eps, self.weight_decay, self.lr_scale, _ptr(self.grad_norm),
+            _ptr(self.diag), _ptr(grad[self.n_pad:]), self.guard_tail, _ptr(self.skip), _ptr(self.ratio), s))
+
+    def step(self):
+        s = _stream_ptr()
+        check(lib().hrl_grad_sumsq(_ptr(self.flat_grad), self.n_pad, _ptr(self.partials), s))
+        self._clip_lamb(self.flat_grad, s)
+        _count(4)
+        from . import fastnet
+        fastnet.new_step()          # cached adjoint weights of the convolutions are stale now
+
+
 def _check_skip(skip):
     if not (skip.is_cuda and skip.dtype == torch.int32 and skip.numel() == 1):
         raise _capi.HrlError('handyrl_b200: skip must be a one-element int32 CUDA tensor')

@@ -609,6 +609,28 @@ class ReplayCheckpoints:
             self.thread = None
 
 
+def optimizer_config(value):
+    """train_args['optimizer'] -> {'name': 'adam'} (key absent, None or 'adam': clip + Adam, ops.FlatAdam) or
+    {'name': 'lamb', 'lr_scale': s} ('lamb', or {'name': 'lamb', 'lr_scale': s} with s a finite number > 0, default 1.0:
+    clip + LAMB, ops.FlatLamb).  Anything else -- another name, another dict key, a bad lr_scale -- raises ValueError."""
+    if value is None or (isinstance(value, str) and value == 'adam'):
+        return {'name': 'adam'}
+    if isinstance(value, str) and value == 'lamb':
+        return {'name': 'lamb', 'lr_scale': 1.0}
+    if not isinstance(value, dict):
+        raise ValueError("train_args['optimizer'] must be 'adam', 'lamb' or {'name': 'lamb', 'lr_scale': s}; got %r" % (value,))
+    unknown = sorted(str(k) for k in value if k not in ('name', 'lr_scale'))
+    if unknown:
+        raise ValueError("train_args['optimizer']: unknown key(s) %s (known: name, lr_scale)" % ', '.join(unknown))
+    if value.get('name') != 'lamb':
+        raise ValueError("train_args['optimizer']: the dict form is {'name': 'lamb', 'lr_scale': s}; got name %r"
+                         % (value.get('name'),))
+    s = value.get('lr_scale', 1.0)
+    if isinstance(s, bool) or not isinstance(s, numbers.Real) or not 0.0 < float(s) < float('inf'):
+        raise ValueError("train_args['optimizer']: lr_scale must be a finite number > 0; got %r" % (s,))
+    return {'name': 'lamb', 'lr_scale': float(s)}
+
+
 def nonfinite_guard(args):
     """train_args['skip_nonfinite'] -> whether optimiser steps whose loss or gradient is not finite are rejected on the device
     (key absent, False or None: off)."""
@@ -698,9 +720,13 @@ class OptimizerStateFormat:
     Parameter i is the i-th of net.parameters(), words [off_i, off_i + numel_i) of FlatAdam's flat buckets; the words from n
     up to n_pad are padding, not part of the format, and zero after a load.  'step' is the number of optimiser steps taken
     (FlatAdam.step_count), a float32 tensor as torch keeps it.  'schedule' holds what the next step uses: the learning rate
-    and the data-count average it came from (the device's float32 values), and the step count it was scheduled at."""
+    and the data-count average it came from (the device's float32 values), and the step count it was scheduled at.
 
-    def __init__(self, named_params, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-5, max_norm=4.0):
+    A LAMB learner (optimizer_config(...)['name'] == 'lamb', `optimizer`) adds two top-level entries, 'algorithm': 'lamb'
+    and 'lr_scale': float; its moments and step mean what Adam's do.  A dict without 'algorithm' is an Adam dict, and an Adam
+    learner writes exactly the entries above.  unpack() refuses a dict of the other algorithm; lr_scale is not compared."""
+
+    def __init__(self, named_params, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-5, max_norm=4.0, optimizer=None):
         self.names, self.shapes, self.offsets = [], [], []
         off = 0
         for k, p in named_params:
@@ -712,6 +738,7 @@ class OptimizerStateFormat:
         self.n_pad = (off + 3) // 4 * 4
         self.betas = (float(betas[0]), float(betas[1]))
         self.eps, self.weight_decay, self.max_norm = float(eps), float(weight_decay), float(max_norm)
+        self.optimizer = optimizer if optimizer is not None else {'name': 'adam'}
 
     def _spans(self):
         for name, shape, off in zip(self.names, self.shapes, self.offsets):
@@ -730,16 +757,26 @@ class OptimizerStateFormat:
             state[i] = {'step': torch.tensor(float(step), dtype=torch.float32),
                         'exp_avg': exp_avg[off:off + n].clone().view(shape),
                         'exp_avg_sq': exp_avg_sq[off:off + n].clone().view(shape)}
-        return {'optimizer': {'state': state, 'param_groups': groups},
-                'param_names': list(self.names),
-                'schedule': {'steps': int(steps), 'data_cnt_ema': float(data_cnt_ema), 'lr': float(lr)},
-                'max_norm': self.max_norm}
+        d = {'optimizer': {'state': state, 'param_groups': groups},
+             'param_names': list(self.names),
+             'schedule': {'steps': int(steps), 'data_cnt_ema': float(data_cnt_ema), 'lr': float(lr)},
+             'max_norm': self.max_norm}
+        if self.optimizer['name'] == 'lamb':
+            d['algorithm'], d['lr_scale'] = 'lamb', self.optimizer['lr_scale']
+        return d
+
+    def check_algorithm(self, d):
+        """Raise ValueError when the dict `d` was written by the other optimiser (its 'algorithm' entry, absent: Adam)."""
+        got, want = d.get('algorithm', 'adam'), self.optimizer['name']
+        if got != want:
+            raise ValueError('optimiser state: written by %s, the learner runs %s (train_args[\'optimizer\'])' % (got, want))
 
     def unpack(self, d):
         """Check a dict of this format against the net and the optimiser's settings and return its flat form
         (exp_avg, exp_avg_sq: float32 CPU tensors of n_pad words with zero padding; step; lr; data_cnt_ema; steps).
         Raises KeyError (an entry or a parameter name missing or extra) or ValueError (a shape, betas, eps, weight_decay or
-        max_norm that differs)."""
+        max_norm that differs, or a dict of the other algorithm: check_algorithm)."""
+        self.check_algorithm(d)
         for key in ('optimizer', 'param_names', 'schedule', 'max_norm'):
             if key not in d:
                 raise KeyError('optimiser state: no %r entry' % key)
@@ -965,6 +1002,13 @@ class LearnerStep:
     (`distill_accum`; accum_layout); the teacher's weights are in no bucket, hand-off or checkpoint.  With c_n = 0 the step
     is bit for bit the step without the key.  Validation passes are unchanged.
 
+    optimizer (default: train_args['optimizer'], Adam; optimizer_config): 'lamb' or {'name': 'lamb', 'lr_scale': s} runs the
+    optimiser step as clip + LAMB (ops.FlatLamb, hrl_clip_lamb_step: Adam's moments, one trust ratio |w_i| / |u_i| per
+    parameter tensor, the step lr * s * r_i * u) in place of clip + Adam, in step() and in the peer all-reduce path alike: one
+    more launch per step.  `self.optimizer` is the parsed setting.  The moments, step count, guard, diagnostics, weight
+    average, gradient accumulation and the hand-off are the same; the saved optimiser state carries 'algorithm': 'lamb'
+    (OptimizerStateFormat), and load_optimizer_state() refuses a file of the other algorithm.
+
     A feature that adds device state registers it in __init__, where it allocates it: in `_mutable` (or `_zeroed`) when a
     step or validation pass changes it, so that the capture's warm-up leaves it as it was, and in `_handoff` (a _Handoff)
     when the epoch boundary carries it to the host; end_epoch, _snapshot and _restore have no per-feature code.
@@ -974,7 +1018,8 @@ class LearnerStep:
                  max_norm=4.0, weight_decay=1e-5, time_loss_kernel=False, channels_last=True, cudnn_benchmark=True,
                  small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None,
                  weight_ema=None, save_optimizer=None, validation=None, skip_nonfinite=None, save_replay=None,
-                 gradient_accumulation=None, distill=None, teacher=None):
+                 gradient_accumulation=None, distill=None, teacher=None, optimizer=None):
+        self.optimizer = optimizer_config(args.get('optimizer') if optimizer is None else optimizer)
         self.distill = distill_mod.config({'distill': distill} if distill is not None else args, teacher_given=teacher is not None)
         if self.distill is None and teacher is not None:
             self.distill = distill_mod.config({'distill': {}}, teacher_given=True)
@@ -1048,12 +1093,15 @@ class LearnerStep:
             peer_allreduce = self.world > 1 and os.environ.get('HRL_PEER_ALLREDUCE', '1') != '0'
         self.peer = ops.PeerAllReduce(self.pg, self.device) if (peer_allreduce and self.world > 1) else None
         self.state = StateStore(self.model, self.device)
-        self.opt = ops.FlatAdam(params, lr=lr, weight_decay=weight_decay, max_norm=max_norm, extra=self.slots.n_tail,
-                                grad_alloc=self.peer.alloc if self.peer is not None else None,
-                                param_storage=self.state.flat_param)
+        bucket = dict(lr=lr, weight_decay=weight_decay, max_norm=max_norm, extra=self.slots.n_tail,
+                      grad_alloc=self.peer.alloc if self.peer is not None else None, param_storage=self.state.flat_param)
+        if self.optimizer['name'] == 'lamb':
+            self.opt = ops.FlatLamb(params, lr_scale=self.optimizer['lr_scale'], **bucket)
+        else:
+            self.opt = ops.FlatAdam(params, **bucket)
         self.state.index_params(self.model)
         self.optim_format = OptimizerStateFormat(self.model.named_parameters(), betas=self.opt.betas, eps=self.opt.eps,
-                                                 weight_decay=weight_decay, max_norm=max_norm)
+                                                 weight_decay=weight_decay, max_norm=max_norm, optimizer=self.optimizer)
         self.schedule_steps = 0          # the step count the current learning rate was scheduled at
         # what a step or a validation pass changes and the capture's warm-up must leave as it was: _snapshot clones `_mutable`,
         # _restore copies the clones back into the same tensors (the graphs bake their pointers) and zeroes `_zeroed`.
@@ -1623,7 +1671,8 @@ class LearnerStep:
         """Resume from an OptimizerStateFormat dict (e.g. a <epoch>.optim.pth file): Adam's moments and step count, the
         learning rate and the data-count average.  Call it before the first step (or warm_up), which snapshots the state
         around the capture's warm-up steps.  A dict whose parameter names or shapes differ from the net's, or whose betas,
-        eps, weight_decay or max_norm differ from this learner's, raises KeyError / ValueError and changes nothing."""
+        eps, weight_decay or max_norm differ from this learner's, or that another optimiser wrote (Adam / LAMB,
+        OptimizerStateFormat.check_algorithm), raises KeyError / ValueError and changes nothing."""
         if self._captured:
             raise RuntimeError('load_optimizer_state must come before the first step / warm_up()')
         m, v, step, lr, data_cnt_ema, steps = self.optim_format.unpack(d)
@@ -2299,9 +2348,15 @@ class Trainer:
     train_args['distill'] = {'teacher': path, 'net': 'module:function', 'coef': c0, 'anneal_steps': N} (distill.py): the
     teacher is built and loaded here (ValueError for a bad key, file or net), and every step adds the annealed term
     c_n * KL(teacher || student) on the trained policy rows (LearnerStep).  Each epoch prints 'distill = kl:<kl> term:<c_n kl>'
-    (both over dcnt) after the loss and diagnostics lines.  Helper ranks build their teacher from the same key."""
+    (both over dcnt) after the loss and diagnostics lines.  Helper ranks build their teacher from the same key.
+
+    train_args['optimizer'] = 'lamb' or {'name': 'lamb', 'lr_scale': s} (optimizer_config; ValueError for anything but these,
+    'adam' and None): every rank's LearnerStep runs clip + LAMB instead of clip + Adam on the same all-reduced bucket, with
+    the learning rate of the same schedule times s.  The .optim.pth files carry 'algorithm': 'lamb', and a restart refuses a
+    file the other optimiser wrote."""
 
     def __init__(self, args, model):
+        self.optimizer = optimizer_config(args.get('optimizer'))
         ratio = replay_ratio(args)
         self.micro_batches = gradient_accumulation(args)
         if args['batch_size'] % self.micro_batches:
@@ -2467,6 +2522,7 @@ class Trainer:
             path = self.optim_files.seed_path('optim')
             if path is not None:
                 optim_state = torch.load(path, map_location='cpu')
+                OptimizerStateFormat((), optimizer=self.optimizer).check_algorithm(optim_state)
                 sched = optim_state['schedule']         # before the helper ranks spawn: they start at self.lr
                 self.steps, self.data_cnt_ema, self.lr = int(sched['steps']), float(sched['data_cnt_ema']), float(sched['lr'])
             else:

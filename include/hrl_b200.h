@@ -18,6 +18,9 @@
  *   hrl_grad_sumsq /
  *   hrl_clip_adam_step    <- handyrl/train.py:370-371 (clip_grad_norm_(params, 4.0) + Adam.step,
  *                            Adam(lr, weight_decay=1e-5) of train.py:331)
+ *   hrl_lamb_plan /
+ *   hrl_clip_lamb_step    <- the same clip + LAMB (Adam with per-tensor trust ratios) in place of Adam; opt-in, no
+ *                            reference counterpart
  *   hrl_step_commit       <- with the guard of hrl_clip_adam_step: the same step, rejected on the device when its loss
  *                            or gradient is not finite; no reference counterpart
  *   hrl_weight_ema        <- a per-step moving average of the weights; no reference counterpart (scripts/aux_swa.py
@@ -237,6 +240,39 @@ int hrl_clip_adam_step(float *param, const float *grad, float *exp_avg, float *e
  * *grad_norm_out is written either way.  *skip (device int32) is set to 1 when rejected, 0 when accepted.  skip == NULL:
  * tail and n_tail are ignored and every step is taken.
  */
+
+/*
+ * LAMB on the same bucket (opt-in; You et al., 2020, Algorithm 2): Adam's moments with one trust ratio per parameter tensor,
+ * so that each tensor's relative step is bounded by lr * lr_scale whatever the batch size.  With t the step count after this
+ * step, c the clip coefficient of hrl_clip_adam_step (same partials, same fold) and w the weights before the step:
+ *     g = c * grad                          (no weight_decay * w term here, unlike hrl_clip_adam_step)
+ *     m = m + (g - m)(1 - beta1);   v = beta2 v + (1 - beta2) g^2          (fp32, hrl_clip_adam_step's order)
+ *     u = (m / (1 - beta1^t)) / (sqrt(v) / sqrt(1 - beta2^t) + eps) + weight_decay * w
+ *     r_i = |w_i| / |u_i| over the words of tensor i when both are > 0, else 1
+ *     w <- w - (lr * lr_scale * r_i) * u
+ * Tensor i is words [off_i, off_i + numel_i) of the bucket, in order; words outside every tensor (padding) are not touched.
+ *
+ * hrl_lamb_plan (host, no device work): cuts tensors of numel[0 .. n_tensors) words, laid out back to back from word 0, into
+ * chunks of at most 1024 words that never cross a tensor, and returns their count (a negative HrlStatus on error:
+ * HRL_ERR_BAD_ARG for numel NULL, n_tensors <= 0 or a numel <= 0).  plan != NULL (a host buffer of 5 int64 per chunk)
+ * receives, per chunk in bucket order, {first word, words, tensor index, the tensor's first chunk, the tensor's chunk count}.
+ *
+ * hrl_clip_lamb_step: three launches -- the moments, u (into `update`, n floats of scratch) and per-chunk fp64 sums of w^2
+ * and u^2 (into chunk_sums, 2 * n_chunks doubles); the ratios (each folded from its tensor's chunk sums in a fixed order, so
+ * repeated launches, graph replays and ranks give identical bits) and the weight update; then *step += 1.  `plan` is
+ * hrl_lamb_plan's table (n_chunks entries) copied to the device.  partials, lr, step, grad_norm_out, diag_accum, tail,
+ * n_tail and skip mean what they mean for hrl_clip_adam_step, and the guard rejects on the same condition: a rejected step
+ * writes neither param, the moments, update, chunk_sums, ratio nor diag_accum, and does not count.  ratio != NULL (device
+ * floats, one per tensor) receives each tensor's r_i.  HRL_ERR_BAD_ARG: a required pointer NULL, n <= 0, n_chunks <= 0,
+ * tail NULL with n_tail > 0 under the guard, or lr_scale not finite and > 0.
+ */
+int64_t hrl_lamb_plan(const int64_t *numel, int32_t n_tensors, int64_t *plan /* may be NULL */);
+int hrl_clip_lamb_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, float *update, int64_t n,
+                       const int64_t *plan, int32_t n_chunks, double *chunk_sums, const float *partials, const float *lr,
+                       int64_t *step, double max_norm, double beta1, double beta2, double eps, double weight_decay,
+                       double lr_scale, float *grad_norm_out /* may be NULL */, double *diag_accum /* may be NULL */,
+                       const float *tail, int32_t n_tail, int32_t *skip /* may be NULL */, float *ratio /* may be NULL */,
+                       void *stream);
 
 /*
  * The accumulation that follows a guarded step, in one launch that reads *skip:
