@@ -52,7 +52,7 @@ class HrlLossArgs(C.Structure):
         ('tap_target_value', C.c_void_p), ('tap_target_return', C.c_void_p), ('tap_advantage', C.c_void_p),
         ('tap_logp', C.c_void_p), ('tap_rho', C.c_void_p), ('tap_entropy', C.c_void_p),
         ('workspace', C.c_void_p), ('workspace_bytes', C.c_size_t),
-        ('tuning', HrlLossTuning), ('io_bf16', C.c_int32), ('window_weight', C.c_void_p),
+        ('tuning', HrlLossTuning), ('io_bf16', C.c_int32), ('external_heads', C.c_int32), ('window_weight', C.c_void_p),
     ]
 
 
@@ -135,6 +135,16 @@ class HrlDistillArgs(C.Structure):
     ]
 
 
+class HrlValueBinsArgs(C.Structure):
+    _fields_ = [
+        ('B', C.c_int32), ('T', C.c_int32), ('P', C.c_int32), ('Pa', C.c_int32), ('K', C.c_int32), ('burn_in', C.c_int32),
+        ('low', C.c_float), ('high', C.c_float), ('symlog', C.c_int32), ('sigma', C.c_float), ('head', C.c_int32),
+        ('logits', C.c_void_p), ('expect', C.c_void_p), ('target', C.c_void_p), ('observation_mask', C.c_void_p),
+        ('window_weight', C.c_void_p), ('dlogits', C.c_void_p), ('losses', C.c_void_p),
+        ('workspace', C.c_void_p), ('workspace_bytes', C.c_size_t),
+    ]
+
+
 # every symbol include/hrl_b200.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     'hrl_loss_workspace_bytes': (C.c_size_t, [C.c_int32] * 5),
@@ -200,6 +210,9 @@ SYMBOLS = {
     'hrl_hidden_blend_bwd': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     'hrl_distill_workspace_bytes': (C.c_size_t, [C.c_int32] * 5),
     'hrl_distill_fwd_bwd': (C.c_int, [C.POINTER(HrlDistillArgs), C.c_void_p]),
+    'hrl_value_bins_workspace_bytes': (C.c_size_t, [C.c_int32] * 5),
+    'hrl_value_bins_expect': (C.c_int, [C.POINTER(HrlValueBinsArgs), C.c_void_p]),
+    'hrl_value_bins_fwd_bwd': (C.c_int, [C.POINTER(HrlValueBinsArgs), C.c_void_p]),
     'hrl_last_error': (C.c_char_p, []),
     'hrl_abi_version': (C.c_int32, []),
 }

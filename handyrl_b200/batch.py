@@ -115,6 +115,22 @@ def flatten_moments(moments, outcome, players=None):
     return fe
 
 
+def reduce_values(fe, value_bins):
+    """A FlatEpisode whose stored values are a categorical value head's K logits (train_args['value_bins'], parsed by
+    value_bins.config) with each present value reduced to its expectation: fe.value becomes (S, Ps, 1), what the replay
+    stores.  A value is present where the player observed (flags bit 1); absent ones stay 0.  Episodes with scalar values,
+    and every episode when the value head is not categorical, are returned as they are."""
+    spec = (value_bins or {}).get('value')
+    if spec is None or fe.value.shape[-1] == 1:
+        return fe
+    if fe.value.shape[-1] != spec['bins']:
+        raise ValueError("train_args['value_bins']['value'] has %d bins, but an episode stores %d values per moment"
+                         % (spec['bins'], fe.value.shape[-1]))
+    from .value_bins import reduce_values as reduce
+    fe.value = reduce(fe.value, (fe.flags & 2) != 0, spec)
+    return fe
+
+
 def window_rows(T, burn_in, start, end, train_start):
     """Where a window [start, end) lands in the T batch steps (train.py:92-95): returns
     (t0, n) = first batch step holding real data and how many."""

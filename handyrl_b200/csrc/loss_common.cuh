@@ -11,6 +11,7 @@ struct LossParams {
     int EPB;      // episodes per CTA
     int stage_z;  // masked logits kept in shared memory between the statistics and the gradient phase
     int has_v, has_r;
+    int loss_v, loss_r;   // the head's regression sum and gradient are written here (not an external categorical head)
     int row_stride;   // floats between consecutive rows of the staged logits (>= A)
     int scan;             // recurrences as a parallel suffix scan (long windows) instead of a serial loop per column
     int cluster;          // CTAs per window (bulk kernel): 1, or 2 = thread-block cluster splitting the time axis
@@ -557,13 +558,14 @@ __device__ __forceinline__ void finalize_losses(const LossParams &prm, const Sme
             s[i] = 0;
             for (int w2 = 0; w2 < nwarp; w2++) s[i] += dred[i * 32 + w2];
         }
-        const double lv = 0.5 * s[1];
+        // an external (categorical) head's regression sum is left out: its cross-entropy kernel writes the head's entry
+        const double lv = prm.loss_v ? 0.5 * s[1] : 0.0, lr = prm.loss_r ? s[2] : 0.0;
         float *out = prm.a.losses;
         out[HRL_LOSS_P] = (float)s[0];
         out[HRL_LOSS_V] = (float)lv;
-        out[HRL_LOSS_R] = (float)s[2];
+        out[HRL_LOSS_R] = (float)lr;
         out[HRL_LOSS_ENT] = (float)s[3];
-        out[HRL_LOSS_TOTAL] = (float)(s[0] + lv + s[2] - (double)prm.a.entropy_regularization * s[4]);  // train.py:211-213
+        out[HRL_LOSS_TOTAL] = (float)(s[0] + lv + lr - (double)prm.a.entropy_regularization * s[4]);  // train.py:211-213
         out[HRL_LOSS_DCNT] = (float)s[5];
         *counter = 0u;  // leave the workspace ready for the next launch
     }

@@ -105,8 +105,8 @@ __device__ __forceinline__ void zero_burn_in(const LossParams &prm, const CtaCtx
             for (int i = c.tid; i < nz; i += c.nthr) a.dpolicy_raw[g0 * c.A + i] = 0.0f;
         }
         for (int i = c.tid; i < nzr; i += c.nthr) {
-            if (prm.has_v) a.dvalue_raw[g0 + i] = 0.0f;
-            if (prm.has_r) a.dreturn_raw[g0 + i] = 0.0f;
+            if (prm.loss_v) a.dvalue_raw[g0 + i] = 0.0f;
+            if (prm.loss_r) a.dreturn_raw[g0 + i] = 0.0f;
         }
     }
 }
@@ -328,8 +328,8 @@ __global__ void __launch_bounds__(512) loss_rows_kernel(const LossParams prm) {
             }
         }
         if (lane == 0) {
-            if (prm.has_v) a.dvalue_raw[grow] = f.gv;
-            if (prm.has_r) a.dreturn_raw[grow] = f.gr;
+            if (prm.loss_v) a.dvalue_raw[grow] = f.gv;
+            if (prm.loss_r) a.dreturn_raw[grow] = f.gr;
         }
     }
     if (IOS && GRAD) {
@@ -439,8 +439,8 @@ __global__ void __launch_bounds__(1024) loss_elem_kernel(const LossParams prm) {
         smem[L.se + r] = f.w;
         smem[L.sw + r] = f.k;
         const size_t grow = ((size_t)(c.b0 + e) * T0 + bi) * Pa + rr;
-        if (prm.has_v) a.dvalue_raw[grow] = f.gv;
-        if (prm.has_r) a.dreturn_raw[grow] = f.gr;
+        if (prm.loss_v) a.dvalue_raw[grow] = f.gv;
+        if (prm.loss_r) a.dreturn_raw[grow] = f.gr;
     }
     __syncthreads();
     HRL_STAMP(18);
@@ -543,8 +543,8 @@ __global__ void __launch_bounds__(1024) loss_group_kernel(const LossParams prm) 
             st_stream(a.dpolicy_raw + grow * A + lane, g);
         }
         if (lane == 0) {
-            if (prm.has_v) a.dvalue_raw[grow] = f.gv;
-            if (prm.has_r) a.dreturn_raw[grow] = f.gr;
+            if (prm.loss_v) a.dvalue_raw[grow] = f.gv;
+            if (prm.loss_r) a.dreturn_raw[grow] = f.gr;
         }
     }
     HRL_STAMP(19);
@@ -788,8 +788,8 @@ __global__ void __launch_bounds__(544, 2) loss_bulk_kernel(const LossParams prm)
         if (lane == 0) {
             if (io16) bulk_store(reinterpret_cast<uint16_t *>(a.dpolicy_raw) + grow * A, zrow, (uint32_t)A * 2);
             else bulk_store(a.dpolicy_raw + grow * A, zrow, (uint32_t)A * 4);
-            if (prm.has_v) a.dvalue_raw[grow] = f.gv;
-            if (prm.has_r) a.dreturn_raw[grow] = f.gr;
+            if (prm.loss_v) a.dvalue_raw[grow] = f.gv;
+            if (prm.loss_r) a.dreturn_raw[grow] = f.gr;
         }
     }
     if (GRAD && lane == 0) bulk_store_wait_all();
@@ -860,8 +860,15 @@ static int loss_fwd_bwd(const HrlLossArgs *args, float *diag, void *stream_) {
                     a.observation_mask && a.episode_mask && a.progress && a.outcome,
                 HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: a required input pointer is NULL");
     HRL_REQUIRE(a.losses && (a.dpolicy_raw || !GRAD), HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: a required output pointer is NULL");
-    HRL_REQUIRE(!GRAD || ((a.value_raw != nullptr) == (a.dvalue_raw != nullptr) && (a.return_raw != nullptr) == (a.dreturn_raw != nullptr)),
-                HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: each head needs both its output and its gradient buffer");
+    HRL_REQUIRE(a.external_heads >= 0 && a.external_heads <= 3, HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: external_heads=%d outside 0..3",
+                a.external_heads);
+    const bool ext_v = a.external_heads & 1, ext_r = a.external_heads & 2;
+    HRL_REQUIRE((!ext_v || (a.value_raw && a.tap_target_value)) && (!ext_r || (a.return_raw && a.tap_target_return)), HRL_ERR_BAD_ARG,
+                "hrl_loss_fwd_bwd: an external head needs its output and its target tap");
+    // a head whose loss another kernel computes has no gradient here; every other head needs both buffers
+    HRL_REQUIRE(!GRAD || ((ext_v ? a.dvalue_raw == nullptr : (a.value_raw != nullptr) == (a.dvalue_raw != nullptr)) &&
+                          (ext_r ? a.dreturn_raw == nullptr : (a.return_raw != nullptr) == (a.dreturn_raw != nullptr))),
+                HRL_ERR_BAD_ARG, "hrl_loss_fwd_bwd: each head needs both its output and its gradient buffer (none when external)");
     HRL_REQUIRE(a.A <= 1024, HRL_ERR_UNSUPPORTED, "hrl_loss_fwd_bwd: A=%d > 1024 not built", a.A);
     HRL_REQUIRE(a.P <= 64, HRL_ERR_UNSUPPORTED, "hrl_loss_fwd_bwd: P=%d > 64 not built", a.P);
 
@@ -870,6 +877,8 @@ static int loss_fwd_bwd(const HrlLossArgs *args, float *diag, void *stream_) {
     prm.Tt = a.T - a.burn_in;
     prm.has_v = a.value_raw != nullptr;
     prm.has_r = a.return_raw != nullptr;
+    prm.loss_v = prm.has_v && !ext_v;
+    prm.loss_r = prm.has_r && !ext_r;
     prm.cluster = 1;
     prm.diag = diag;
     const HrlLossTuning &tune = a.tuning;

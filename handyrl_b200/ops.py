@@ -55,13 +55,26 @@ class LossBuffers:
     forward-only pass (loss_fwd), without gradient buffers."""
 
     def __init__(self, B, T, P, Pa, A, has_value, has_return, device, taps=False, policy_dtype=torch.float32, diagnostics=False,
-                 grads=True, advantage=False):
+                 grads=True, advantage=False, value_bins=None):
         f = dict(dtype=torch.float32, device=device)
         self.dims = (B, T, P, Pa, A)
         self.policy_dtype = policy_dtype
+        self.has_value, self.has_return = bool(has_value), bool(has_return)
+        # value_bins (value_bins.config): the categorical heads.  Such a head has no scalar gradient here: the fused loss
+        # reads its expectation (`expect`, (B, T, Pa, 1)), writes its targets to `bins_target` (B, T, P, 1), and the
+        # cross-entropy kernel writes its logit gradient to `dlogits` (B, T, Pa, K)
+        self.value_bins = dict(value_bins or {})
+        cat = {h for h in self.value_bins if (has_value if h == 'value' else has_return)}
+        self.value_bins = {h: s for h, s in self.value_bins.items() if h in cat}
         self.dpolicy = torch.empty((B, T, Pa, A), dtype=policy_dtype, device=device) if grads else None   # bf16 logits: bf16 gradients
-        self.dvalue = torch.empty((B, T, Pa, 1), **f) if has_value and grads else None
-        self.dreturn = torch.empty((B, T, Pa, 1), **f) if has_return and grads else None
+        self.dvalue = torch.empty((B, T, Pa, 1), **f) if has_value and grads and 'value' not in cat else None
+        self.dreturn = torch.empty((B, T, Pa, 1), **f) if has_return and grads and 'return' not in cat else None
+        self.expect = {h: torch.zeros((B, T, Pa, 1), **f) for h in cat}
+        self.dlogits = {h: torch.empty((B, T, Pa, s['bins']), **f) for h, s in self.value_bins.items()} if grads else {}
+        self.bins_target = {h: torch.zeros((B, T, P, 1), **f) for h in cat}
+        self.bins_workspace = torch.zeros(max([lib().hrl_value_bins_workspace_bytes(B, T, P, Pa, s['bins'])
+                                               for s in self.value_bins.values()] or [0]), dtype=torch.uint8, device=device) \
+            if cat else None
         self.losses = torch.zeros(NUM_LOSS, **f)
         self.taps = None
         if taps:
@@ -183,6 +196,10 @@ def _loss_call(outputs, batch, args, buffers, taps, tuning, form, window_weight=
         a.tap_logp, a.tap_rho, a.tap_entropy = _ptr(t['logp']), _ptr(t['rho']), _ptr(t['entropy'])
     elif getattr(buffers, 'advantage', None) is not None:
         a.tap_advantage = _ptr(buffers.advantage)
+    for bit, head, tap in ((1, 'value', 'tap_target_value'), (2, 'return', 'tap_target_return')):
+        if head in buffers.value_bins:      # a categorical head: its loss is the cross-entropy kernel's (value_bins_fwd_bwd)
+            a.external_heads |= bit
+            setattr(a, tap, _ptr(bins_targets(buffers)[head]))
     a.window_weight = _ptr(window_weight)
     a.io_bf16 = int(io_bf16)
     ws = buffers.diag_workspace if diagnostics else buffers.workspace
@@ -218,6 +235,85 @@ def _launch(a, buffers, form):
     else:
         check(lib().hrl_loss_fwd_bwd(C.byref(a), _stream_ptr()))
     _count()
+
+
+def bins_targets(buffers):
+    """Where the loss pass writes the targets of each categorical head: the taps' tensors when the buffers keep taps."""
+    if buffers.taps is not None:
+        return {h: buffers.taps['target_' + h] for h in buffers.value_bins}
+    return buffers.bins_target
+
+
+def _bins_args(spec, head, logits, batch_dims, burn_in):
+    B, T, Pa, K = logits.shape
+    if K != spec['bins']:
+        raise ValueError("value_bins: the %s head has %d logits per row, the key %d bins" % (head, K, spec['bins']))
+    a = _capi.HrlValueBinsArgs()
+    a.B, a.T, a.P, a.Pa, a.K = B, T, batch_dims, Pa, K
+    a.burn_in = int(burn_in)
+    a.low, a.high, a.symlog, a.sigma = spec['low'], spec['high'], int(spec['symlog']), spec['sigma']
+    a.head = 0 if head == 'value' else 1
+    a.logits = _ptr(logits)
+    return a
+
+
+def _bins_logits(logits, head):
+    if not (logits.is_cuda and logits.dtype == torch.float32 and logits.is_contiguous() and logits.dim() == 4):
+        raise _capi.HrlError('handyrl_b200: the %s logits must be a contiguous (B, T, Pa, K) float32 CUDA tensor' % head)
+    return logits
+
+
+def value_bins_expect(logits, spec, head='value', out=None, P=None):
+    """The expectation v = s^-1(sum_k softmax(z)_k c_k) of a categorical head (hrl_value_bins_expect; the law in
+    value_bins.py): (B, T, Pa, K) float32 logits -> out (B, T, Pa, 1), allocated when None.  P: the batch's players (Pa when
+    None).  Returns out."""
+    logits = _bins_logits(logits, head)
+    B, T, Pa, K = logits.shape
+    if out is None:
+        out = torch.empty((B, T, Pa, 1), dtype=torch.float32, device=logits.device)
+    assert out.is_contiguous() and out.dtype == torch.float32 and out.numel() == B * T * Pa
+    a = _bins_args(spec, head, logits, Pa if P is None else P, 0)
+    a.expect = _ptr(out)
+    check(lib().hrl_value_bins_expect(C.byref(a), _stream_ptr()))
+    _count()
+    return out
+
+
+def value_bins_fwd_bwd(logits, head, spec, batch, args, buffers, window_weight=None, forward_only=False):
+    """The cross-entropy of a categorical head (hrl_value_bins_fwd_bwd; the law in value_bins.py), launched after the fused
+    loss pass that wrote `buffers` (LossBuffers with value_bins) on the same batch, from the targets that pass left in
+    bins_targets(buffers)[head].  Writes buffers.losses[v|r] = L and adds L to the total; writes dL/dz to
+    buffers.dlogits[head] unless forward_only (the held-out form: no gradient, window_weight ignored).  Returns the
+    (B, T, Pa, K) gradient, or None when forward_only."""
+    logits = _bins_logits(logits, head)
+    B, T, Pa, K = logits.shape
+    P = batch['observation_mask'].shape[2]
+    assert buffers.dims[:4] == (B, T, P, Pa) and head in buffers.value_bins
+    om = batch['observation_mask']
+    grad = None if forward_only else buffers.dlogits[head]
+    if window_weight is not None and not (window_weight.is_cuda and window_weight.dtype == torch.float32 and
+                                          window_weight.is_contiguous() and window_weight.numel() == B):
+        raise _capi.HrlError('handyrl_b200: window_weight must be a contiguous float32 CUDA tensor of B=%d weights' % B)
+    target = bins_targets(buffers)[head]
+    burn_in = int(args.get('burn_in_steps', 0))
+    key = (logits.data_ptr(), om.data_ptr(), target.data_ptr(), 0 if window_weight is None else window_weight.data_ptr(),
+           0 if grad is None else grad.data_ptr(), buffers.losses.data_ptr(), burn_in, tuple(sorted(spec.items())))
+    slot = '_cached_bins_%s_%d' % (head, int(forward_only))     # static buffers (CUDA-graph replays): the same argument block
+    cached = getattr(buffers, slot, None)
+    if cached is None or cached[0] != key:
+        keep = [_dev_f32(om, 'observation_mask')]
+        a = _bins_args(spec, head, logits, P, burn_in)
+        a.target, a.observation_mask = _ptr(target), _ptr(keep[0])
+        a.window_weight = None if forward_only else _ptr(window_weight)
+        a.dlogits, a.losses = _ptr(grad), _ptr(buffers.losses)
+        a.workspace, a.workspace_bytes = _ptr(buffers.bins_workspace), buffers.bins_workspace.numel()
+        cached = (key, a, keep)
+        if keep[0] is om:
+            setattr(buffers, slot, cached)
+    check(lib().hrl_value_bins_fwd_bwd(C.byref(cached[1]), _stream_ptr()))
+    setattr(buffers, '_bins_keep_' + head, cached[2])       # the launch is asynchronous: keep temporaries alive
+    _count()
+    return grad
 
 
 def distill_fwd_bwd(policy, teacher, batch, args, buffers, step_count, coef, anneal_steps=0, window_weight=None, sums=None):

@@ -30,7 +30,8 @@ import torch
 
 from . import ops, fastnet, priority, symmetry
 from . import distill as distill_mod
-from .batch import tree_map, tree_leaves, make_batch, gather_windows, sample_window
+from . import value_bins as value_bins_mod
+from .batch import tree_map, tree_leaves, make_batch, gather_windows, sample_window, reduce_values
 from ._capi import DIAG_KEYS, LOSS_KEYS, NUM_DIAG, NUM_LOSS, NUM_LOSS_DIAG
 
 
@@ -146,7 +147,11 @@ class _FusedLoss(torch.autograd.Function):
 
 def compute_loss(batch, model, hidden, args):
     """Drop-in for handyrl.train.compute_loss (train.py:218-267): returns
-    ({'p','v','r','ent','total'} 0-d tensors, dcnt float).  `total` is differentiable."""
+    ({'p','v','r','ent','total'} 0-d tensors, dcnt float).  `total` is differentiable.  Categorical heads
+    (train_args['value_bins']) are trained by LearnerStep and Trainer only: with that key on this raises ValueError."""
+    if value_bins_mod.config(args) is not None:
+        raise ValueError("train_args['value_bins']: the drop-in compute_loss trains scalar heads only; categorical heads train "
+                         "through LearnerStep or Trainer")
     outs = forward_raw(model, hidden, batch, args)
     keys = [k for k in ('policy', 'value', 'return') if k in outs]
     total, vec = _FusedLoss.apply(batch, args, keys, *[outs[k] for k in keys])
@@ -1009,6 +1014,15 @@ class LearnerStep:
     average, gradient accumulation and the hand-off are the same; the saved optimiser state carries 'algorithm': 'lamb'
     (OptimizerStateFormat), and load_optimizer_state() refuses a file of the other algorithm.
 
+    value_bins (default: train_args['value_bins'], off; value_bins.py): categorical value / return heads.  The key is parsed
+    here, and a probe call of the net on one observation checks that it outputs every listed head (ValueError otherwise); the
+    first forward of warm_up() checks that each such head has K logits in its last dimension (ValueError otherwise -- so a
+    net with one-output heads, such as the fused tower's, is refused).  Each micro-batch then runs, after the net's forward,
+    one ops.value_bins_expect launch per categorical head (the expectation the fused loss reads in place of the head), the
+    fused loss with that head's term and gradient left to the next launch, and one ops.value_bins_fwd_bwd launch per head
+    (the cross-entropy: its sum replaces the head's loss sum and joins the total, its logit gradient goes to the net's
+    backward).  Validation passes run the forward-only forms.  With the key off nothing of this runs.
+
     A feature that adds device state registers it in __init__, where it allocates it: in `_mutable` (or `_zeroed`) when a
     step or validation pass changes it, so that the capture's warm-up leaves it as it was, and in `_handoff` (a _Handoff)
     when the epoch boundary carries it to the host; end_epoch, _snapshot and _restore have no per-feature code.
@@ -1018,8 +1032,9 @@ class LearnerStep:
                  max_norm=4.0, weight_decay=1e-5, time_loss_kernel=False, channels_last=True, cudnn_benchmark=True,
                  small_boards=True, peer_allreduce=None, allow_tf32=None, fused_tower=True, tensor_cores=None, diagnostics=None,
                  weight_ema=None, save_optimizer=None, validation=None, skip_nonfinite=None, save_replay=None,
-                 gradient_accumulation=None, distill=None, teacher=None, optimizer=None):
+                 gradient_accumulation=None, distill=None, teacher=None, optimizer=None, value_bins=None):
         self.optimizer = optimizer_config(args.get('optimizer') if optimizer is None else optimizer)
+        self.value_bins = value_bins_mod.config({'value_bins': value_bins} if value_bins is not None else args)
         self.distill = distill_mod.config({'distill': distill} if distill is not None else args, teacher_given=teacher is not None)
         if self.distill is None and teacher is not None:
             self.distill = distill_mod.config({'distill': {}}, teacher_given=True)
@@ -1054,6 +1069,8 @@ class LearnerStep:
         torch.backends.cudnn.allow_tf32 = allow_tf32
         torch.backends.cuda.matmul.allow_tf32 = allow_tf32
         self.model = model.to(self.device)
+        if self.value_bins is not None:         # a categorical head the net does not output: refused before anything runs
+            value_bins_mod.check_net_heads(self.value_bins, self._probe_outputs(example_batch), bins=False)
         # cuDNN's default heuristics pick FFT / NCHW-spatial kernels that are 5x slower than its NHWC
         # implicit-GEMM kernels on the tiny boards of these games; NHWC + autotune is a pure layout choice
         # tiny boards: convolutions as one SGEMM, BatchNorm as fused reductions (fastnet.py); NCHW stays as is
@@ -1211,6 +1228,19 @@ class LearnerStep:
         self.stream = torch.cuda.Stream(device=self.device)
         self._warm = PackedBatch(self.layout).fill(example_batch)
 
+    def _probe_outputs(self, example_batch):
+        """The net's outputs on one observation (eval mode, no gradient): which heads it has."""
+        obs = tree_map(lambda o: o[:1, :1, :1].flatten(0, 2).to(self.device), example_batch['observation'])
+        hidden = None
+        if hasattr(self.model, 'init_hidden'):
+            hidden = tree_map(lambda h: h.to(self.device), self.model.init_hidden([obs_rows(obs)]))
+        was_training = self.model.training
+        self.model.eval()
+        with torch.no_grad():
+            outs = self.model(obs, hidden)
+        self.model.train(was_training)
+        return {k: v for k, v in outs.items() if k != 'hidden' and v is not None}
+
     def _uses_dense_convs(self, example_batch, model=None):
         """One no-grad probe call of the net (or of `model`, the teacher) on a two-sample slice: do its convolutions take the
         dense small-board path (then activations stay NCHW) or cuDNN (then NHWC, whose implicit-GEMM kernels are the fast
@@ -1250,8 +1280,9 @@ class LearnerStep:
         loss_buf is micro-batch 0's; val_buf takes the validation passes' forward-only outputs."""
         B, T, P, Pa, A = self.dims
         Bm = B // self.micro_batches
+        value_bins_mod.check_net_heads(self.value_bins, outs)
         heads = ('value' in outs, 'return' in outs)
-        base = ops.LossBuffers(Bm, T, P, Pa, A, *heads, self.device, diagnostics=self.diagnostics)
+        base = ops.LossBuffers(Bm, T, P, Pa, A, *heads, self.device, diagnostics=self.diagnostics, value_bins=self.value_bins)
         self._loss_bufs = []
         for i in range(self.micro_batches):
             buf = copy.copy(base)
@@ -1263,7 +1294,7 @@ class LearnerStep:
             self._loss_bufs.append(buf)
         self.loss_buf = self._loss_bufs[0]
         if self.validation:
-            self.val_buf = ops.LossBuffers(Bm, T, P, Pa, A, *heads, self.device, grads=False)
+            self.val_buf = ops.LossBuffers(Bm, T, P, Pa, A, *heads, self.device, grads=False, value_bins=self.value_bins)
 
     def _net_backward(self, outs, buf, accumulate=False):
         """The net's backward from the loss kernel's output gradients in `buf`, into the gradient bucket (added to it when
@@ -1273,12 +1304,10 @@ class LearnerStep:
                                  buf.dreturn.flatten(0, 2) if buf.dreturn is not None else None, accumulate=accumulate)
         else:
             heads, grads = [outs['policy']], [buf.dpolicy]
-            if 'value' in outs:
-                heads.append(outs['value'])
-                grads.append(buf.dvalue)
-            if 'return' in outs:
-                heads.append(outs['return'])
-                grads.append(buf.dreturn)
+            for h, g in (('value', buf.dvalue), ('return', buf.dreturn)):
+                if h in outs:
+                    heads.append(outs[h])
+                    grads.append(buf.dlogits[h] if h in buf.value_bins else g)      # a categorical head: its logit gradient
             with ops.deferred_weight_gradients():       # shared (recurrent) convolution weights: one product per weight, at the end
                 torch.autograd.backward(heads, grads)
 
@@ -1294,12 +1323,14 @@ class LearnerStep:
             if self.loss_buf is None:
                 self._build_loss_buffers(outs)
             buf = self._loss_bufs[i]
-            loss = functools.partial(ops.loss_fwd_bwd, {k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, dev,
+            loss = functools.partial(ops.loss_fwd_bwd, self._loss_heads(outs, buf), dev,
                                      self.args, buffers=buf, diagnostics=self.diagnostics, window_weight=weight)
             if i == len(self._micro) - 1:
                 yield loss
             else:
                 loss()
+            for h, spec in buf.value_bins.items():      # the categorical heads' cross-entropy, from the targets the loss left
+                ops.value_bins_fwd_bwd(outs[h].contiguous(), h, spec, dev, self.args, buf, window_weight=weight)
             if teacher is not None:
                 ops.distill_fwd_bwd(outs['policy'], teacher, dev, self.args, buf, self.opt.step_count, self.distill['coef'],
                                     self.distill['anneal_steps'], window_weight=weight,
@@ -1314,6 +1345,14 @@ class LearnerStep:
         else:
             ops.sum_rows(self.loss_rows, n, self.opt.extra_slots)
         self._finish_step()
+
+    def _loss_heads(self, outs, buf):
+        """The heads the fused loss reads: the net's raw outputs, each categorical head replaced by its expectation (one
+        ops.value_bins_expect launch per head, into buf.expect)."""
+        heads = {k: outs[k] for k in ('policy', 'value', 'return') if k in outs}
+        for h, spec in buf.value_bins.items():
+            heads[h] = ops.value_bins_expect(outs[h].contiguous(), spec, h, out=buf.expect[h], P=self.dims[2])
+        return heads
 
     def _finish_step(self):
         """The step's tail, once per step: the (all-reduced) bucket -> the optimiser and what follows it."""
@@ -1369,8 +1408,9 @@ class LearnerStep:
                 outs = self._forward(dev)
             if self.loss_buf is None:
                 self._build_loss_buffers(outs)
-            sums = ops.loss_fwd({k: outs[k] for k in ('policy', 'value', 'return') if k in outs}, dev, self.args,
-                                buffers=self.val_buf)
+            sums = ops.loss_fwd(self._loss_heads(outs, self.val_buf), dev, self.args, buffers=self.val_buf)
+            for h, spec in self.val_buf.value_bins.items():
+                ops.value_bins_fwd_bwd(outs[h].contiguous(), h, spec, dev, self.args, self.val_buf, forward_only=True)
             (self.val_ema_accum if averaged else self.val_accum).add_(sums)
             del outs
         store.bytes.copy_(self.val_saved)
@@ -1960,6 +2000,10 @@ class GpuBatcher:
     (priority.sampler_key) and the counter is the number of batches drawn.  Symmetry transforms are still drawn on the host.
     fill_validation() keeps the host sampler.
 
+    With train_args['value_bins'] listing the value head (value_bins.py), the feeder reduces each arriving episode's stored
+    K-vector values (the categorical head's logits) to their expectation before staging, so the ring keeps one value per
+    player.
+
     With a `limiter` (a ReplayRatioLimiter, train_args['replay_ratio']), the feeder adds the steps of the episodes it committed
     to the training ring after each commit; held-out episodes add nothing.
 
@@ -1992,6 +2036,7 @@ class GpuBatcher:
         self.sym_rng = symmetry.sampler_rng(seed) if self.symmetry is not None else None
         self.sym_tables = None
         self.priority = priority.config(args)
+        self.value_bins = value_bins_mod.config(args)
         self.prio_key = priority.sampler_key(seed)
         self.prio_batches = 0               # the Philox counter of the next prioritised batch
         self.fed = 0
@@ -2080,7 +2125,7 @@ class GpuBatcher:
             try:
                 if self.forward is not None:
                     self.forward(eps)
-                fes = [episode_to_flat(ep) for ep in eps]
+                fes = [reduce_values(episode_to_flat(ep), self.value_bins) for ep in eps]
                 held = [held_out(fe, self.validation) for fe in fes]
                 train = [fe for fe, h in zip(fes, held) if not h]
                 val = [fe for fe, h in zip(fes, held) if h] if self.val_replay is not None else []
@@ -2353,7 +2398,13 @@ class Trainer:
     train_args['optimizer'] = 'lamb' or {'name': 'lamb', 'lr_scale': s} (optimizer_config; ValueError for anything but these,
     'adam' and None): every rank's LearnerStep runs clip + LAMB instead of clip + Adam on the same all-reduced bucket, with
     the learning rate of the same schedule times s.  The .optim.pth files carry 'algorithm': 'lamb', and a restart refuses a
-    file the other optimiser wrote."""
+    file the other optimiser wrote.
+
+    train_args['value_bins'] = {'value': {'bins': K, 'low': lo, 'high': hi, 'symlog': bool, 'sigma': s}, 'return': {...}}
+    (value_bins.py; ValueError here for a malformed key): the listed heads output K logits and train by cross-entropy against
+    two-hot (sigma 0) or HL-Gauss targets (LearnerStep).  The GPU replay reduces the K logits the workers stored as each
+    moment's value to their expectation when the episode arrives, so the replay and its files hold one value per player as
+    before.  The epoch line's v: / r: is then the mean cross-entropy per dcnt."""
 
     def __init__(self, args, model):
         self.optimizer = optimizer_config(args.get('optimizer'))
@@ -2368,6 +2419,7 @@ class Trainer:
         self.symmetry = symmetry.config(args)
         self.priority = priority.config(args)
         self.distill = distill_mod.config(args)
+        self.value_bins = value_bins_mod.config(args)      # malformed train_args['value_bins'] fails here
         # the teacher of train_args['distill'], built now (a deep copy of the net as received, before the learner rewrites it)
         self.teacher = distill_mod.teacher_net(self.distill, model) if self.distill is not None else None
         self.validate_every = max(1, int(round(1.0 / self.validation))) if self.validation is not None else 0
@@ -2549,8 +2601,7 @@ class Trainer:
                                           limiter=self.limiter, restore=self.restored)
             self.gpu_batcher.run()
         loss_buf = self.stepper.loss_buf
-        self.heads = ['p'] + (['v'] if loss_buf.dvalue is not None else []) + \
-            (['r'] if loss_buf.dreturn is not None else []) + ['ent', 'total']
+        self.heads = ['p'] + (['v'] if loss_buf.has_value else []) + (['r'] if loss_buf.has_return else []) + ['ent', 'total']
 
     def train(self):
         if len(self.params) == 0:          # non-parametric model (train.py:348-350)

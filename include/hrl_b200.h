@@ -33,6 +33,10 @@
  *                            per-episode priority, with importance weights; no reference counterpart
  *   hrl_distill_fwd_bwd   <- an annealed KL(teacher || student) term on the trained policy rows ("kickstarting"), launched
  *                            after hrl_loss_fwd_bwd; no reference counterpart
+ *   hrl_value_bins_expect /
+ *   hrl_value_bins_fwd_bwd <- categorical value / return heads (two-hot or HL-Gauss targets, cross-entropy) in place of
+ *                            the squared-error / smooth-L1 terms of compose_losses (train.py:204-206); opt-in, no
+ *                            reference counterpart
  *   hrl_gemm_tf32x3       <- the Linear/Conv contractions of the user's net inside train.py:142-146 (+ autograd, :369)
  *
  * Conventions
@@ -146,6 +150,13 @@ typedef struct HrlLossArgs {
                                     move through HBM.  Wide rows only (256 < A <= 512, A % 8 == 0); everything in between --
                                     masks, softmax statistics, targets, the gradient before its final rounding -- stays fp32, so
                                     the losses equal those of the fp32 call on the widened logits bit for bit              */
+    int32_t external_heads;      /* heads whose loss another kernel computes (categorical heads, hrl_value_bins_fwd_bwd):
+                                    bit 0 value, bit 1 return.  For such a head the pass still reads its raw output (the
+                                    expectation) to form targets, advantages and the diagnostics sums, but adds no term to
+                                    losses[HRL_LOSS_V|R] (left 0) or the total, never writes its gradient -- whose pointer must
+                                    be NULL -- and requires its tap_target_* (where the cross-entropy kernel reads the targets).
+                                    0 = every present head is a scalar regression, as before.  It fills the padding before
+                                    window_weight: the struct keeps its size and every other offset                     */
     const float *window_weight;  /* (B) importance weight of each window (prioritised replay), or NULL = 1.  It multiplies every
                                     per-cell loss term of window b (policy, value, return, entropy, entropy regulariser) and
                                     their gradients; dcnt and the diagnostics sums stay unweighted.  Weights of exactly 1
@@ -734,6 +745,50 @@ typedef struct HrlDistillArgs {
 
 size_t hrl_distill_workspace_bytes(int32_t B, int32_t T, int32_t P, int32_t Pa, int32_t A);
 int hrl_distill_fwd_bwd(const HrlDistillArgs *args, void *stream);
+
+/*
+ * Categorical value heads (opt-in): a value or return head that outputs K logits per row, a distribution over K bins, trained
+ * by cross-entropy against a two-hot or HL-Gauss target distribution.  Row (b, t, q) of the (B,T,Pa,K) logits z:
+ *   bins         D = (high - low) / (K - 1), centres c_k = low + k D, edges e_k = low + (k - 1/2) D   (k = 0 .. K)
+ *   transform    s(y) = sign(y) log(1 + |y|) when symlog, else y;   s^-1(m) = sign(m) (exp|m| - 1)
+ *   expectation  p = softmax(z),  v = s^-1(sum_k p_k c_k)                     (what the fused loss reads as the head's output)
+ *   target       x = clamp(s(y), low, high) for a target y (the loss pass's tap_target_value / _return)
+ *                sigma == 0 (two-hot): j = min(floor((x - low) / D), K - 2), u = (x - c_j) / D, pi_j = 1 - u, pi_j+1 = u
+ *                sigma > 0 (HL-Gauss): pi_k = [Phi((e_k+1 - x) / sigma) - Phi((e_k - x) / sigma)] /
+ *                                             [Phi((e_K - x) / sigma) - Phi((e_0 - x) / sigma)]
+ *   loss         over trained columns (b, t, p) -- t >= burn_in, or T == 1 -- with q = p when Pa == P, else 0:
+ *                L = sum w_b om_btp (-sum_k pi_k(y_btp) log p_k(z_btq)),  dz_btq = sum_p w_b om_btp (p - pi(y_btp))
+ *                om = observation_mask, w_b = window_weight[b] (1 when NULL); rows not trained get dz = 0.
+ *
+ * hrl_value_bins_expect   logits -> expect (B,T,Pa), every row.
+ * hrl_value_bins_fwd_bwd  one head per launch: dlogits (overwritten; rows of weight 0 are zero and never read),
+ *                         losses[HRL_LOSS_V] (head 0) or losses[HRL_LOSS_R] (head 1) = L, losses[HRL_LOSS_TOTAL] += L.
+ *                         dlogits == NULL: the forward-only form (held-out losses), which ignores window_weight.
+ *                         Block partials are folded in fp64 in a fixed order by the last CTA, which resets the workspace
+ *                         counter: repeated launches and graph replays give identical bits.
+ * Both: 2 <= K <= 1024, P <= 64, Pa = 1 or P (else HRL_ERR_UNSUPPORTED); low < high finite, sigma finite >= 0 (HRL_ERR_BAD_ARG).
+ */
+typedef struct HrlValueBinsArgs {
+    int32_t B, T, P, Pa, K;
+    int32_t burn_in;
+    float low, high;              /* the centres span [low, high] (in symlog space when symlog)                */
+    int32_t symlog;
+    float sigma;                  /* 0 two-hot, > 0 HL-Gauss width in bin-space units                           */
+    int32_t head;                 /* 0 value (losses[HRL_LOSS_V]), 1 return (losses[HRL_LOSS_R])               */
+    const float *logits;          /* (B,T,Pa,K)                                                                 */
+    float *expect;                /* (B,T,Pa) out of hrl_value_bins_expect                                      */
+    const float *target;          /* (B,T,P) the loss pass's target tap of this head                            */
+    const float *observation_mask;/* (B,T,P)                                                                    */
+    const float *window_weight;   /* (B) importance weights, or NULL = 1                                        */
+    float *dlogits;               /* (B,T,Pa,K) out, or NULL (forward only)                                     */
+    float *losses;                /* [HRL_NUM_LOSS] of the loss pass                                            */
+    void *workspace;              /* >= hrl_value_bins_workspace_bytes(...), first 64 bytes zero on the first call */
+    size_t workspace_bytes;
+} HrlValueBinsArgs;
+
+size_t hrl_value_bins_workspace_bytes(int32_t B, int32_t T, int32_t P, int32_t Pa, int32_t K);
+int hrl_value_bins_expect(const HrlValueBinsArgs *args, void *stream);
+int hrl_value_bins_fwd_bwd(const HrlValueBinsArgs *args, void *stream);
 
 /* Text of the last error raised on the calling thread ("" if none). */
 const char *hrl_last_error(void);
