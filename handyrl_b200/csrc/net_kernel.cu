@@ -107,8 +107,9 @@ __global__ void board_pack_kernel(const PackJobs jobs) {
     board_pack_body(jobs.job[k], blockIdx.x - jobs.first_block[k], jobs.first_block[k + 1] - jobs.first_block[k]);
 }
 
-// one CTA per output channel o: its HW rows of the dense gradient (a contiguous slab of HW * Cin*HW floats per K slice) are
-// summed over the slices with coalesced reads (fixed order -> deterministic) into shared memory, then folded onto the taps
+// one CTA per output channel o and group of input channels: the HW rows of the dense gradient of o (HW * Cin*HW floats per K slice),
+// in the group's columns only, are summed over the slices with coalesced reads (fixed order -> deterministic) into shared memory,
+// then folded onto the group's taps
 struct FoldJobs {
     HrlFoldJob job[HRL_MAX_BOARD_JOBS];
     int first_block[HRL_MAX_BOARD_JOBS + 1];
@@ -117,7 +118,7 @@ struct FoldJobs {
 };
 
 __global__ void board_fold_kernel(const FoldJobs jobs) {
-    extern __shared__ float slab[];                   // [HW][Cin*HW]; a CTA fills only the columns of its input channels
+    extern __shared__ float slab[];                   // [HW][c_n]: the HW rows of this CTA's own columns, the input channels i_lo..i_hi
     int jk = 0;
     while (jk + 1 < jobs.n && (int)blockIdx.x >= jobs.first_block[jk + 1]) jk++;
     const HrlFoldJob &J = jobs.job[jk];
@@ -136,7 +137,7 @@ __global__ void board_fold_kernel(const FoldJobs jobs) {
     // slice order through shared memory -- deterministic
     const int n_elem = HW * c_n, n_pad = (n_elem + 31) & ~31;
     const int parts = min((int)blockDim.x / n_pad, splits);
-    float *partial = slab + HW * cols;                // [parts][n_pad], behind the slab
+    float *partial = slab + n_elem;                   // [parts][n_pad], behind the slab
     if (parts >= 2) {
         const int part = threadIdx.x / n_pad, e0 = threadIdx.x - part * n_pad;
         if (part < parts && e0 < n_elem) {
@@ -152,10 +153,10 @@ __global__ void board_fold_kernel(const FoldJobs jobs) {
         }
         __syncthreads();
         if ((int)threadIdx.x < n_elem) {
-            const int e0 = threadIdx.x, e = (e0 / c_n) * cols + c_lo + e0 % c_n;
+            const int e0 = threadIdx.x;
             float sum = partial[e0];
             for (int q = 1; q < parts; q++) sum += partial[q * n_pad + e0];
-            slab[e] = sum;
+            slab[e0] = sum;
         }
     } else {
         for (int e0 = threadIdx.x; e0 < n_elem; e0 += blockDim.x) {
@@ -167,7 +168,7 @@ __global__ void board_fold_kernel(const FoldJobs jobs) {
                 for (int u = 0; u < 8; u++) acc[u] += __ldg(base + (long long)(sp + u) * split_stride + e);
             }
             for (; sp < splits; sp++) acc[0] += __ldg(base + (long long)sp * split_stride + e);
-            slab[e] = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
+            slab[e0] = ((acc[0] + acc[1]) + (acc[2] + acc[3])) + ((acc[4] + acc[5]) + (acc[6] + acc[7]));
         }
     }
     __syncthreads();
@@ -181,7 +182,7 @@ __global__ void board_fold_kernel(const FoldJobs jobs) {
             for (int qx = 0; qx < W; qx++) {
                 const int px = qx + b - kw / 2;
                 if (px < 0 || px >= W) continue;
-                s += slab[(qy * W + qx) * cols + i * HW + py * W + px];
+                s += slab[(qy * W + qx) * c_n + (i - i_lo) * HW + py * W + px];
             }
         }
         float *d = dw + ((long long)(o * Cin + i) * kh + a) * kw + b;
@@ -489,17 +490,20 @@ extern "C" int hrl_board_fold_many(const HrlFoldJob *jobs, int32_t n_jobs, void 
         HRL_REQUIRE(j.ddense && j.dw && j.splits >= 1 && j.Cout > 0 && j.Cin > 0 && j.kh > 0 && j.kw > 0 && j.H > 0 && j.W > 0 && (j.kh & 1) &&
                         (j.kw & 1),
                     HRL_ERR_BAD_ARG, "hrl_board_fold: NULL pointer or bad shape (odd kernels only)");
-        const size_t slab_bytes = (size_t)j.H * j.W * j.Cin * j.H * j.W * sizeof(float) + 512 * sizeof(float);      // + slice-run partials
-        HRL_REQUIRE(slab_bytes <= 200 * 1024, HRL_ERR_UNSUPPORTED, "hrl_board_fold: Cin*(H*W)^2 = %zu floats exceed shared memory",
-                    slab_bytes / sizeof(float));
-        if (slab_bytes > slab_max) slab_max = slab_bytes;
         fj.job[k] = j;
         // (output channel, group of input channels) CTAs: at least about two per SM, and few enough elements per CTA (<= 128) that
         // several threads can share the K slices of one element
         int groups = (2 * kNumSM + j.Cout - 1) / j.Cout;
-        const int cells2 = j.H * j.W * j.H * j.W, i_per = cells2 >= 128 ? 1 : 128 / cells2;
-        if (groups < (j.Cin + i_per - 1) / i_per) groups = (j.Cin + i_per - 1) / i_per;
+        const int cells2 = j.H * j.W * j.H * j.W, i_max = cells2 >= 128 ? 1 : 128 / cells2;
+        if (groups < (j.Cin + i_max - 1) / i_max) groups = (j.Cin + i_max - 1) / i_max;
         if (groups > j.Cin) groups = j.Cin;
+        const int i_per = (j.Cin + groups - 1) / groups;      // input channels per CTA, as the kernel splits them
+        groups = (j.Cin + i_per - 1) / i_per;                 // the same split, with no CTA left without a channel
+        // a CTA's slab holds the rows of its own columns only, + the slice-run partials
+        const size_t slab_bytes = ((size_t)j.H * j.W * j.H * j.W * i_per + 512) * sizeof(float);
+        HRL_REQUIRE(slab_bytes <= 200 * 1024, HRL_ERR_UNSUPPORTED, "hrl_board_fold: (H*W)^2 x %d channels = %zu floats exceed shared memory",
+                    i_per, slab_bytes / sizeof(float));
+        if (slab_bytes > slab_max) slab_max = slab_bytes;
         fj.groups[k] = groups;
         fj.first_block[k + 1] = fj.first_block[k] + j.Cout * groups;
     }
