@@ -161,6 +161,9 @@ SYMBOLS = {
     'hrl_lamb_plan': (C.c_int64, [C.c_void_p, C.c_int32, C.c_void_p]),
     'hrl_clip_lamb_step': (C.c_int, [C.c_void_p] * 5 + [C.c_int64, C.c_void_p, C.c_int32] + [C.c_void_p] * 4 + [C.c_double] * 6 +
                            [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'hrl_muon_plan': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'hrl_clip_muon_step': (C.c_int, [C.c_void_p] * 4 + [C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32] + [C.c_void_p] * 3 +
+                           [C.c_double] * 6 + [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     'hrl_step_commit': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                                   C.c_void_p]),
     'hrl_weight_ema': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float, C.c_int32, C.c_void_p, C.c_void_p]),

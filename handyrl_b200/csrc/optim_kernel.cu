@@ -6,12 +6,9 @@
 // => bit-reproducible), hrl_clip_adam_step has every block fold those partials itself and
 // then update its slice.  lr and the step counter are read from device memory so a captured
 // CUDA graph keeps working while the host changes the learning rate (train.py:383-384).
-#include "common.cuh"
+#include "optim_common.cuh"
 
 namespace hrl {
-
-constexpr int kPartials = 2 * kNumSM;  // 264 blocks: two per SM
-constexpr int kOptThreads = 256;
 
 __global__ void __launch_bounds__(kOptThreads) grad_sumsq_kernel(const float *__restrict__ g, int64_t n,
                                                                   float *__restrict__ partials) {
@@ -45,59 +42,14 @@ __global__ void __launch_bounds__(kOptThreads) clip_adam_kernel(
     float *__restrict__ exp_avg_sq, int64_t n, const float *__restrict__ partials, const float *__restrict__ lr_p,
     int64_t *step_p, double max_norm_d, double beta1_d, double beta2_d, double eps_d, double wd_d,
     float *grad_norm_out, double *diag, const float *__restrict__ tail, int n_tail, int32_t *skip) {
-    const float max_norm = (float)max_norm_d, beta2 = (float)beta2_d, eps = (float)eps_d, wd = (float)wd_d;
     // every block folds the partial sums in the same order -> identical clip coefficient everywhere
-    __shared__ double red[kOptThreads / 32];
-    __shared__ float s_coef;
-    __shared__ int s_reject;
-    double acc = 0.0;
-    for (int i = threadIdx.x; i < kPartials; i += blockDim.x) acc += (double)partials[i];
-    acc = warp_sum_d(acc);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-        for (int w = 0; w < kOptThreads / 32; w++) s += red[w];
-        float total_norm = (float)sqrt(s);
-        float coef = max_norm / (total_norm + 1e-6f);  // torch clip_grad_norm_
-        s_coef = fminf(coef, 1.0f);
-        if (blockIdx.x == 0 && grad_norm_out) *grad_norm_out = total_norm;
-        bool reject = false;
-        if (GUARD) {
-            reject = !isfinite(s);                      // also a finite gradient whose fp32 sum of squares overflowed
-            for (int i = 0; i < n_tail; i++) reject |= !isfinite(tail[i]);
-            s_reject = reject ? 1 : 0;
-            if (blockIdx.x == 0) *skip = reject ? 1 : 0;
-        }
-        if (DIAG && blockIdx.x == 0 && !reject) {
-            diag[0] += (double)total_norm;
-            diag[1] += (double)total_norm * (double)total_norm;
-            diag[2] += total_norm > max_norm ? 1.0 : 0.0;
-            diag[3] += 1.0;
-        }
-    }
-    __syncthreads();
-    if (GUARD && s_reject) return;
-    const float coef = s_coef;
-    const int64_t t = *step_p + 1;
-    const float lr = *lr_p;
-    const double bc1 = 1.0 - pow(beta1_d, (double)t);
-    const double bc2 = 1.0 - pow(beta2_d, (double)t);
-    const float step_size = (float)((double)lr / bc1);
-    const float bc2_sqrt = (float)sqrt(bc2);
-    const float omb1 = (float)(1.0 - beta1_d), omb2 = (float)(1.0 - beta2_d);
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        float p = param[i];
-        float g = grad[i] * coef;
-        g = g + wd * p;
-        float m = exp_avg[i], v = exp_avg_sq[i];
-        m = m + (g - m) * omb1;
-        v = v * beta2 + omb2 * g * g;
-        float denom = sqrtf(v) / bc2_sqrt + eps;
-        param[i] = p - step_size * (m / denom);
-        exp_avg[i] = m;
-        exp_avg_sq[i] = v;
-    }
+    float coef;
+    bool reject;
+    clip_prologue<DIAG, GUARD>(partials, (float)max_norm_d, grad_norm_out, diag, tail, n_tail, skip, coef, reject);
+    if (reject) return;
+    const AdamConsts a = adam_consts(lr_p, step_p, beta1_d, beta2_d, eps_d, wd_d);
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        adam_word(param, grad, exp_avg, exp_avg_sq, i, coef, a);
 }
 
 // ---- LAMB (You et al., 2020, Algorithm 2) on the same bucket: Adam's moments, one trust ratio per parameter tensor --------
@@ -108,16 +60,6 @@ __global__ void __launch_bounds__(kOptThreads) clip_adam_kernel(
 constexpr int kLambChunk = 1024;   // words per chunk: 4 per thread of a kOptThreads block
 constexpr int kLambPlanWords = 5;  // int64 per chunk: start, length, tensor, that tensor's first chunk and chunk count
 
-__device__ __forceinline__ double block_sum_d(double x, double *red) {   // fixed order; red: kOptThreads / 32 doubles
-    x = warp_sum_d(x);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = x;
-    __syncthreads();
-    double s = 0.0;
-    for (int w = 0; w < kOptThreads / 32; w++) s += red[w];
-    __syncthreads();
-    return s;
-}
-
 // DIAG, GUARD: as clip_adam_kernel, whose global-norm fold, clip coefficient and guard decision this prologue repeats word
 // for word; a rejected step writes neither param, the moments, update, chunk_sums nor diag.
 template <bool DIAG, bool GUARD>
@@ -126,39 +68,12 @@ __global__ void __launch_bounds__(kOptThreads) clip_lamb_moments_kernel(
     float *__restrict__ exp_avg_sq, float *__restrict__ update, const int64_t *__restrict__ plan, double *__restrict__ chunk_sums,
     const float *__restrict__ partials, const int64_t *step_p, double max_norm_d, double beta1_d, double beta2_d, double eps_d,
     double wd_d, float *grad_norm_out, double *diag, const float *__restrict__ tail, int n_tail, int32_t *skip) {
-    const float max_norm = (float)max_norm_d, beta2 = (float)beta2_d, eps = (float)eps_d, wd = (float)wd_d;
+    const float beta2 = (float)beta2_d, eps = (float)eps_d, wd = (float)wd_d;
     __shared__ double red[kOptThreads / 32];
-    __shared__ float s_coef;
-    __shared__ int s_reject;
-    double acc = 0.0;
-    for (int i = threadIdx.x; i < kPartials; i += blockDim.x) acc += (double)partials[i];
-    acc = warp_sum_d(acc);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double s = 0.0;
-        for (int w = 0; w < kOptThreads / 32; w++) s += red[w];
-        float total_norm = (float)sqrt(s);
-        float coef = max_norm / (total_norm + 1e-6f);  // torch clip_grad_norm_
-        s_coef = fminf(coef, 1.0f);
-        if (blockIdx.x == 0 && grad_norm_out) *grad_norm_out = total_norm;
-        bool reject = false;
-        if (GUARD) {
-            reject = !isfinite(s);
-            for (int i = 0; i < n_tail; i++) reject |= !isfinite(tail[i]);
-            s_reject = reject ? 1 : 0;
-            if (blockIdx.x == 0) *skip = reject ? 1 : 0;
-        }
-        if (DIAG && blockIdx.x == 0 && !reject) {
-            diag[0] += (double)total_norm;
-            diag[1] += (double)total_norm * (double)total_norm;
-            diag[2] += total_norm > max_norm ? 1.0 : 0.0;
-            diag[3] += 1.0;
-        }
-    }
-    __syncthreads();
-    if (GUARD && s_reject) return;
-    const float coef = s_coef;
+    float coef;
+    bool reject;
+    clip_prologue<DIAG, GUARD>(partials, (float)max_norm_d, grad_norm_out, diag, tail, n_tail, skip, coef, reject);
+    if (reject) return;
     const int64_t t = *step_p + 1;
     const float bc1 = (float)(1.0 - pow(beta1_d, (double)t));
     const float bc2_sqrt = (float)sqrt(1.0 - pow(beta2_d, (double)t));
@@ -308,6 +223,15 @@ __global__ void bump_step_kernel(int64_t *step_p) { *step_p += 1; }
 // guarded form: a rejected step is not counted
 __global__ void bump_step_guarded_kernel(int64_t *step_p, const int32_t *skip) { *step_p += *skip ? 0 : 1; }
 
+int launch_bump_step(int64_t *step, const int32_t *skip, cudaStream_t stream) {
+    if (skip)
+        bump_step_guarded_kernel<<<1, 1, 0, stream>>>(step, skip);
+    else
+        bump_step_kernel<<<1, 1, 0, stream>>>(step);
+    HRL_CUDA_CHECK(cudaGetLastError());
+    return HRL_OK;
+}
+
 // After a guarded optimiser step.  Accepted: accum[i] += (double)tail[i], i < n_tail (one rounding, as ATen's fp64 add_
 // of an fp32 tensor).  Rejected: *skip_count += 1, and the saved bytes go back to `state` (the buffers the forward moved).
 __global__ void __launch_bounds__(kOptThreads) step_commit_kernel(const int32_t *__restrict__ skip, const float *__restrict__ tail,
@@ -412,12 +336,7 @@ extern "C" int hrl_clip_adam_step(float *param, const float *grad, float *exp_av
     kernel<<<grid, kOptThreads, 0, s>>>(param, grad, exp_avg, exp_avg_sq, n, partials, lr, step, max_norm, beta1, beta2, eps,
                                         weight_decay, grad_norm_out, diag_accum, tail, n_tail, skip);
     HRL_CUDA_CHECK(cudaGetLastError());
-    if (skip)
-        bump_step_guarded_kernel<<<1, 1, 0, s>>>(step, skip);
-    else
-        bump_step_kernel<<<1, 1, 0, s>>>(step);
-    HRL_CUDA_CHECK(cudaGetLastError());
-    return HRL_OK;
+    return launch_bump_step(step, skip, s);
 }
 
 extern "C" int64_t hrl_lamb_plan(const int64_t *numel, int32_t n_tensors, int64_t *plan) {
@@ -465,12 +384,7 @@ extern "C" int hrl_clip_lamb_step(float *param, const float *grad, float *exp_av
     auto apply = skip ? lamb_apply_kernel<true> : lamb_apply_kernel<false>;
     apply<<<n_chunks, kOptThreads, 0, s>>>(param, update, plan, chunk_sums, lr, lr_scale, ratio, skip);
     HRL_CUDA_CHECK(cudaGetLastError());
-    if (skip)
-        bump_step_guarded_kernel<<<1, 1, 0, s>>>(step, skip);
-    else
-        bump_step_kernel<<<1, 1, 0, s>>>(step);
-    HRL_CUDA_CHECK(cudaGetLastError());
-    return HRL_OK;
+    return launch_bump_step(step, skip, s);
 }
 
 extern "C" int hrl_step_commit(const int32_t *skip, const float *tail, int32_t n_tail, double *accum, double *skip_count,

@@ -592,6 +592,75 @@ class FlatLamb(FlatAdam):
         fastnet.new_step()          # cached adjoint weights of the convolutions are stale now
 
 
+MUON_KINDS = ('adam', 'matrix', 'too_large')     # HrlMuonKind
+
+
+def muon_plan(shapes):
+    """hrl_muon_plan on the host for parameters of `shapes` laid out back to back from word 0: (kinds, mats, spans) with
+    kinds[i] in MUON_KINDS -- 'matrix' for a Muon-owned tensor, 'too_large' for a matrix outside the kernel's envelope
+    (Adam-owned), 'adam' for the rest -- mats the (matrices, 4) int64 CPU tensor {first word, r, k, transposed} and spans the
+    (spans, 2) int64 CPU tensor {first word, words} of the Adam-owned words."""
+    shapes = [tuple(int(d) for d in s) for s in shapes]
+    dims = torch.tensor([d for s in shapes for d in s] or [0], dtype=torch.int64)
+    ndim = torch.tensor([len(s) for s in shapes], dtype=torch.int32)
+    kind = torch.zeros(len(shapes), dtype=torch.int32)
+    counts = torch.zeros(2, dtype=torch.int32)
+    check(lib().hrl_muon_plan(_ptr(dims), _ptr(ndim), len(shapes), _ptr(kind), _ptr(counts), None, None))
+    mats = torch.zeros((int(counts[0]), 4), dtype=torch.int64)
+    spans = torch.zeros((int(counts[1]), 2), dtype=torch.int64)
+    check(lib().hrl_muon_plan(_ptr(dims), _ptr(ndim), len(shapes), _ptr(kind), _ptr(counts), _ptr(mats), _ptr(spans)))
+    return [MUON_KINDS[int(k)] for k in kind], mats, spans
+
+
+class FlatMuon(FlatAdam):
+    """clip_grad_norm_(max_norm) + Muon on FlatAdam's bucket (hrl_clip_muon_step): each Muon-owned weight matrix (muon_plan)
+    takes its Nesterov momentum (mu = 0.95, kept in exp_avg; its exp_avg_sq stays zero) orthogonalised by five Newton-Schulz
+    iterations on bf16 tensor-core products, scaled by lr_scale * 0.2 * sqrt(max(r, k)), with decoupled weight decay; every
+    other word takes FlatAdam's update bit for bit.  `names` (optional, one per parameter) name the parameters; `muon_params`
+    lists the names (or indices) of the Muon-owned ones.  `ortho`: None, or a float32 CUDA tensor of n_pad words that every
+    step fills with O at the matrices' words.  Everything else -- buffers, guard, diagnostics, the peer all-reduce path -- is
+    FlatAdam's, and a step takes as many launches as FlatAdam's."""
+
+    def __init__(self, params, lr, lr_scale=1.0, names=None, **kw):
+        params = list(params)
+        super().__init__(params, lr, **kw)
+        device = self.flat_param.device
+        self.lr_scale = float(lr_scale)
+        names = list(range(len(params))) if names is None else list(names)
+        assert len(names) == len(params)
+        self.kinds, mats, spans = muon_plan([tuple(p.shape) for p in params])
+        self.muon_params = [k for k, kind in zip(names, self.kinds) if kind == 'matrix']
+        self.mats, self.spans = mats.to(device), spans.to(device)
+        self.ortho = None
+
+    def step_reduced(self, reduced):
+        """clip + Muon on an already all-reduced bucket whose sum-of-squares partials are in self.partials."""
+        self._clip_muon(reduced, _stream_ptr())
+        _count(2)
+
+    def _clip_muon(self, grad, s):
+        if self.diag is not None:
+            assert self.diag.is_cuda and self.diag.dtype == torch.float64 and self.diag.numel() == 4 and self.diag.is_contiguous()
+        if self.skip is not None:
+            assert self.skip.is_cuda and self.skip.dtype == torch.int32 and self.skip.numel() == 1
+            assert 0 <= self.guard_tail <= self.extra and grad.numel() >= self.n_pad + self.extra
+        if self.ortho is not None:
+            assert self.ortho.is_cuda and self.ortho.dtype == torch.float32 and self.ortho.numel() >= self.n_pad
+        check(lib().hrl_clip_muon_step(
+            _ptr(self.flat_param), _ptr(grad), _ptr(self.exp_avg), _ptr(self.exp_avg_sq), self.n_pad,
+            _ptr(self.mats), self.mats.shape[0], _ptr(self.spans), self.spans.shape[0], _ptr(self.partials), _ptr(self.lr),
+            _ptr(self.step_count), self.max_norm, self.betas[0], self.betas[1], self.eps, self.weight_decay, self.lr_scale,
+            _ptr(self.grad_norm), _ptr(self.diag), _ptr(grad[self.n_pad:]), self.guard_tail, _ptr(self.skip), _ptr(self.ortho), s))
+
+    def step(self):
+        s = _stream_ptr()
+        check(lib().hrl_grad_sumsq(_ptr(self.flat_grad), self.n_pad, _ptr(self.partials), s))
+        self._clip_muon(self.flat_grad, s)
+        _count(3)
+        from . import fastnet
+        fastnet.new_step()          # cached adjoint weights of the convolutions are stale now
+
+
 def _check_skip(skip):
     if not (skip.is_cuda and skip.dtype == torch.int32 and skip.numel() == 1):
         raise _capi.HrlError('handyrl_b200: skip must be a one-element int32 CUDA tensor')

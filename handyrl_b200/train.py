@@ -615,25 +615,27 @@ class ReplayCheckpoints:
 
 
 def optimizer_config(value):
-    """train_args['optimizer'] -> {'name': 'adam'} (key absent, None or 'adam': clip + Adam, ops.FlatAdam) or
-    {'name': 'lamb', 'lr_scale': s} ('lamb', or {'name': 'lamb', 'lr_scale': s} with s a finite number > 0, default 1.0:
-    clip + LAMB, ops.FlatLamb).  Anything else -- another name, another dict key, a bad lr_scale -- raises ValueError."""
+    """train_args['optimizer'] -> {'name': 'adam'} (key absent, None or 'adam': clip + Adam, ops.FlatAdam),
+    {'name': 'lamb', 'lr_scale': s} ('lamb', or {'name': 'lamb', 'lr_scale': s}: clip + LAMB, ops.FlatLamb) or
+    {'name': 'muon', 'lr_scale': s} ('muon', or {'name': 'muon', 'lr_scale': s}: clip + Muon, ops.FlatMuon), with s a finite
+    number > 0, default 1.0.  Anything else -- another name, another dict key, a bad lr_scale -- raises ValueError."""
     if value is None or (isinstance(value, str) and value == 'adam'):
         return {'name': 'adam'}
-    if isinstance(value, str) and value == 'lamb':
-        return {'name': 'lamb', 'lr_scale': 1.0}
+    if isinstance(value, str) and value in ('lamb', 'muon'):
+        return {'name': value, 'lr_scale': 1.0}
     if not isinstance(value, dict):
-        raise ValueError("train_args['optimizer'] must be 'adam', 'lamb' or {'name': 'lamb', 'lr_scale': s}; got %r" % (value,))
+        raise ValueError("train_args['optimizer'] must be 'adam', 'lamb', 'muon' or {'name': 'lamb' or 'muon', 'lr_scale': s}; "
+                         "got %r" % (value,))
     unknown = sorted(str(k) for k in value if k not in ('name', 'lr_scale'))
     if unknown:
         raise ValueError("train_args['optimizer']: unknown key(s) %s (known: name, lr_scale)" % ', '.join(unknown))
-    if value.get('name') != 'lamb':
-        raise ValueError("train_args['optimizer']: the dict form is {'name': 'lamb', 'lr_scale': s}; got name %r"
+    if value.get('name') not in ('lamb', 'muon'):
+        raise ValueError("train_args['optimizer']: the dict form is {'name': 'lamb' or 'muon', 'lr_scale': s}; got name %r"
                          % (value.get('name'),))
     s = value.get('lr_scale', 1.0)
     if isinstance(s, bool) or not isinstance(s, numbers.Real) or not 0.0 < float(s) < float('inf'):
         raise ValueError("train_args['optimizer']: lr_scale must be a finite number > 0; got %r" % (s,))
-    return {'name': 'lamb', 'lr_scale': float(s)}
+    return {'name': value['name'], 'lr_scale': float(s)}
 
 
 def nonfinite_guard(args):
@@ -728,8 +730,11 @@ class OptimizerStateFormat:
     and the data-count average it came from (the device's float32 values), and the step count it was scheduled at.
 
     A LAMB learner (optimizer_config(...)['name'] == 'lamb', `optimizer`) adds two top-level entries, 'algorithm': 'lamb'
-    and 'lr_scale': float; its moments and step mean what Adam's do.  A dict without 'algorithm' is an Adam dict, and an Adam
-    learner writes exactly the entries above.  unpack() refuses a dict of the other algorithm; lr_scale is not compared."""
+    and 'lr_scale': float; its moments and step mean what Adam's do.  A Muon learner adds 'algorithm': 'muon', 'lr_scale' and
+    'muon_params', the names of the parameters Muon owns (ops.muon_plan); their 'exp_avg' is Muon's momentum and their
+    'exp_avg_sq' is zero, and the other parameters' moments are Adam's.  A dict without 'algorithm' is an Adam dict, and an
+    Adam learner writes exactly the entries above.  unpack() refuses a dict of another algorithm, and a Muon dict whose
+    'muon_params' differ from the learner's split; lr_scale is not compared."""
 
     def __init__(self, named_params, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-5, max_norm=4.0, optimizer=None):
         self.names, self.shapes, self.offsets = [], [], []
@@ -744,6 +749,10 @@ class OptimizerStateFormat:
         self.betas = (float(betas[0]), float(betas[1]))
         self.eps, self.weight_decay, self.max_norm = float(eps), float(weight_decay), float(max_norm)
         self.optimizer = optimizer if optimizer is not None else {'name': 'adam'}
+        self.muon_params = None
+        if self.optimizer['name'] == 'muon' and self.names:
+            kinds = ops.muon_plan(self.shapes)[0]
+            self.muon_params = [k for k, kind in zip(self.names, kinds) if kind == 'matrix']
 
     def _spans(self):
         for name, shape, off in zip(self.names, self.shapes, self.offsets):
@@ -768,19 +777,25 @@ class OptimizerStateFormat:
              'max_norm': self.max_norm}
         if self.optimizer['name'] == 'lamb':
             d['algorithm'], d['lr_scale'] = 'lamb', self.optimizer['lr_scale']
+        elif self.optimizer['name'] == 'muon':
+            d['algorithm'], d['lr_scale'], d['muon_params'] = 'muon', self.optimizer['lr_scale'], list(self.muon_params)
         return d
 
     def check_algorithm(self, d):
-        """Raise ValueError when the dict `d` was written by the other optimiser (its 'algorithm' entry, absent: Adam)."""
+        """Raise ValueError when the dict `d` was written by another optimiser (its 'algorithm' entry, absent: Adam), or by a
+        Muon learner whose split into Muon- and Adam-owned parameters ('muon_params') differs from this one's."""
         got, want = d.get('algorithm', 'adam'), self.optimizer['name']
         if got != want:
             raise ValueError('optimiser state: written by %s, the learner runs %s (train_args[\'optimizer\'])' % (got, want))
+        if want == 'muon' and self.muon_params is not None and list(d.get('muon_params', ())) != self.muon_params:
+            raise ValueError('optimiser state: Muon owns %s in the file, %s in the learner'
+                             % (list(d.get('muon_params', ())), self.muon_params))
 
     def unpack(self, d):
         """Check a dict of this format against the net and the optimiser's settings and return its flat form
         (exp_avg, exp_avg_sq: float32 CPU tensors of n_pad words with zero padding; step; lr; data_cnt_ema; steps).
         Raises KeyError (an entry or a parameter name missing or extra) or ValueError (a shape, betas, eps, weight_decay or
-        max_norm that differs, or a dict of the other algorithm: check_algorithm)."""
+        max_norm that differs, or a dict of another algorithm or Muon split: check_algorithm)."""
         self.check_algorithm(d)
         for key in ('optimizer', 'param_names', 'schedule', 'max_norm'):
             if key not in d:
@@ -1012,7 +1027,11 @@ class LearnerStep:
     parameter tensor, the step lr * s * r_i * u) in place of clip + Adam, in step() and in the peer all-reduce path alike: one
     more launch per step.  `self.optimizer` is the parsed setting.  The moments, step count, guard, diagnostics, weight
     average, gradient accumulation and the hand-off are the same; the saved optimiser state carries 'algorithm': 'lamb'
-    (OptimizerStateFormat), and load_optimizer_state() refuses a file of the other algorithm.
+    (OptimizerStateFormat), and load_optimizer_state() refuses a file of the other algorithm.  'muon' or {'name': 'muon',
+    'lr_scale': s} runs clip + Muon (ops.FlatMuon, hrl_clip_muon_step: on each weight matrix the kernel's envelope holds,
+    momentum orthogonalised by Newton-Schulz iterations on bf16 tensor cores, the step lr * s * 0.2 * sqrt(max(r, k)) plus
+    decoupled weight decay; Adam on every other word) with as many launches as Adam; its saved state carries 'algorithm':
+    'muon' and 'muon_params'.
 
     value_bins (default: train_args['value_bins'], off; value_bins.py): categorical value / return heads.  The key is parsed
     here, and a probe call of the net on one observation checks that it outputs every listed head (ValueError otherwise); the
@@ -1114,6 +1133,9 @@ class LearnerStep:
                       grad_alloc=self.peer.alloc if self.peer is not None else None, param_storage=self.state.flat_param)
         if self.optimizer['name'] == 'lamb':
             self.opt = ops.FlatLamb(params, lr_scale=self.optimizer['lr_scale'], **bucket)
+        elif self.optimizer['name'] == 'muon':
+            self.opt = ops.FlatMuon(params, lr_scale=self.optimizer['lr_scale'], names=[k for k, _ in self.model.named_parameters()],
+                                    **bucket)
         else:
             self.opt = ops.FlatAdam(params, **bucket)
         self.state.index_params(self.model)
@@ -2398,7 +2420,8 @@ class Trainer:
     train_args['optimizer'] = 'lamb' or {'name': 'lamb', 'lr_scale': s} (optimizer_config; ValueError for anything but these,
     'adam' and None): every rank's LearnerStep runs clip + LAMB instead of clip + Adam on the same all-reduced bucket, with
     the learning rate of the same schedule times s.  The .optim.pth files carry 'algorithm': 'lamb', and a restart refuses a
-    file the other optimiser wrote.
+    file the other optimiser wrote.  'muon' or {'name': 'muon', 'lr_scale': s} does the same with clip + Muon (LearnerStep);
+    its files carry 'algorithm': 'muon' and 'muon_params'.
 
     train_args['value_bins'] = {'value': {'bins': K, 'low': lo, 'high': hi, 'symlog': bool, 'sigma': s}, 'return': {...}}
     (value_bins.py; ValueError here for a malformed key): the listed heads output K logits and train by cross-entropy against

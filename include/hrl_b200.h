@@ -21,6 +21,9 @@
  *   hrl_lamb_plan /
  *   hrl_clip_lamb_step    <- the same clip + LAMB (Adam with per-tensor trust ratios) in place of Adam; opt-in, no
  *                            reference counterpart
+ *   hrl_muon_plan /
+ *   hrl_clip_muon_step    <- the same clip + Muon (momentum orthogonalised by Newton-Schulz iterations) on the weight
+ *                            matrices, Adam on the other words; opt-in, no reference counterpart
  *   hrl_step_commit       <- with the guard of hrl_clip_adam_step: the same step, rejected on the device when its loss
  *                            or gradient is not finite; no reference counterpart
  *   hrl_weight_ema        <- a per-step moving average of the weights; no reference counterpart (scripts/aux_swa.py
@@ -283,6 +286,45 @@ int hrl_clip_lamb_step(float *param, const float *grad, float *exp_avg, float *e
                        int64_t *step, double max_norm, double beta1, double beta2, double eps, double weight_decay,
                        double lr_scale, float *grad_norm_out /* may be NULL */, double *diag_accum /* may be NULL */,
                        const float *tail, int32_t n_tail, int32_t *skip /* may be NULL */, float *ratio /* may be NULL */,
+                       void *stream);
+
+/*
+ * Muon on the same bucket (opt-in): each weight matrix's Nesterov momentum, orthogonalised by five Newton-Schulz
+ * iterations, replaces Adam's step on that matrix; every other word takes hrl_clip_adam_step's update bit for bit.  A tensor
+ * of shape (r, ...) is viewed as the r x k matrix, k = numel / r.  It is Muon-owned (HRL_MUON_MATRIX) when it has two or
+ * more dimensions, min(r, k) >= 2 and the matrix fits one CTA: with m <= n its sides and m_p, n_p those rounded up to 16,
+ * m_p <= 128 and m_p * n_p <= 128 * 576.  A matrix with min(r, k) >= 2 outside that is HRL_MUON_TOO_LARGE and takes Adam,
+ * as does everything else (HRL_MUON_ADAM).  With c the clip coefficient of hrl_clip_adam_step, lr the device's learning
+ * rate and W, M a Muon-owned matrix and its momentum (the exp_avg words; its exp_avg_sq words are not touched):
+ *     G = c * grad;   M <- 0.95 M + G;   N = G + 0.95 M                       (fp32, each product and sum rounded)
+ *     X = N / (|N|_F + 1e-7) as bf16, transposed when r > k so that X is m x n
+ *     5 times:  A = bf16(X X^T);  B = bf16(b A + c A A);  X = bf16(a X + B X)   (a, b, c) = (3.4445, -4.7750, 2.0315)
+ *     O = X (transposed back);   W <- W - lr (s O + weight_decay W),   s = fp32(lr_scale * 0.2 * sqrt(max(r, k)))
+ * The products take bf16 operands (round to nearest even) and accumulate in fp32 on the tensor cores.
+ *
+ * hrl_muon_plan (host, no device work): tensors t < n_tensors of ndim[t] dimensions dims[...] (the shapes back to back; a
+ * scalar has ndim 0), laid out back to back from word 0.  kind[t] receives its HrlMuonKind and counts[0..1] the numbers of
+ * matrices and of Adam spans.  mats != NULL (4 int64 per matrix) receives {first word, r, k, transposed} per Muon-owned
+ * tensor in bucket order; spans != NULL (2 int64 per span) receives {first word, words}: the Adam-owned words in runs of
+ * adjacent tensors, cut into pieces of at most 4096.  HRL_ERR_BAD_ARG: a NULL pointer, n_tensors <= 0, ndim < 0 or an empty
+ * dimension.
+ *
+ * hrl_clip_muon_step: two launches -- one CTA per matrix and one per Adam span of hrl_muon_plan's tables (copied to the
+ * device), then *step += 1; the same count as hrl_clip_adam_step.  Fixed-order reductions and no atomics: repeated launches,
+ * graph replays and ranks give identical bits.  partials, lr, step, grad_norm_out, diag_accum, tail, n_tail and skip mean
+ * what they mean for hrl_clip_adam_step, and the guard rejects on the same condition: a rejected step writes neither param,
+ * the moments, ortho nor diag_accum, and does not count.  ortho != NULL (n device floats) receives O at each matrix's words.
+ * HRL_ERR_BAD_ARG: a required pointer NULL, n <= 0, an empty plan, tail NULL with n_tail > 0 under the guard, or lr_scale
+ * not finite and > 0.
+ */
+typedef enum { HRL_MUON_ADAM = 0, HRL_MUON_MATRIX = 1, HRL_MUON_TOO_LARGE = 2 } HrlMuonKind;
+int hrl_muon_plan(const int64_t *dims, const int32_t *ndim, int32_t n_tensors, int32_t *kind, int32_t *counts,
+                  int64_t *mats /* may be NULL */, int64_t *spans /* may be NULL */);
+int hrl_clip_muon_step(float *param, const float *grad, float *exp_avg, float *exp_avg_sq, int64_t n, const int64_t *mats,
+                       int32_t n_mats, const int64_t *spans, int32_t n_spans, const float *partials, const float *lr,
+                       int64_t *step, double max_norm, double beta1, double beta2, double eps, double weight_decay,
+                       double lr_scale, float *grad_norm_out /* may be NULL */, double *diag_accum /* may be NULL */,
+                       const float *tail, int32_t n_tail, int32_t *skip /* may be NULL */, float *ortho /* may be NULL */,
                        void *stream);
 
 /*
